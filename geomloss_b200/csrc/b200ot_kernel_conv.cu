@@ -76,7 +76,9 @@ __global__ void conv_bwd_finalize_kernel(const float* __restrict__ part, int n_s
   if (i >= N) return;
   float go = grad_out ? grad_out[i] : 1.f;  // no upstream gradient: the unit row gradient (value + gradient pass)
   float wmax = 1.f;
-  if (w_absmax != nullptr && *w_absmax > 0.f) wmax = *w_absmax;  // tensor-core path: weights were normalised
+  // tensor-core path: the weights were normalised to max|w| = kTcPScale (tc_pack_kernel); all-zero weights leave
+  // all-zero sums
+  if (w_absmax != nullptr && *w_absmax > 0.f) wmax = *w_absmax / kTcPScale;
   go *= wmax;
   if (kind == B200OT_KERNEL_GAUSSIAN) {
     const int na = D + 1;
@@ -232,7 +234,7 @@ bool tc_any_routed(int D, int64_t N, int64_t M) {
 // Tuning of the row-gradient kernels (tcbwd.cuh), $B200OT_TC_BWD = "p_terms,epi,ldall,merge" for A/B timing and the
 // variants' parity tests (the settings string of the C ABI, see b200ot.h):
 //   p_terms  fp16 terms of P in GEMM 2 (PT).  PT = 1 saves a third of the GEMM-2 work but feeds GEMM 2 an 11-bit image
-//            of P whose subnormal flush also reaches the row sums — kept as a knob, not the default.  Measured on an
+//            of P (every weight perturbed by <= 2^-12) — kept as a knob, not the default.  Measured on an
 //            H100 80GB HBM3 (400 W) at N = M = 4e5, gaussian / softmin row gradients, ms: D = 16 119.5 / 111.9 (PT = 2)
 //            against 107.7 / 91.3 (PT = 1); D = 64 260 / 222 against 229 / 196.
 //   merge    hi.[Y_h | Y_l] as one N = 2 dk instruction per K step (1) or two N = dk instructions (0): the same
@@ -273,6 +275,8 @@ static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd = false) {
   p.nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
   p.smem = tc_a_span(p.kp) + p.nstage * p.b_bytes + bar_bytes;
   int64_t want = ceil_div64((int64_t)num_sms() * 4, p.a_tiles);
+  const int forced = forced_splits();  // test hook (plan.cuh)
+  if (forced > 0) want = forced;
   if (want < 1) want = 1;
   if (want > 64) want = 64;
   if (want > p.b_tiles) want = p.b_tiles;
@@ -304,7 +308,7 @@ int bwd_partial_tc(int kind, const float* x, const float* y, const float* w, con
   float* part = reinterpret_cast<float*>(base + p.off_part);
   float* w_absmax = nullptr;
   if (w != nullptr) {
-    // P = w_j e_ij feeds an fp16 GEMM: normalise the weights to max|w| = 1 (undone by the finalize kernel)
+    // P = w_j e_ij feeds an fp16 GEMM: normalise the weights to max|w| = kTcPScale (undone by the finalize kernel)
     w_absmax = reinterpret_cast<float*>(base + p.off_misc);
     B200OT_CUDA_TRY(cudaMemsetAsync(w_absmax, 0, sizeof(float), st));
     absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(M, 256), 1024), 256, 0, st>>>(w, M, w_absmax);

@@ -41,14 +41,23 @@ __global__ void softmin_bwd_finalize_kernel(const float* __restrict__ part, int 
   }
 }
 
-// merged[e] = sum_s part[s * n_elems + e]
+// merged[e] = scale * sum_s part[s * n_elems + e]
 __global__ void rowsum_merge_kernel(const float* __restrict__ part, int n_part, float* __restrict__ merged,
-                                    int64_t n_elems) {
+                                    int64_t n_elems, float scale) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_elems) return;
   float a = 0.f;
   for (int s = 0; s < n_part; ++s) a += part[(int64_t)s * n_elems + e];
-  merged[e] = a;
+  merged[e] = scale * a;
+}
+
+static int rowsum_merge(const float* part, int n_part, int width, float* merged, int64_t N, float scale,
+                        cudaStream_t st) {
+  const int threads = 256;
+  rowsum_merge_kernel<<<(unsigned)ceil_div64(N * width, threads), threads, 0, st>>>(part, n_part, merged, N * width,
+                                                                                    scale);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
 }
 
 template <int MODE, int D>
@@ -93,11 +102,7 @@ extern "C" {
 B200OT_API int b200ot_rowsum_merge(const float* part, int32_t n_part, int32_t width, float* merged, int64_t N,
                                    void* stream) {
   if (!part || !merged || n_part <= 0 || width <= 0 || N <= 0) return B200OT_EINVAL;
-  const int threads = 256;
-  rowsum_merge_kernel<<<(unsigned)ceil_div64(N * width, threads), threads, 0, (cudaStream_t)stream>>>(
-      part, n_part, merged, N * width);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
+  return rowsum_merge(part, n_part, width, merged, N, 1.f, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_partial(const float* x, const float* center, const float* cols, const float* lse2,
@@ -150,17 +155,19 @@ B200OT_API int b200ot_softmin_bwd_finalize(const float* part, int32_t n_part, co
   return B200OT_OK;
 }
 
-// Runs pack + partial reduction of the row-gradient pass and leaves n_part sets of (N, D+1) sums in scratch.
+// Runs pack + partial reduction of the row-gradient pass and leaves n_part sets of (N, D+1) sums in scratch, each
+// `*scale_out` times the softmax-weighted sums (kTcPScale on the tensor-core path, common.cuh; 1 otherwise).
 static int softmin_bwd_partials(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
                                 const float* center, const float* lse2, int64_t N, int64_t M, int32_t D, int32_t p,
                                 float eps, void* scratch, int64_t scratch_bytes, void* stream, float** part_out,
-                                int* n_part_out) {
+                                int* n_part_out, float* scale_out) {
   const bool tc = p_exponent(p) == 2 && tc_routed(kTcSoftminBwd, D, N, M);
   if (!x || !y || !h_a || !lse2 || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) || !valid_p(p) ||
       !(eps > 0.f))
     return B200OT_EINVAL;
   if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
   if (scratch_bytes < b200ot_softmin_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
+  *scale_out = tc ? kTcPScale : 1.f;
   if (tc)
     return bwd_partial_tc(1, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M, D,
                           scratch, part_out, n_part_out, (cudaStream_t)stream, nullptr);
@@ -183,10 +190,12 @@ B200OT_API int b200ot_softmin_bwd_sums(const float* x, const float* y, const flo
   if (!sums) return B200OT_EINVAL;
   float* part = nullptr;
   int n_part = 0;
+  float p_scale = 1.f;
   const int rc = softmin_bwd_partials(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch,
-                                      scratch_bytes, stream, &part, &n_part);
+                                      scratch_bytes, stream, &part, &n_part, &p_scale);
   if (rc) return rc;
-  return b200ot_rowsum_merge(part, n_part, D + 1, sums, N, stream);
+  // raw sums leave the library (the multi-GPU engine adds them over the column shards): undo the P scale here
+  return rowsum_merge(part, n_part, D + 1, sums, N, 1.f / p_scale, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -196,8 +205,9 @@ B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float*
   if (!grad_out || !grad_x) return B200OT_EINVAL;
   float* part = nullptr;
   int n_part = 0;
+  float p_scale = 1.f;  // cancels: the finalize divides by the row sum of P
   const int rc = softmin_bwd_partials(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch,
-                                      scratch_bytes, stream, &part, &n_part);
+                                      scratch_bytes, stream, &part, &n_part, &p_scale);
   if (rc) return rc;
   return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
 }

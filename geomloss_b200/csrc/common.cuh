@@ -16,6 +16,12 @@ constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 // "minus infinity" that stays finite under (a - b): used to initialise running maxima.
 constexpr float kNegBig = -1.0e30f;
+// The tensor-core row gradients (tcbwd.cuh) feed 2^kTcPLog2 * P to their fp16 GEMM instead of P <= 1: the weights of
+// a softmax over M columns are ~1/M, below fp16's normal range (6.1e-5) once M >~ 16k, where the fixed 6e-8 subnormal
+// grid would round them with a bias.  2^14 P < 65504 (fp16's maximum) holds for P < 4.  Undone before any sum leaves
+// the library: conv_bwd_finalize_kernel and b200ot_softmin_bwd_sums (softmin_bwd_finalize divides it out).
+constexpr int kTcPLog2 = 14;
+constexpr float kTcPScale = 16384.f;  // 2^kTcPLog2
 
 // ---------------------------------------------------------------------------------------------
 // Packed column layout ("colpack"), produced by pack_cols_kernel and consumed by every

@@ -36,6 +36,15 @@ struct ReducePlan {
 // consumers visit whole chunks: 32 columns = 16 column pairs, the longest chunk of any dense instantiation
 constexpr int kTailAlign = 32;
 
+// Test hook ($B200OT_FORCE_SPLITS, tools/sanitize_smoke.py and the streaming tests): force the number of column splits of
+// both the dense plan below and the tensor-core plan (make_tc_plan), e.g. 1 so that one CTA streams every column tile
+// of a small problem and re-uses each stage of its ring many times.  Read on every call, like $B200OT_TC_MIN_D; the
+// scratch query and the launch call the same plan function, so they stay consistent.  0 / unset: the default plan.
+inline int forced_splits() {
+  const char* e = getenv("B200OT_FORCE_SPLITS");
+  return e ? atoi(e) : 0;
+}
+
 inline ReducePlan make_plan(int64_t N, int64_t M, int D = 3) {
   (void)D;
   ReducePlan p;
@@ -51,12 +60,7 @@ inline ReducePlan make_plan(int64_t N, int64_t M, int D = 3) {
   p.row_tiles = ceil_div64(N, p.rows_cta);
   const int64_t target_ctas = (int64_t)num_sms() * 2 * kPlanWaves;
   int64_t want = ceil_div64(target_ctas, p.row_tiles);
-  // test hook (tools/sanitize_smoke.py): force the number of column splits, e.g. 1 to make a small problem re-use
-  // the stages of its TMA ring many times under compute-sanitizer
-  static const int forced = [] {
-    const char* e = getenv("B200OT_FORCE_SPLITS");
-    return e ? atoi(e) : 0;
-  }();
+  const int forced = forced_splits();
   if (forced > 0) want = forced;
   if (want < 1) want = 1;
   if (want > 64) want = 64;

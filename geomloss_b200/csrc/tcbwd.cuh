@@ -14,9 +14,13 @@
 //
 // * The accumulator of GEMM 1 (64 x 128 per warpgroup) has, two 8-column blocks at a time, the shape of the f16 A
 //   fragment of a k16 MMA step: P is packed to fp16 in the registers it was computed in and fed to GEMM 2 directly.
-// * P = hi + lo (2 fp16 terms; |P| <= 1: softmax weights, or kernel values times weights normalised to
-//   max|w| = 1 by the pack kernel), Y = h + l (the image's two terms): G = hi.h + hi.l + lo.h, error
-//   ~2^-22 |P||Y| (+ 6e-8 absolute where P falls into fp16's subnormal range).
+// * P = hi + lo (2 fp16 terms), Y = h + l (the image's two terms): G = hi.h + hi.l + lo.h, error ~2^-22 |P||Y|.
+//   P is the weight times kTcPScale = 2^14 (common.cuh): softmax weights with +14 folded into the exponent through
+//   the row image's rank-one chunk (r = -|X|^2/2 - lse2 + 14), or kernel values times weights normalised to
+//   max|w| = 2^14 by the pack kernel; so P <= 2^14 (< 65504 while the true weight is < 4), and a weight stays in
+//   fp16's normal range down to 2^-28 instead of 2^-14.  Unscaled, the ~1/M weights of a softmax over M >~ 16k
+//   columns would sit on the fixed 6e-8 subnormal grid: a bias, not noise, when points repeat.  The finalize kernels
+//   undo the scale (softmin: it cancels in sum P Y / sum P).
 // * The column image of tcconv.cuh ([kgroup][column][8 halves], K-major for GEMM 1) is, read with k = column,
 //   exactly the canonical MN-major no-swizzle layout (core matrix = 8 columns x 16 B of one 8-dim group), so
 //   GEMM 2 needs no second copy of Y: only a descriptor read MN-major, LBO = 128 B (next 8 columns),
@@ -49,8 +53,9 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t d
   if constexpr (N == 128) wgmma_rs_n128(d, a, db);
 }
 
-// MODE 2: gaussian row gradient (P = w_j 2^S), MODE 3: softmin row gradient (P = 2^(S - lse2_i): lse2 rides in the
-// row operand's rank-one chunk).  part[(split*N + row)*(D+1) + {0, 1+k}] = sum_j P_ij {1, Y_jk}
+// MODE 2: gaussian row gradient (P = w_j 2^S, w scaled to max|w| = 2^14), MODE 3: softmin row gradient
+// (P = 2^(S - lse2_i + 14): lse2 - 14 rides in the row operand's rank-one chunk).
+// part[(split*N + row)*(D+1) + {0, 1+k}] = sum_j P_ij {1, Y_jk}
 // DK = the padded dimension tc_dk(D) (N of GEMM 2 is a compile-time constant).
 // MERGE: hi.Y_h and hi.Y_l as one N = 2 DK instruction per K step, or as two N = DK instructions into G_a and G_b.
 //

@@ -92,7 +92,8 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
   // rank-one chunk (16 wide): rows [1,1,1, r_h,r_m,r_l, 0..]   columns [c_h,c_m,c_l, 1,1,1, 0..]
   {
     float r = live ? -0.5f * sq : 0.f;
-    if (!is_cols && row_extra != nullptr && live) r -= row_extra[p];  // softmin backward: exponent - lse2_i
+    // softmin backward: exponent - lse2_i + kTcPLog2 (P = 2^14 softmax weight, common.cuh)
+    if (!is_cols && row_extra != nullptr && live) r -= row_extra[p] - (float)kTcPLog2;
     if (is_cols && h_a != nullptr) {
       if (live) {
         float h = h_a[p];
@@ -124,9 +125,10 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
     *reinterpret_cast<uint4*>(img + ((int64_t)(chunk + 1) * tile + pt) * 16) = make_uint4(0u, 0u, 0u, 0u);
   }
   if (is_cols) {
-    // (row-gradient kernels feed P = w e to an fp16 GEMM: weights are normalised to |w| <= 1, undone in the finalize)
+    // (row-gradient kernels feed P = w e to an fp16 GEMM: weights are normalised to |w| <= kTcPScale = 2^14, which
+    // keeps P out of fp16's subnormal range; undone in the finalize)
     float wv = (live && w) ? w[p] : 0.f;
-    if (w_absmax != nullptr && *w_absmax > 0.f) wv /= *w_absmax;
+    if (w_absmax != nullptr && *w_absmax > 0.f) wv = (wv / *w_absmax) * kTcPScale;
     reinterpret_cast<float*>(img + (int64_t)tile * kp * 2)[pt] = wv;
   }
 }

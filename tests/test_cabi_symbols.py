@@ -113,6 +113,33 @@ def test_routing_below_nine_dimensions_shows_in_the_scratch_size(L, monkeypatch)
     assert L.b200ot_softmin_scratch_bytes(n, n, 16) > 0 and L.b200ot_softmin_scratch_bytes(n, n, 65) == 0
 
 
+def test_forced_column_splits_reach_both_plans(L, monkeypatch):
+    """$B200OT_FORCE_SPLITS (csrc/plan.cuh) is read on every call and sets the column splits of the tensor-core plan
+    (make_tc_plan) as well as the dense one, so that the streaming tests (test_gpu_tc_streaming.py) really stream
+    many column tiles through one CTA.  It shows in the scratch size: the row-gradient partials take
+    n_split * N * (D+1) * 4 bytes, the larger need of the shape.  Splits cover ceil(13 / ceil(13 / k)) tiles each."""
+    n, m, d = 256, 128 * 13 - 37, 64  # 2 row tiles, 13 column tiles; N (D+1) 4 is a multiple of the 256-byte grain
+    per_split = n * (d + 1) * 4
+    monkeypatch.delenv("B200OT_FORCE_SPLITS", raising=False)
+    default = (L.b200ot_softmin_scratch_bytes(n, m, d), L.b200ot_kernel_conv_scratch_bytes(n, m, d))
+    sizes = {}
+    for k in (1, 2, 3, 13, 99):
+        monkeypatch.setenv("B200OT_FORCE_SPLITS", str(k))
+        sizes[k] = (L.b200ot_softmin_scratch_bytes(n, m, d), L.b200ot_kernel_conv_scratch_bytes(n, m, d))
+    for k, n_split in ((2, 2), (3, 3), (13, 13), (99, 13)):  # 7+6, 5+5+3, one tile each, never more than the tiles
+        assert sizes[k][0] - sizes[1][0] == (n_split - 1) * per_split, (k, sizes)
+        assert sizes[k][1] - sizes[1][1] == (n_split - 1) * per_split, (k, sizes)
+    # default: ceil(4 SMs / 2 row tiles) splits, capped at one per column tile
+    assert default == sizes[13]
+    # the dense plan of the CUDA-core kernels follows the same variable, re-read on every call
+    ntiles = -(-10**5 // 1024)
+    for k in (1, 5, 7):
+        monkeypatch.setenv("B200OT_FORCE_SPLITS", str(k))
+        assert L.b200ot_softmin_num_splits(10**5, 10**5, 3) == -(-ntiles // -(-ntiles // k))
+    monkeypatch.delenv("B200OT_FORCE_SPLITS")
+    assert L.b200ot_softmin_scratch_bytes(n, m, d) == default[0]
+
+
 def test_one_pass_value_and_gradient_entry_validates_its_arguments(L):
     null, fake = ctypes.c_void_p(None), ctypes.c_void_p(0x1000)
     args = (10, 10, 3)

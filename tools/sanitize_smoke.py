@@ -2,6 +2,7 @@
 
     compute-sanitizer --tool memcheck  python tools/sanitize_smoke.py
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
+    B200OT_FORCE_SPLITS=1 compute-sanitizer --tool racecheck python tools/sanitize_smoke.py ring tc
 
 Shapes are the smallest that select each code path (big / small tile shapes, ranges mode, tensor-core kernels, 2-D and
 3-D grid passes with both tile widths); results are checked against torch so a silent corruption also fails."""
@@ -43,6 +44,25 @@ if "ring" in which:
     w = torch.rand(40000, generator=g)
     conv = ops.kernel_conv("laplacian", xg, y.to(DEV), w.to(DEV), 0.3)
     assert torch.isfinite(conv).all()
+    # the four tensor-core kernels with one split: 32 column tiles of 128 pass through the 4-slot ring of every CTA
+    # (tc_reduce_kernel<1>, tc_bwd_kernel<3>, tc_reduce_kernel<0>, tc_bwd_kernel<2>)
+    for d in (16, 64):
+        x, y = torch.rand(700, d, generator=g), torch.rand(4000, d, generator=g)
+        h, w = torch.randn(4000, generator=g), torch.rand(4000, generator=g)
+        xd, yd, hd, wd = x.to(DEV), y.to(DEV), h.to(DEV), w.to(DEV)
+        center, ones = ops.default_center(xd, yd), torch.ones(700, device=DEV)
+        d2 = ((x[:, None, :].double() - y[None, :, :].double()) ** 2).sum(-1)
+        out, lse2 = ops.softmin_raw(1.0, xd, yd, hd, p=2, center=center, want_lse2=True)
+        check(f"ring_tc_softmin_d{d}", out, ref_softmin(1.0, x, y, h, 2), 1e-4)
+        gx = ops.softmin_grad_rows(1.0, xd, yd, hd, None, 0.0, lse2, ones, p=2, center=center)
+        prob = torch.softmax(h.double()[None, :] - d2 / 2.0, dim=1)
+        check(f"ring_tc_softmin_grad_d{d}", gx, x.double() - prob @ y.double(), 1e-4)
+        K = (-d2 / 8.0).exp()  # blur = 2
+        conv = ops.kernel_conv_raw("gaussian", xd, yd, wd, 2.0, center=center)
+        check(f"ring_tc_conv_d{d}", conv, K @ w.double(), 1e-4)
+        gc = ops.kernel_conv_grad_rows("gaussian", xd, yd, wd, 2.0, ones, center=center)
+        Kw = K * w.double()[None, :]
+        check(f"ring_tc_conv_grad_d{d}", gc, (Kw @ y.double() - Kw.sum(1, keepdim=True) * x.double()) / 4.0, 1e-4)
 if "softmin" in which:
     for tag, n, m, d, p in (("big", 4200, 4300, 3, 2), ("small", 300, 500, 2, 1), ("big_p1", 4100, 4100, 1, 1),
                             ("d8", 600, 700, 8, 2)):
