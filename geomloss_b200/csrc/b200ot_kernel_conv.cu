@@ -56,24 +56,31 @@ static ConvScales conv_scales(int kind_flags, float blur) {
   return c;
 }
 
+// coord_absmax (tensor-core energy kernel): the sums are in coordinates scaled by tc_energy_coord_scale, undone here
 __global__ void conv_fwd_finalize_kernel(const float* __restrict__ part, int n_split, float sign,
-                                         float* __restrict__ out, int64_t N) {
+                                         float* __restrict__ out, int64_t N,
+                                         const float* __restrict__ coord_absmax = nullptr) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   float a = 0.f;
   for (int s = 0; s < n_split; ++s) a += part[(int64_t)s * N + i];
+  if (coord_absmax != nullptr) a /= tc_energy_coord_scale(*coord_absmax);  // a power of two: exact
   out[i] = sign * a;
 }
 
 // gaussian: part (n_split, N, D+1): [0] = sum W e, [1+k] = sum W e Y_k   -> go (accY - X acc0) / (scale blur^2)
 // laplacian / energy: part (n_split, N, D): sum W e u_k                    -> -go acc / blur   (energy: -go acc)
+// (the tensor-core laplacian / energy sums have the gaussian's layout and are finalized as kind 0; coord_absmax: the
+// energy kernel's coordinate scale, applied to X as the kernel applied it to the clouds)
 __global__ void conv_bwd_finalize_kernel(const float* __restrict__ part, int n_split, const float* __restrict__ x,
                                          const float* __restrict__ center, const float* __restrict__ grad_out,
                                          float* __restrict__ grad_x, int64_t N, int D, int kind, float scale,
                                          float coef, const float* __restrict__ w_absmax,
-                                         float* __restrict__ value_out = nullptr) {
+                                         float* __restrict__ value_out = nullptr,
+                                         const float* __restrict__ coord_absmax = nullptr) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
+  if (coord_absmax != nullptr) scale *= tc_energy_coord_scale(*coord_absmax);
   float go = grad_out ? grad_out[i] : 1.f;  // no upstream gradient: the unit row gradient (value + gradient pass)
   float wmax = 1.f;
   // tensor-core path: the weights were normalised to max|w| = kTcPScale (tc_pack_kernel); all-zero weights leave
@@ -106,6 +113,20 @@ __global__ void absmax_kernel(const float* __restrict__ w, int64_t n, float* __r
   float m = 0.f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     m = fmaxf(m, fabsf(w[i]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m > 0.f && !(m != m)) atomicMax(reinterpret_cast<unsigned int*>(out), __float_as_uint(m));
+}
+
+// max_k |pts[i, k] - center[k]| over the rows of a (na x D) and b (nb x D) into *out (zero-initialised by the caller)
+__global__ void coord_absmax_kernel(const float* __restrict__ a, int64_t na, const float* __restrict__ b, int64_t nb,
+                                    int D, const float* __restrict__ center, float* __restrict__ out) {
+  float m = 0.f;
+  const int64_t ta = na * D, tot = ta + nb * D;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < tot; e += (int64_t)gridDim.x * blockDim.x) {
+    const float v = e < ta ? a[e] : b[e - ta];
+    m = fmaxf(m, fabsf(v - (center ? center[e % D] : 0.f)));
+  }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > 0.f && !(m != m)) atomicMax(reinterpret_cast<unsigned int*>(out), __float_as_uint(m));
@@ -178,7 +199,7 @@ static float conv_bwd_coef(int kind_flags, const ConvScales& cs, float blur) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// tensor-core path (gaussian, 8 < D <= 64): see tcconv.cuh
+// tensor-core path (gaussian, and laplacian / energy for 8 < D <= 64): see tcconv.cuh
 // ---------------------------------------------------------------------------------------------------
 struct TcPlan {
   int kp, nstage, n_split, tiles_per_split;
@@ -295,11 +316,13 @@ int64_t tc_scratch_bytes(int64_t N, int64_t M, int D) {
   return std::max(make_tc_plan(N, M, D, false).total, make_tc_plan(N, M, D, true).total);
 }
 
-// Row gradients on the tensor-core path (gaussian conv: kind 0 / softmin p=2: kind 1).  Leaves n_part sets of
-// (N, D+1) partial sums in *part_out.
-int bwd_partial_tc(int kind, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
+// Row gradients on the tensor-core path; `mode` is the MODE of tc_bwd_kernel (2 gaussian conv, 3 softmin p = 2,
+// 4 laplacian, 5 energy; clampq and coord_absmax: see there).  Leaves n_part sets of (N, D+1) partial sums in
+// *part_out.
+int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
-                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out) {
+                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out,
+                   float clampq, const float* coord_absmax) {
   const TcPlan p = make_tc_plan(N, M, D, true);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
@@ -317,17 +340,18 @@ int bwd_partial_tc(int kind, const float* x, const float* y, const float* w, con
   if (w_absmax_out) *w_absmax_out = w_absmax;
   const int threads = 128;
   tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, lse2);
+      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, lse2, nullptr, coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
   tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, w, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, w_absmax);
+      y, w, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, w_absmax,
+      coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
-  const int self_mode = (kind == 0 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
+  const int self_mode = (mode != 3 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
   auto launch = [&](auto kern) -> int {
     B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
     kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, (int)p.b_tiles, p.tiles_per_split,
-                                                   p.nstage, D, self_mode);
+                                                   p.nstage, D, self_mode, clampq, coord_absmax);
     B200OT_CUDA_TRY(cudaGetLastError());
     return B200OT_OK;
   };
@@ -350,7 +374,15 @@ int bwd_partial_tc(int kind, const float* x, const float* y, const float* w, con
       return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::true_type{}) : pick_dk(mode_tag, T2{}, std::true_type{});
     return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::false_type{}) : pick_dk(mode_tag, T2{}, std::false_type{});
   };
-  const int rc = (kind == 0) ? pick(std::integral_constant<int, 2>{}) : pick(std::integral_constant<int, 3>{});
+  // (the laplacian and energy row gradients have the default variant only: PT = 2, MERGE)
+  using T2 = std::integral_constant<int, 2>;
+  int rc;
+  switch (mode) {
+    case 2: rc = pick(std::integral_constant<int, 2>{}); break;
+    case 3: rc = pick(std::integral_constant<int, 3>{}); break;
+    case 4: rc = pick_dk(std::integral_constant<int, 4>{}, T2{}, std::true_type{}); break;
+    default: rc = pick_dk(std::integral_constant<int, 5>{}, T2{}, std::true_type{}); break;
+  }
   if (rc) return rc;
   *part_out = part;
   *n_part_out = p.n_split;  // G of a CTA is complete over its column split (both column halves feed one GEMM)
@@ -380,15 +412,29 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
   kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, (int)p.b_tiles,
-                                                        p.tiles_per_split, p.nstage, D, 0);
+                                                        p.tiles_per_split, p.nstage, D, 0, 0.f, nullptr);
   B200OT_CUDA_TRY(cudaGetLastError());
   *part_out = part;
   *n_part_out = p.n_split * kTcParts;
   return B200OT_OK;
 }
 
-static int conv_fwd_tc(const float* x, const float* y, const float* w, const float* center, float* out, int64_t N,
-                       int64_t M, int D, float blur, void* scratch, cudaStream_t st) {
+// Energy on the tensor cores: the largest centred coordinate of both clouds, from which every kernel of the pass
+// derives the same power-of-two coordinate scale (tc_energy_coord_scale).  Kept in the scratch's misc block, [1].
+static int energy_coord_absmax(const float* x, int64_t N, const float* y, int64_t M, int D, const float* center,
+                               unsigned char* misc, cudaStream_t st, const float** out) {
+  float* a = reinterpret_cast<float*>(misc) + 1;
+  B200OT_CUDA_TRY(cudaMemsetAsync(a, 0, sizeof(float), st));
+  coord_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((N + M) * D, 256), 1024), 256, 0, st>>>(x, N, y, M, D,
+                                                                                                       center, a);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  *out = a;
+  return B200OT_OK;
+}
+
+static int conv_fwd_tc(int kind_flags, const float* x, const float* y, const float* w, const float* center, float* out,
+                       int64_t N, int64_t M, int D, float blur, void* scratch, cudaStream_t st) {
+  const int kind = kind_base(kind_flags);
   const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
   const TcPlan p = make_tc_plan(N, M, D);
   if (p.nstage < 1) return B200OT_EINVAL;
@@ -396,21 +442,32 @@ static int conv_fwd_tc(const float* x, const float* y, const float* w, const flo
   unsigned char* a_imgs = base;
   unsigned char* b_imgs = base + p.off_b;
   float* part = reinterpret_cast<float*>(base + p.off_part);
-  const float scale = sqrtf(kLog2e) / blur;
+  // gaussian: 2^(-|X-Y|^2/2) with X = x sqrt(log2e) / blur; laplacian / energy: conv_scales' coordinates and clamp
+  const ConvScales cs = conv_scales(kind_flags, blur);
+  const float scale = kind == B200OT_KERNEL_GAUSSIAN ? sqrtf(kLog2e) / blur : cs.scale;
+  const float* coord_absmax = nullptr;
+  if (kind == B200OT_KERNEL_ENERGY) {
+    const int rc = energy_coord_absmax(x, N, y, M, D, center, base + p.off_misc, st, &coord_absmax);
+    if (rc) return rc;
+  }
   const int threads = 128;
   tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs);
+      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, nullptr, nullptr,
+      coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
   tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, w, nullptr, nullptr, 0.f, 0.f, center, scale, M, D, p.kp, kTcBN, 1, b_imgs);
+      y, w, nullptr, nullptr, 0.f, 0.f, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr, coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
-  auto kern = tc_reduce_kernel<0>;
+  auto kern = kind == B200OT_KERNEL_GAUSSIAN ? tc_reduce_kernel<0>
+              : kind == B200OT_KERNEL_LAPLACIAN ? tc_reduce_kernel<4> : tc_reduce_kernel<5>;
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
   kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, (int)p.b_tiles,
-                                                        p.tiles_per_split, p.nstage, D, self_mode);
+                                                        p.tiles_per_split, p.nstage, D, self_mode, cs.clampq,
+                                                        coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
-  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(part, p.n_split * kTcParts, 1.f, out, N);
+  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
+      part, p.n_split * kTcParts, kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, N, coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
@@ -488,13 +545,15 @@ B200OT_API int b200ot_kernel_conv_partial_ranges(const float* x, const float* ce
 B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
                                       float* out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
                                       void* scratch, int64_t scratch_bytes, void* stream) {
-  const bool tc = (kind_base(kind) == B200OT_KERNEL_GAUSSIAN) && tc_routed(kTcConvFwd, D, N, M);
+  // laplacian / energy: the tensor cores serve 8 < D <= 64 only (no measured cross-over below)
+  const bool tc = (kind_base(kind) == B200OT_KERNEL_GAUSSIAN) ? tc_routed(kTcConvFwd, D, N, M)
+                                                              : (D > B200OT_MAX_D && tc_capable_dim(D));
   if (!x || !y || !w || !out || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) || !valid_kind(kind))
     return B200OT_EINVAL;
   if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
   if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
   if (scratch_bytes < b200ot_kernel_conv_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
-  if (tc) return conv_fwd_tc(x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream);
+  if (tc) return conv_fwd_tc(kind, x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -513,20 +572,47 @@ static int conv_bwd_x_impl(const float* x, const float* y, const float* w, const
                            float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
                            void* scratch, int64_t scratch_bytes, void* stream) {
   const bool gauss = kind_base(kind) == B200OT_KERNEL_GAUSSIAN;
-  const bool tc = gauss && tc_routed(kTcConvBwd, D, N, M);
+  const bool tc = gauss ? tc_routed(kTcConvBwd, D, N, M) : (D > B200OT_MAX_D && tc_capable_dim(D));
   if (!x || !y || !w || !grad_x || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) ||
       !valid_kind(kind) || (value_out && !gauss))
     return B200OT_EINVAL;
   if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
   if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
   if (scratch_bytes < b200ot_kernel_conv_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
+  if (tc && !gauss) {
+    // grad = coef (sum_j P Y_j - X_i sum_j P) with P = w k'(d) / d scaled by 2^-kTcNormPLog2 (tcbwd.cuh): the
+    // gaussian's finalize with coef = 2^kTcNormPLog2 / blur (laplacian, X = x log2e / blur) or 2^kTcNormPLog2 (energy)
+    const int kb = kind_base(kind);
+    const ConvScales cs = conv_scales(kind, blur);
+    cudaStream_t st = (cudaStream_t)stream;
+    const float* coord_absmax = nullptr;
+    if (kb == B200OT_KERNEL_ENERGY) {
+      const TcPlan p = make_tc_plan(N, M, D, true);
+      const int rc = energy_coord_absmax(x, N, y, M, D, center, reinterpret_cast<unsigned char*>(scratch) + p.off_misc,
+                                         st, &coord_absmax);
+      if (rc) return rc;
+    }
+    float* tc_part = nullptr;
+    int n_part = 0;
+    const float* w_absmax = nullptr;
+    const int rc = bwd_partial_tc(kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5, x, y, w, nullptr, nullptr, 0.f, nullptr,
+                                  center, cs.scale, N, M, D, scratch, &tc_part, &n_part, st, &w_absmax, cs.clampq,
+                                  coord_absmax);
+    if (rc) return rc;
+    const float coef = (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
+    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
+        tc_part, n_part, x, center, grad_out, grad_x, N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax, nullptr,
+        coord_absmax);
+    B200OT_CUDA_TRY(cudaGetLastError());
+    return B200OT_OK;
+  }
   if (tc) {
     float* tc_part = nullptr;
     int n_part = 0;
     const float scale = sqrtf(kLog2e) / blur;
     const float* w_absmax = nullptr;
-    const int rc = bwd_partial_tc(0, x, y, w, nullptr, nullptr, 0.f, nullptr, center, scale, N, M, D, scratch,
-                                  &tc_part, &n_part, (cudaStream_t)stream, &w_absmax);
+    const int rc = bwd_partial_tc(2, x, y, w, nullptr, nullptr, 0.f, nullptr, center, scale, N, M, D, scratch,
+                                  &tc_part, &n_part, (cudaStream_t)stream, &w_absmax, 0.f, nullptr);
     if (rc) return rc;
     conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, (cudaStream_t)stream>>>(
         tc_part, n_part, x, center, grad_out, grad_x, N, D, 0, scale, 1.0f / (scale * blur * blur), w_absmax,

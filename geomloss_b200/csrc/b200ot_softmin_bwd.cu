@@ -169,7 +169,7 @@ static int softmin_bwd_partials(const float* x, const float* y, const float* h_a
   if (scratch_bytes < b200ot_softmin_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
   *scale_out = tc ? kTcPScale : 1.f;
   if (tc)
-    return bwd_partial_tc(1, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M, D,
+    return bwd_partial_tc(3, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M, D,
                           scratch, part_out, n_part_out, (cudaStream_t)stream, nullptr);
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);

@@ -55,6 +55,9 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t d
 
 // MODE 2: gaussian row gradient (P = w_j 2^S, w scaled to max|w| = 2^14), MODE 3: softmin row gradient
 // (P = 2^(S - lse2_i + 14): lse2 - 14 rides in the row operand's rank-one chunk).
+// MODE 4 / 5: laplacian / energy row gradient, P = w_j 2^-kTcNormPLog2 k'(d) / d with k' = 2^-d (laplacian) or 1
+// (energy), and P = 0 for a pair below its row's coincidence bound (tcconv.cuh; `clampq` and `coord_absmax` are read
+// by these modes only).  The gradient is then coef (sum_j P_ij Y_j - X_i sum_j P_ij): the finalize of the gaussian.
 // part[(split*N + row)*(D+1) + {0, 1+k}] = sum_j P_ij {1, Y_jk}
 // DK = the padded dimension tc_dk(D) (N of GEMM 2 is a compile-time constant).
 // MERGE: hi.Y_h and hi.Y_l as one N = 2 DK instruction per K step, or as two N = DK instructions into G_a and G_b.
@@ -67,11 +70,22 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t d
 //
 // self_mode: rows and columns are the same cloud (the K_xx term): the exponent of pair (i, i) is exactly 0, as in
 // tc_reduce_kernel — matters when sum_j P_ij is used as the forward VALUE (b200ot_kernel_conv_fwd_bwd_x).
+// MODE 4 / 5: P of one pair from its exponent s (the rsqrt of a pair below the bound t is discarded by the select)
+template <int MODE>
+__device__ __forceinline__ float tc_norm_p(float s, float t, float w) {
+  const float q = -2.f * s;
+  const float r = rsqrt_approx(q);
+  float p = w * r;
+  if constexpr (MODE == 4) p *= ex2_approx(-(q * r));
+  return q < t ? 0.f : p;
+}
+
 template <int MODE, int PT, bool MERGE, int DK>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_bwd_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                   float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE, int D,
-                  int self_mode) {
+                  int self_mode, float clampq, const float* __restrict__ coord_absmax) {
+  static_assert(MODE == 2 || MODE == 3 || MODE == 4 || MODE == 5, "row-gradient modes");
   static_assert(PT == 1 || PT == 2, "P is fed to GEMM 2 as one or two fp16 terms");
   static_assert(DK % 16 == 0 && DK <= 64, "padded dimension");
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -124,6 +138,13 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   for (int i = 0; i < DK; ++i) g[i] = 0.f;
   float sum[2] = {0.f, 0.f};
   mbar_wait(bar_a, 0);
+  float tb[2] = {0.f, 0.f};  // MODE 4 / 5: coincidence bound of each row
+  if constexpr (MODE >= 4) {
+    clampq = tc_norm_clampq(clampq, coord_absmax);
+    const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    tb[0] = tc_norm_row_bound(sa, kp, lr, clampq);
+    tb[1] = tc_norm_row_bound(sa, kp, lr + 8, clampq);
+  }
   for (int k = 0; k < nt; ++k) {
     const int st = k % NSTAGE;
     mbar_wait(&full_b[st], (k / NSTAGE) & 1);
@@ -133,7 +154,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     tc_exponent_gemm(s, a_addr, b_addr, DK / 8);
     wgmma_wait<0>();
     reg_fence(s);
-    if constexpr (MODE == 2) {
+    if constexpr (MODE != 3) {
       if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(t0 + k) * kTcBN, cq);
     }
     // ---- S -> P, packed as the A fragments of GEMM 2 (ph[2 n8 + h] = the pair of row h in 8-column block n8) ----
@@ -143,10 +164,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 #pragma unroll
     for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
       float2 w = make_float2(1.f, 1.f);
-      if constexpr (MODE == 2) w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
+      if constexpr (MODE != 3) w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
+      if constexpr (MODE >= 4) {
+        w.x *= 1.f / (float)(1 << kTcNormPLog2);
+        w.y *= 1.f / (float)(1 << kTcNormPLog2);
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float p0 = ex2_approx(s[4 * n8 + 2 * h]), p1 = ex2_approx(s[4 * n8 + 2 * h + 1]);
+        float p0, p1;
+        if constexpr (MODE >= 4) {
+          p0 = tc_norm_p<MODE>(s[4 * n8 + 2 * h], tb[h], w.x);
+          p1 = tc_norm_p<MODE>(s[4 * n8 + 2 * h + 1], tb[h], w.y);
+        } else {
+          p0 = ex2_approx(s[4 * n8 + 2 * h]);
+          p1 = ex2_approx(s[4 * n8 + 2 * h + 1]);
+        }
         if constexpr (MODE == 2) {
           p0 *= w.x;
           p1 *= w.y;

@@ -40,6 +40,49 @@ __host__ __device__ inline int64_t tc_a_span(int kp) { return ((tc_a_img_bytes(k
 __host__ __device__ inline int64_t tc_b_img_bytes(int kp, int bn) { return (int64_t)bn * kp * 2 + (int64_t)bn * 4; }
 
 // ---------------------------------------------------------------------------------------------------
+// laplacian / energy kernels (MODE 4 / 5 of tc_reduce_kernel and tc_bwd_kernel): the same exponent GEMM gives
+// S = -|X - Y|^2 / 2, so d^2 = -2 S, d = d^2 rsqrt(d^2) and k = 2^-d (laplacian, X = x log2e / blur) or k = d (energy).
+//
+// Resolution.  The split operands carry 22 bits (|X_k - h_k - l_k| <= 2^-22 |X_k|, the l.l product is dropped), the
+// rank-one terms 24, and the fp32 accumulation of 3 dk/16 + 1 <= 13 MMAs rounds at the scale of |X|^2 + |Y|^2.
+// Summed, |computed d^2 - d^2| <= 2^-18 (|X|^2 + |Y|^2) in the worst case (random signs make it ~2^-21).  A pair
+// whose d^2 is below that bound cannot be told from a coincident one; since |Y_j| ~ |X_i| for exactly those pairs,
+// the kernels test d^2 against the row's own bound
+//     T_i = max(2^-17 |X_i|^2 + 2^-14, clamp)
+// (2^-14: a floor in the scaled units, d < 2^-7, which also caps P below) and give such a pair the value of a
+// coincident one (d = sqrt(clamp): the reference's 1e-8 clamp, or ~0 under the pykeops convention) and zero gradient.  The
+// gradient of a pair has norm |w_j| for the energy and <= |w_j| / blur for the laplacian, so a pair treated this way
+// moves a row gradient by at most that much; its value by at most |w_j| sqrt(T_i) (energy; laplacian: ln2 times
+// that, in units of blur / log2e).  The diagonal of K_xx / K_yy is exact (tc_zero_diagonal: S = 0).
+//
+// Energy coordinates are unscaled on the CUDA cores.  Here they are multiplied by the power of two that puts the
+// largest centred coordinate of either cloud in [2^9, 2^10): the fp16 l term of any coordinate above 2^-3 (2^-13 of
+// the largest) then stays in fp16's normal range instead of on its 2^-24 subnormal grid, and |X| <= 2^13 keeps every
+// operand far from fp16's 65504.  k = d is linear, so the finalize divides the sum by that power of two exactly; the
+// gradient (X_i - Y_j) / d does not depend on it.
+constexpr int kTcEnergyTopLog2 = 10;
+constexpr float kTcNormRel = 1.0f / 131072.f;    // 2^-17: coefficient of |X_i|^2 in T_i
+constexpr float kTcNormFloor = 1.0f / 16384.f;  // 2^-14: floor of T_i (scaled units)
+// Row gradients: P = w_j k'(d) / d feeds an fp16 GEMM.  The pack normalises the weights to max|w| = kTcPScale = 2^14
+// (as for the gaussian) and the kernel multiplies them by 2^-kTcNormPLog2, so |w| <= 2^8 and, with d >= 2^-7
+// (T_i >= 2^-14), P <= 2^15 < 65504.  Energy: d <= 2^11 sqrt(64) = 2^14, so the P of a weight within 2^-8 of the
+// largest stays normal (>= 2^-14).  Laplacian: P = w 2^-d / d of the largest weight stays normal up to d ~ 18
+// (k ~ 2^-18); farther pairs sit on fp16's 2^-24 subnormal grid, an absolute error of 2^-25 next to P's 2^8 scale.
+// The finalize undoes both scales.
+constexpr int kTcNormPLog2 = 6;
+
+// power of two that maps the largest centred coordinate `amax` into [2^9, 2^10) (1 for an all-zero cloud); the
+// exponent is bounded so that clamp * scale^2 stays finite
+__host__ __device__ inline float tc_energy_coord_scale(float amax) {
+  if (!(amax > 0.f) || !(amax <= 3.0e38f)) return 1.f;
+  int e;
+  frexpf(amax, &e);  // amax < 2^e
+  e = kTcEnergyTopLog2 - e;
+  e = e < -40 ? -40 : (e > 40 ? 40 : e);
+  return ldexpf(1.f, e);
+}
+
+// ---------------------------------------------------------------------------------------------------
 // pack: one thread per (padded) point; writes its 16-byte piece of every K chunk of its tile image
 // ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint4 pack8_f16(const __half* src) {
@@ -55,16 +98,19 @@ __device__ __forceinline__ uint4 pack8_f16(const __half* src) {
 //   c_j = h_scale * (h_a[j] + h_scale_b * h_b[j]) - |Y_j|^2 / 2      (h_a null: just the fold)
 // in the rank-one chunk, and the fp32 weight w_j (kernel conv) behind the bf16 data.  Padding columns get
 // c = -1e38 when h_a is given (softmin: they must vanish from the log-sum-exp) and w = 0 otherwise.
+// `coord_absmax` (energy kernel, see tc_energy_coord_scale): the coordinates are further multiplied by a power of two.
 static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float* __restrict__ w,
                                       const float* __restrict__ h_a, const float* __restrict__ h_b,
                                       float h_scale_b, float h_scale, const float* __restrict__ center,
                                       float scale, int64_t n, int D, int kp, int tile, int is_cols,
                                       unsigned char* __restrict__ out,
                                       const float* __restrict__ row_extra = nullptr,
-                                      const float* __restrict__ w_absmax = nullptr) {
+                                      const float* __restrict__ w_absmax = nullptr,
+                                      const float* __restrict__ coord_absmax = nullptr) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t npad = ((n + tile - 1) / tile) * tile;
   if (p >= npad) return;
+  if (coord_absmax != nullptr) scale *= tc_energy_coord_scale(*coord_absmax);
   const int64_t t = p / tile;
   const int pt = (int)(p % tile);
   const int dk = tc_dk(D);
@@ -173,9 +219,40 @@ __device__ __forceinline__ void tc_zero_diagonal(float (&s)[64], int64_t diag, i
     if (8 * (j >> 2) + cq + (j & 1) == diag + 8 * ((j >> 1) & 1)) s[j] = 0.f;
 }
 
+// MODE 4 / 5: |X_i|^2 of a row of the row image, from its rank-one chunk (r = -|X|^2/2 in three bf16 terms at
+// elements 3..5; no row term is folded in for these modes), and the row's coincidence bound T_i (see above).
+// `clampq` is the clamp on the scaled d^2, already multiplied by the energy coordinate scale squared.
+__device__ __forceinline__ float tc_norm_row_bound(const unsigned char* sa, int kp, int local_row, float clampq) {
+  const int chunk = kTcTerms * (tc_dk_of_kp(kp) / 8);
+  const uint4 v = *reinterpret_cast<const uint4*>(sa + ((int64_t)chunk * kTcM + local_row) * 16);
+  const float r = __bfloat162float(__ushort_as_bfloat16((unsigned short)(v.y >> 16))) +
+                  __bfloat162float(__ushort_as_bfloat16((unsigned short)(v.z & 0xffffu))) +
+                  __bfloat162float(__ushort_as_bfloat16((unsigned short)(v.z >> 16)));
+  return fmaxf(fmaf(-2.f * kTcNormRel, r, kTcNormFloor), clampq);
+}
+// the clamp on the scaled d^2 (never below 1e-30, so that d^2 rsqrt(d^2) of a coincident pair is 0, not NaN)
+__device__ __forceinline__ float tc_norm_clampq(float clampq, const float* coord_absmax) {
+  if (coord_absmax != nullptr) {
+    const float c = tc_energy_coord_scale(*coord_absmax);
+    clampq *= c * c;
+  }
+  return fmaxf(clampq, 1e-30f);
+}
+// k(d) of one pair from its exponent s: d^2 = clamp for a pair below the row bound t (and the diagonal), else -2 s
+template <int MODE>
+__device__ __forceinline__ float tc_norm_value(float s, float t, float clampq) {
+  const float q = -2.f * s;
+  const float d2 = q < t ? clampq : q;
+  const float d = d2 * rsqrt_approx(d2);
+  if constexpr (MODE == 4) return ex2_approx(-d);
+  return d;
+}
+
 // MODE 0: gaussian kernel conv  part[(split*kTcParts + q)*N + row]   = sum_j w_j 2^S_ij
 // MODE 1: softmin               part2[(split*kTcParts + q)*N + row]  = (m, s) with sum_j 2^S_ij = s 2^m  (lazy max,
 //         sum-guarded exactly like softmin.cuh; same partial format as softmin_partial_kernel)
+// MODE 4: laplacian kernel conv  part[...] = sum_j w_j 2^-d_ij       MODE 5: energy  part[...] = sum_j w_j d_ij
+//         (d_ij from the exponent as described above; `clampq` and `coord_absmax` are read by these modes only)
 // (row gradients — modes 2 and 3 — are a two-GEMM kernel of their own: tcbwd.cuh)
 //
 // A CTA owns one 128-row tile: its row image is loaded once by TMA and stays in shared memory, the column tiles
@@ -188,8 +265,8 @@ template <int MODE>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_reduce_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                      float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE,
-                     int D, int self_mode) {
-  static_assert(MODE == 0 || MODE == 1, "row gradients live in tcbwd.cuh");
+                     int D, int self_mode, float clampq, const float* __restrict__ coord_absmax) {
+  static_assert(MODE == 0 || MODE == 1 || MODE == 4 || MODE == 5, "row gradients live in tcbwd.cuh");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int a_bytes = kTcM * kp * 2;
   const int b_bytes = kTcBN * kp * 2 + kTcBN * 4;
@@ -239,6 +316,13 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   float acc[2] = {0.f, 0.f};                 // MODE 0: weighted sums
   float m[2] = {kNegBig, kNegBig}, srun[2] = {0.f, 0.f};  // MODE 1: running (m, s)
   mbar_wait(bar_a, 0);
+  float tb[2] = {0.f, 0.f};  // MODE 4 / 5: coincidence bound of each row
+  if constexpr (MODE >= 4) {
+    clampq = tc_norm_clampq(clampq, coord_absmax);
+    const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    tb[0] = tc_norm_row_bound(sa, kp, lr, clampq);
+    tb[1] = tc_norm_row_bound(sa, kp, lr + 8, clampq);
+  }
   for (int k = 0; k < nt; ++k) {
     const int st = k % NSTAGE;
     mbar_wait(&full_b[st], (k / NSTAGE) & 1);
@@ -257,6 +341,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
         for (int h = 0; h < 2; ++h) {
           ts[h] = fmaf(ex2_approx(s[4 * n8 + 2 * h]), w.x, ts[h]);
           ts[h] = fmaf(ex2_approx(s[4 * n8 + 2 * h + 1]), w.y, ts[h]);
+        }
+      }
+      acc[0] += ts[0];
+      acc[1] += ts[1];
+    } else if constexpr (MODE >= 4) {
+      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(t0 + k) * kTcBN, cq);
+      const float* wts = reinterpret_cast<const float*>(sb + st * b_bytes + kTcBN * kp * 2);
+      float ts[2] = {0.f, 0.f};
+#pragma unroll
+      for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+        const float2 w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          ts[h] = fmaf(tc_norm_value<MODE>(s[4 * n8 + 2 * h], tb[h], clampq), w.x, ts[h]);
+          ts[h] = fmaf(tc_norm_value<MODE>(s[4 * n8 + 2 * h + 1], tb[h], clampq), w.y, ts[h]);
         }
       }
       acc[0] += ts[0];
@@ -297,7 +396,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   for (int h = 0; h < 2; ++h) {
     const int64_t row = row0 + 8 * h;
     if (row < N) {
-      if constexpr (MODE == 0) {
+      if constexpr (MODE != 1) {
         part[((int64_t)split * kTcParts + q) * N + row] = acc[h];
       } else {
         reinterpret_cast<float2*>(part)[((int64_t)split * kTcParts + q) * N + row] = make_float2(m[h], srun[h]);

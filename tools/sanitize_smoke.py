@@ -121,6 +121,15 @@ if "tc" in which:
         check(f"tc_softmin_d{d}", sm, ref_softmin(1.0, x, y, h, 2), 1e-4)
         (gx,) = torch.autograd.grad(sm.sum(), xg)
         assert torch.isfinite(gx).all()
+        # laplacian / energy kernels (tc_reduce_kernel<4/5>, tc_bwd_kernel<4/5>), both conventions; the self term
+        d2 = ((x[:, None, :].double() - x[None, :, :].double()) ** 2).sum(-1)
+        for kind, name in ((1, "laplacian"), (2, "energy"), (0x101, "laplacian_unclamped"), (0x102, "energy_unclamped")):
+            ka = d2.clamp_min(1e-8 if kind < 0x100 else 0.0).sqrt()
+            K = (-ka / 2.0).exp() if (kind & 0xFF) == 1 else -ka
+            out = ops.kernel_conv(kind, xg, x.to(DEV), w[:700].to(DEV), 2.0)
+            check(f"tc_{name}_d{d}", out, (K @ w[:700].double()).float(), 1e-3)
+            (gx,) = torch.autograd.grad(out.sum(), xg)
+            assert torch.isfinite(gx).all()
 if "grid" in which:
     for shape in ((1, 2, 32, 32), (1, 1, 16, 16, 16), (1, 1, 1024, 1024)):
         h = torch.randn(*shape, generator=g)
