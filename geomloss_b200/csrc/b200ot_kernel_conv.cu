@@ -71,13 +71,14 @@ __global__ void conv_fwd_finalize_kernel(const float* __restrict__ part, int n_s
 // gaussian: part (n_split, N, D+1): [0] = sum W e, [1+k] = sum W e Y_k   -> go (accY - X acc0) / (scale blur^2)
 // laplacian / energy: part (n_split, N, D): sum W e u_k                    -> -go acc / blur   (energy: -go acc)
 // (the tensor-core laplacian / energy sums have the gaussian's layout and are finalized as kind 0; coord_absmax: the
-// energy kernel's coordinate scale, applied to X as the kernel applied it to the clouds)
+// energy kernel's coordinate scale, applied to X as the kernel applied it to the clouds; n_per > 0: a batch of elements
+// of n_per rows each, whose weights were normalised per element, w_absmax[i / n_per])
 __global__ void conv_bwd_finalize_kernel(const float* __restrict__ part, int n_split, const float* __restrict__ x,
                                          const float* __restrict__ center, const float* __restrict__ grad_out,
                                          float* __restrict__ grad_x, int64_t N, int D, int kind, float scale,
                                          float coef, const float* __restrict__ w_absmax,
                                          float* __restrict__ value_out = nullptr,
-                                         const float* __restrict__ coord_absmax = nullptr) {
+                                         const float* __restrict__ coord_absmax = nullptr, int64_t n_per = 0) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   if (coord_absmax != nullptr) scale *= tc_energy_coord_scale(*coord_absmax);
@@ -85,7 +86,8 @@ __global__ void conv_bwd_finalize_kernel(const float* __restrict__ part, int n_s
   float wmax = 1.f;
   // tensor-core path: the weights were normalised to max|w| = kTcPScale (tc_pack_kernel); all-zero weights leave
   // all-zero sums
-  if (w_absmax != nullptr && *w_absmax > 0.f) wmax = *w_absmax / kTcPScale;
+  const float wa = w_absmax != nullptr ? w_absmax[n_per > 0 ? i / n_per : 0] : 0.f;
+  if (wa > 0.f) wmax = wa / kTcPScale;
   go *= wmax;
   if (kind == B200OT_KERNEL_GAUSSIAN) {
     const int na = D + 1;
@@ -108,8 +110,11 @@ __global__ void conv_bwd_finalize_kernel(const float* __restrict__ part, int n_s
   }
 }
 
-// max_j |w_j| into *out (zero-initialised by the caller); bit order of non-negative floats = integer order
+// max_j |w_j| into *out (zero-initialised by the caller); bit order of non-negative floats = integer order.
+// gridDim.y > 1: one maximum per batch element of n weights, out[blockIdx.y]
 __global__ void absmax_kernel(const float* __restrict__ w, int64_t n, float* __restrict__ out) {
+  w += (int64_t)blockIdx.y * n;
+  out += blockIdx.y;
   float m = 0.f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     m = fmaxf(m, fabsf(w[i]));
@@ -203,6 +208,7 @@ static float conv_bwd_coef(int kind_flags, const ConvScales& cs, float blur) {
 // ---------------------------------------------------------------------------------------------------
 struct TcPlan {
   int kp, nstage, n_split, tiles_per_split;
+  int rtpe, ctpe;  // row / column tiles per batch element
   int64_t a_tiles, b_tiles, a_bytes, b_bytes, smem;
   int64_t off_b, off_part, off_misc, total;
 };
@@ -282,11 +288,17 @@ static TcBwdTuning tc_bwd_tuning() {
   return t;
 }
 
-static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd = false) {
+// B > 1 (the batched entry points): B problems of N rows x M columns side by side, each element padded to whole tiles on
+// its own (tc_pack_kernel).  The split count is chosen for the whole grid, as without a batch, and cuts each element's
+// ctpe column tiles (so it is capped at ctpe); a CTA never reads another element's columns.  B = 1 is the plan of one
+// problem.
+static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd = false, int64_t B = 1) {
   TcPlan p;
   p.kp = tc_kp(D);
-  p.a_tiles = ceil_div64(N, kTcM);
-  p.b_tiles = ceil_div64(M, kTcBN);
+  p.rtpe = (int)ceil_div64(N, kTcM);
+  p.ctpe = (int)ceil_div64(M, kTcBN);
+  p.a_tiles = B * p.rtpe;
+  p.b_tiles = B * p.ctpe;
   p.a_bytes = tc_a_img_bytes(p.kp);
   p.b_bytes = tc_b_img_bytes(p.kp, kTcBN);
   const int64_t bar_bytes = 256;  // mbarriers behind the column ring
@@ -300,30 +312,30 @@ static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd = false) {
   if (forced > 0) want = forced;
   if (want < 1) want = 1;
   if (want > 64) want = 64;
-  if (want > p.b_tiles) want = p.b_tiles;
-  p.tiles_per_split = (int)ceil_div64(p.b_tiles, want);
-  p.n_split = (int)ceil_div64(p.b_tiles, p.tiles_per_split);
+  if (want > p.ctpe) want = p.ctpe;
+  p.tiles_per_split = (int)ceil_div64(p.ctpe, want);
+  p.n_split = (int)ceil_div64(p.ctpe, p.tiles_per_split);
   p.off_b = round_up64(p.a_tiles * p.a_bytes, 256);
   p.off_part = p.off_b + round_up64(p.b_tiles * p.b_bytes, 256);
   // partials: (m, s) pairs forward, D+1 sums per row backward
-  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? N * (D + 1) : kTcParts * N * 2) * 4, 256);
-  p.total = p.off_misc + 256;  // [0]: max|w| of the row-gradient pass
+  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? B * N * (D + 1) : kTcParts * B * N * 2) * 4, 256);
+  p.total = p.off_misc + round_up64((B + 1) * 4, 256);  // [0]: energy coordinate max, [1 + b]: max|w| of element b
   return p;
 }
 
-int64_t tc_scratch_bytes(int64_t N, int64_t M, int D) {
+int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
   // forward and row-gradient launches split the columns differently: size for the larger of the two
-  return std::max(make_tc_plan(N, M, D, false).total, make_tc_plan(N, M, D, true).total);
+  return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B).total);
 }
 
 // Row gradients on the tensor-core path; `mode` is the MODE of tc_bwd_kernel (2 gaussian conv, 3 softmin p = 2,
-// 4 laplacian, 5 energy; clampq and coord_absmax: see there).  Leaves n_part sets of (N, D+1) partial sums in
-// *part_out.
+// 4 laplacian, 5 energy; clampq and coord_absmax: see there).  Leaves n_part sets of (B N, D+1) partial sums in
+// *part_out.  `batched`: B elements of N rows / M columns (make_tc_plan), the weights normalised per element.
 int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
                    void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out,
-                   float clampq, const float* coord_absmax) {
-  const TcPlan p = make_tc_plan(N, M, D, true);
+                   float clampq, const float* coord_absmax, int64_t B, bool batched) {
+  const TcPlan p = make_tc_plan(N, M, D, true, B);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
   unsigned char* a_imgs = base;
@@ -331,57 +343,68 @@ int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, con
   float* part = reinterpret_cast<float*>(base + p.off_part);
   float* w_absmax = nullptr;
   if (w != nullptr) {
-    // P = w_j e_ij feeds an fp16 GEMM: normalise the weights to max|w| = kTcPScale (undone by the finalize kernel)
-    w_absmax = reinterpret_cast<float*>(base + p.off_misc);
-    B200OT_CUDA_TRY(cudaMemsetAsync(w_absmax, 0, sizeof(float), st));
-    absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(M, 256), 1024), 256, 0, st>>>(w, M, w_absmax);
+    // P = w_j e_ij feeds an fp16 GEMM: normalise the weights to max|w| = kTcPScale (undone by the finalize kernel),
+    // one maximum per batch element, so that a heavy element cannot push a light one's P into fp16's subnormal range
+    w_absmax = reinterpret_cast<float*>(base + p.off_misc) + 1;
+    B200OT_CUDA_TRY(cudaMemsetAsync(w_absmax, 0, B * sizeof(float), st));
+    const dim3 g((unsigned)std::min<int64_t>(ceil_div64(M, 256), 1024), (unsigned)B);
+    absmax_kernel<<<g, 256, 0, st>>>(w, M, w_absmax);
     B200OT_CUDA_TRY(cudaGetLastError());
   }
   if (w_absmax_out) *w_absmax_out = w_absmax;
   const int threads = 128;
   tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, lse2, nullptr, coord_absmax);
+      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, lse2, nullptr, coord_absmax,
+      B);
   B200OT_CUDA_TRY(cudaGetLastError());
   tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
       y, w, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, w_absmax,
-      coord_absmax);
+      coord_absmax, B);
   B200OT_CUDA_TRY(cudaGetLastError());
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
   const int self_mode = (mode != 3 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
   auto launch = [&](auto kern) -> int {
     B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, (int)p.b_tiles, p.tiles_per_split,
-                                                   p.nstage, D, self_mode, clampq, coord_absmax);
+    kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
+                                                   p.nstage, D, self_mode, clampq, coord_absmax, p.rtpe, N);
     B200OT_CUDA_TRY(cudaGetLastError());
     return B200OT_OK;
   };
   const TcBwdTuning tn = tc_bwd_tuning();
-  // (MODE, PT, MERGE, padded dimension) -> instantiation
-  auto pick_dk = [&](auto mode_tag, auto pt_tag, auto merge_tag) -> int {
+  // (MODE, PT, MERGE, padded dimension, batch) -> instantiation
+  auto pick_dk = [&](auto mode_tag, auto pt_tag, auto merge_tag, auto batch_tag) -> int {
     constexpr int MODE = decltype(mode_tag)::value, PT = decltype(pt_tag)::value;
-    constexpr bool MG = decltype(merge_tag)::value;
+    constexpr bool MG = decltype(merge_tag)::value, BT = decltype(batch_tag)::value;
     switch (tc_dk(D)) {
-      case 16: return launch(tc_bwd_kernel<MODE, PT, MG, 16>);
-      case 32: return launch(tc_bwd_kernel<MODE, PT, MG, 32>);
-      case 48: return launch(tc_bwd_kernel<MODE, PT, MG, 48>);
-      default: return launch(tc_bwd_kernel<MODE, PT, MG, 64>);
+      case 16: return launch(tc_bwd_kernel<MODE, PT, MG, 16, BT>);
+      case 32: return launch(tc_bwd_kernel<MODE, PT, MG, 32, BT>);
+      case 48: return launch(tc_bwd_kernel<MODE, PT, MG, 48, BT>);
+      default: return launch(tc_bwd_kernel<MODE, PT, MG, 64, BT>);
     }
+  };
+  // the default variant (PT = 2, MERGE): the only one of the laplacian and energy row gradients and of every batched
+  // row gradient
+  using T2 = std::integral_constant<int, 2>;
+  auto pick_default = [&](auto mode_tag) -> int {
+    return batched ? pick_dk(mode_tag, T2{}, std::true_type{}, std::true_type{})
+                   : pick_dk(mode_tag, T2{}, std::true_type{}, std::false_type{});
   };
   auto pick = [&](auto mode_tag) -> int {
     using T1 = std::integral_constant<int, 1>;
-    using T2 = std::integral_constant<int, 2>;
+    using NB = std::false_type;
+    if (batched) return pick_default(mode_tag);
     if (tn.merge)
-      return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::true_type{}) : pick_dk(mode_tag, T2{}, std::true_type{});
-    return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::false_type{}) : pick_dk(mode_tag, T2{}, std::false_type{});
+      return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::true_type{}, NB{})
+                             : pick_dk(mode_tag, T2{}, std::true_type{}, NB{});
+    return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::false_type{}, NB{})
+                           : pick_dk(mode_tag, T2{}, std::false_type{}, NB{});
   };
-  // (the laplacian and energy row gradients have the default variant only: PT = 2, MERGE)
-  using T2 = std::integral_constant<int, 2>;
   int rc;
   switch (mode) {
     case 2: rc = pick(std::integral_constant<int, 2>{}); break;
     case 3: rc = pick(std::integral_constant<int, 3>{}); break;
-    case 4: rc = pick_dk(std::integral_constant<int, 4>{}, T2{}, std::true_type{}); break;
-    default: rc = pick_dk(std::integral_constant<int, 5>{}, T2{}, std::true_type{}); break;
+    case 4: rc = pick_default(std::integral_constant<int, 4>{}); break;
+    default: rc = pick_default(std::integral_constant<int, 5>{}); break;
   }
   if (rc) return rc;
   *part_out = part;
@@ -390,11 +413,11 @@ int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, con
 }
 
 // Tensor-core softmin partials (p = 2): packs both clouds, runs the reduction, leaves n_part (m, s) sets in
-// `*part_out` (inside scratch) for b200ot_softmin_finalize.
+// `*part_out` (inside scratch) for b200ot_softmin_finalize.  `batched`: B elements (make_tc_plan), B N rows of partials.
 int softmin_partial_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
                        const float* center, int64_t N, int64_t M, int D, float eps, void* scratch,
-                       float** part_out, int* n_part_out, cudaStream_t st) {
-  const TcPlan p = make_tc_plan(N, M, D);
+                       float** part_out, int* n_part_out, cudaStream_t st, int64_t B, bool batched) {
+  const TcPlan p = make_tc_plan(N, M, D, false, B);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
   unsigned char* a_imgs = base;
@@ -403,27 +426,29 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
   const float scale = softmin_coord_scale(2, eps);
   const int threads = 128;
   tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs);
+      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, nullptr, nullptr, nullptr, B);
   B200OT_CUDA_TRY(cudaGetLastError());
   tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, nullptr, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs);
+      y, nullptr, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr, nullptr,
+      B);
   B200OT_CUDA_TRY(cudaGetLastError());
-  auto kern = tc_reduce_kernel<1>;
+  auto kern = batched ? tc_reduce_kernel<1, true> : tc_reduce_kernel<1>;
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
-  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, (int)p.b_tiles,
-                                                        p.tiles_per_split, p.nstage, D, 0, 0.f, nullptr);
+  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
+                                                 p.nstage, D, 0, 0.f, nullptr, p.rtpe, N);
   B200OT_CUDA_TRY(cudaGetLastError());
   *part_out = part;
   *n_part_out = p.n_split * kTcParts;
   return B200OT_OK;
 }
 
-// Energy on the tensor cores: the largest centred coordinate of both clouds, from which every kernel of the pass
-// derives the same power-of-two coordinate scale (tc_energy_coord_scale).  Kept in the scratch's misc block, [1].
+// Energy on the tensor cores: the largest centred coordinate of both clouds (of every batch element: one scale for the
+// whole batch, a power of two that the finalize undoes exactly), from which every kernel of the pass derives the same
+// power-of-two coordinate scale (tc_energy_coord_scale).  Kept in the scratch's misc block, [0].
 static int energy_coord_absmax(const float* x, int64_t N, const float* y, int64_t M, int D, const float* center,
                                unsigned char* misc, cudaStream_t st, const float** out) {
-  float* a = reinterpret_cast<float*>(misc) + 1;
+  float* a = reinterpret_cast<float*>(misc);
   B200OT_CUDA_TRY(cudaMemsetAsync(a, 0, sizeof(float), st));
   coord_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((N + M) * D, 256), 1024), 256, 0, st>>>(x, N, y, M, D,
                                                                                                        center, a);
@@ -433,10 +458,11 @@ static int energy_coord_absmax(const float* x, int64_t N, const float* y, int64_
 }
 
 static int conv_fwd_tc(int kind_flags, const float* x, const float* y, const float* w, const float* center, float* out,
-                       int64_t N, int64_t M, int D, float blur, void* scratch, cudaStream_t st) {
+                       int64_t N, int64_t M, int D, float blur, void* scratch, cudaStream_t st, int64_t B = 1,
+                       bool batched = false) {
   const int kind = kind_base(kind_flags);
   const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
-  const TcPlan p = make_tc_plan(N, M, D);
+  const TcPlan p = make_tc_plan(N, M, D, false, B);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
   unsigned char* a_imgs = base;
@@ -447,27 +473,28 @@ static int conv_fwd_tc(int kind_flags, const float* x, const float* y, const flo
   const float scale = kind == B200OT_KERNEL_GAUSSIAN ? sqrtf(kLog2e) / blur : cs.scale;
   const float* coord_absmax = nullptr;
   if (kind == B200OT_KERNEL_ENERGY) {
-    const int rc = energy_coord_absmax(x, N, y, M, D, center, base + p.off_misc, st, &coord_absmax);
+    const int rc = energy_coord_absmax(x, B * N, y, B * M, D, center, base + p.off_misc, st, &coord_absmax);
     if (rc) return rc;
   }
   const int threads = 128;
   tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
       x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, nullptr, nullptr,
-      coord_absmax);
+      coord_absmax, B);
   B200OT_CUDA_TRY(cudaGetLastError());
   tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, w, nullptr, nullptr, 0.f, 0.f, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr, coord_absmax);
+      y, w, nullptr, nullptr, 0.f, 0.f, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr, coord_absmax,
+      B);
   B200OT_CUDA_TRY(cudaGetLastError());
-  auto kern = kind == B200OT_KERNEL_GAUSSIAN ? tc_reduce_kernel<0>
-              : kind == B200OT_KERNEL_LAPLACIAN ? tc_reduce_kernel<4> : tc_reduce_kernel<5>;
+  auto kern = kind == B200OT_KERNEL_GAUSSIAN ? (batched ? tc_reduce_kernel<0, true> : tc_reduce_kernel<0>)
+              : kind == B200OT_KERNEL_LAPLACIAN ? (batched ? tc_reduce_kernel<4, true> : tc_reduce_kernel<4>)
+                                                : (batched ? tc_reduce_kernel<5, true> : tc_reduce_kernel<5>);
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
-  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, (int)p.b_tiles,
-                                                        p.tiles_per_split, p.nstage, D, self_mode, cs.clampq,
-                                                        coord_absmax);
+  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
+                                                 p.nstage, D, self_mode, cs.clampq, coord_absmax, p.rtpe, N);
   B200OT_CUDA_TRY(cudaGetLastError());
-  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
-      part, p.n_split * kTcParts, kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, N, coord_absmax);
+  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
+      part, p.n_split * kTcParts, kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, B * N, coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
@@ -567,6 +594,53 @@ B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const floa
   return b200ot_kernel_conv_finalize(part, pl.n_split, out, N, kind, stream);
 }
 
+// Row gradients on the tensor cores (and, with value_out, the forward values from the same pass: gaussian only), of one
+// problem or (`batched`) of B elements of N rows / M columns.  Arguments already validated.
+static int conv_bwd_tc(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
+                       float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                       void* scratch, void* stream, int64_t B = 1, bool batched = false) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t n_per = batched ? N : 0;  // rows per element: the finalize undoes each element's weight scale
+  if (kind_base(kind) != B200OT_KERNEL_GAUSSIAN) {
+    // grad = coef (sum_j P Y_j - X_i sum_j P) with P = w k'(d) / d scaled by 2^-kTcNormPLog2 (tcbwd.cuh): the
+    // gaussian's finalize with coef = 2^kTcNormPLog2 / blur (laplacian, X = x log2e / blur) or 2^kTcNormPLog2 (energy)
+    const int kb = kind_base(kind);
+    const ConvScales cs = conv_scales(kind, blur);
+    const float* coord_absmax = nullptr;
+    if (kb == B200OT_KERNEL_ENERGY) {
+      const TcPlan p = make_tc_plan(N, M, D, true, B);
+      const int rc = energy_coord_absmax(x, B * N, y, B * M, D, center,
+                                         reinterpret_cast<unsigned char*>(scratch) + p.off_misc, st, &coord_absmax);
+      if (rc) return rc;
+    }
+    float* tc_part = nullptr;
+    int n_part = 0;
+    const float* w_absmax = nullptr;
+    const int rc = bwd_partial_tc(kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5, x, y, w, nullptr, nullptr, 0.f, nullptr,
+                                  center, cs.scale, N, M, D, scratch, &tc_part, &n_part, st, &w_absmax, cs.clampq,
+                                  coord_absmax, B, batched);
+    if (rc) return rc;
+    const float coef = (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
+    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
+        tc_part, n_part, x, center, grad_out, grad_x, B * N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax,
+        nullptr, coord_absmax, n_per);
+    B200OT_CUDA_TRY(cudaGetLastError());
+    return B200OT_OK;
+  }
+  float* tc_part = nullptr;
+  int n_part = 0;
+  const float scale = sqrtf(kLog2e) / blur;
+  const float* w_absmax = nullptr;
+  const int rc = bwd_partial_tc(2, x, y, w, nullptr, nullptr, 0.f, nullptr, center, scale, N, M, D, scratch, &tc_part,
+                                &n_part, st, &w_absmax, 0.f, nullptr, B, batched);
+  if (rc) return rc;
+  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
+      tc_part, n_part, x, center, grad_out, grad_x, B * N, D, 0, scale, 1.0f / (scale * blur * blur), w_absmax,
+      value_out, nullptr, n_per);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
 // Row gradients (and, with value_out, the forward values from the same pass: gaussian only).
 static int conv_bwd_x_impl(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
                            float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
@@ -579,47 +653,7 @@ static int conv_bwd_x_impl(const float* x, const float* y, const float* w, const
   if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
   if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
   if (scratch_bytes < b200ot_kernel_conv_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
-  if (tc && !gauss) {
-    // grad = coef (sum_j P Y_j - X_i sum_j P) with P = w k'(d) / d scaled by 2^-kTcNormPLog2 (tcbwd.cuh): the
-    // gaussian's finalize with coef = 2^kTcNormPLog2 / blur (laplacian, X = x log2e / blur) or 2^kTcNormPLog2 (energy)
-    const int kb = kind_base(kind);
-    const ConvScales cs = conv_scales(kind, blur);
-    cudaStream_t st = (cudaStream_t)stream;
-    const float* coord_absmax = nullptr;
-    if (kb == B200OT_KERNEL_ENERGY) {
-      const TcPlan p = make_tc_plan(N, M, D, true);
-      const int rc = energy_coord_absmax(x, N, y, M, D, center, reinterpret_cast<unsigned char*>(scratch) + p.off_misc,
-                                         st, &coord_absmax);
-      if (rc) return rc;
-    }
-    float* tc_part = nullptr;
-    int n_part = 0;
-    const float* w_absmax = nullptr;
-    const int rc = bwd_partial_tc(kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5, x, y, w, nullptr, nullptr, 0.f, nullptr,
-                                  center, cs.scale, N, M, D, scratch, &tc_part, &n_part, st, &w_absmax, cs.clampq,
-                                  coord_absmax);
-    if (rc) return rc;
-    const float coef = (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
-    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
-        tc_part, n_part, x, center, grad_out, grad_x, N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax, nullptr,
-        coord_absmax);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    return B200OT_OK;
-  }
-  if (tc) {
-    float* tc_part = nullptr;
-    int n_part = 0;
-    const float scale = sqrtf(kLog2e) / blur;
-    const float* w_absmax = nullptr;
-    const int rc = bwd_partial_tc(2, x, y, w, nullptr, nullptr, 0.f, nullptr, center, scale, N, M, D, scratch,
-                                  &tc_part, &n_part, (cudaStream_t)stream, &w_absmax, 0.f, nullptr);
-    if (rc) return rc;
-    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, (cudaStream_t)stream>>>(
-        tc_part, n_part, x, center, grad_out, grad_x, N, D, 0, scale, 1.0f / (scale * blur * blur), w_absmax,
-        value_out);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    return B200OT_OK;
-  }
+  if (tc) return conv_bwd_tc(x, y, w, center, grad_out, grad_x, value_out, N, M, D, kind, blur, scratch, stream);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -653,6 +687,52 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
   if (!out) return B200OT_EINVAL;
   return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, N, M, D, kind, blur, scratch, scratch_bytes,
                          stream);
+}
+
+// ---- batches of B problems in the tensor-core dimensions (tc_reduce_kernel / tc_bwd_kernel with BATCH) ----
+B200OT_API int64_t b200ot_batched_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
+  return tc_batched_dims(B, N, M, D) ? tc_scratch_bytes(N, M, D, B) : 0;
+}
+
+B200OT_API int b200ot_kernel_conv_fwd_batched(const float* x, const float* y, const float* w, const float* center,
+                                              float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
+                                              float blur, void* scratch, int64_t scratch_bytes, void* stream) {
+  if (!x || !y || !w || !out || !scratch || !tc_batched_dims(B, N, M, D) || !valid_kind(kind)) return B200OT_EINVAL;
+  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  return conv_fwd_tc(kind, x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream, B, true);
+}
+
+static int conv_bwd_x_batched_impl(const float* x, const float* y, const float* w, const float* center,
+                                   const float* grad_out, float* grad_x, float* value_out, int64_t B, int64_t N,
+                                   int64_t M, int32_t D, int32_t kind, float blur, void* scratch,
+                                   int64_t scratch_bytes, void* stream) {
+  if (!x || !y || !w || !grad_x || !scratch || !tc_batched_dims(B, N, M, D) || !valid_kind(kind) ||
+      (value_out && kind_base(kind) != B200OT_KERNEL_GAUSSIAN))
+    return B200OT_EINVAL;
+  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  return conv_bwd_tc(x, y, w, center, grad_out, grad_x, value_out, N, M, D, kind, blur, scratch, stream, B, true);
+}
+
+B200OT_API int b200ot_kernel_conv_bwd_x_batched(const float* x, const float* y, const float* w, const float* center,
+                                                const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                                int32_t D, int32_t kind, float blur, void* scratch,
+                                                int64_t scratch_bytes, void* stream) {
+  if (!grad_out) return B200OT_EINVAL;
+  return conv_bwd_x_batched_impl(x, y, w, center, grad_out, grad_x, nullptr, B, N, M, D, kind, blur, scratch,
+                                 scratch_bytes, stream);
+}
+
+B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float* y, const float* w,
+                                                    const float* center, float* out, float* grad_unit, int64_t B,
+                                                    int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                                                    void* scratch, int64_t scratch_bytes, void* stream) {
+  if (!out) return B200OT_EINVAL;
+  return conv_bwd_x_batched_impl(x, y, w, center, nullptr, grad_unit, out, B, N, M, D, kind, blur, scratch,
+                                 scratch_bytes, stream);
 }
 
 }  // extern "C"

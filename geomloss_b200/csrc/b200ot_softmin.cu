@@ -288,4 +288,23 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
   return b200ot_softmin_finalize(part, pl.n_split, out_old, alpha_old, beta, out, lse2_out, N, eps, stream);
 }
 
+B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const float* h_a, const float* h_b,
+                                          float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                          float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
+                                          int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                          void* stream) {
+  // p = 2 only: the p = 1 softmin has no tensor-core kernel
+  if (!x || !y || !h_a || !scratch || !tc_batched_dims(B, N, M, D) || !valid_p(p) || p_exponent(p) != 2 ||
+      !(eps > 0.f) || (!out && !lse2_out))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  float* tc_part = nullptr;
+  int n_part = 0;
+  const int rc = softmin_partial_tc(x, y, h_a, h_b, h_scale_b, center, N, M, D, eps, scratch, &tc_part, &n_part,
+                                    (cudaStream_t)stream, B, true);
+  if (rc) return rc;
+  return b200ot_softmin_finalize(tc_part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
+}
+
 }  // extern "C"

@@ -212,4 +212,23 @@ B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float*
   return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
 }
 
+B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, const float* h_a, const float* h_b,
+                                            float h_scale_b, const float* center, const float* lse2,
+                                            const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                            int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                            void* stream) {
+  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_batched_dims(B, N, M, D) || !valid_p(p) ||
+      p_exponent(p) != 2 || !(eps > 0.f))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  // P carries kTcPScale, which cancels: the finalize divides by each row's sum of P
+  const int rc = bwd_partial_tc(3, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M,
+                                D, scratch, &part, &n_part, (cudaStream_t)stream, nullptr, 0.f, nullptr, B, true);
+  if (rc) return rc;
+  return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, p, eps, stream);
+}
+
 }  // extern "C"

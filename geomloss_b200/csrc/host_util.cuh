@@ -47,15 +47,22 @@ enum TcOp { kTcSoftminFwd = 0, kTcSoftminBwd = 1, kTcConvFwd = 2, kTcConvBwd = 3
 inline bool tc_capable_dim(int D) { return D >= 1 && D <= 64; }
 bool tc_routed(int op, int D, int64_t N, int64_t M);
 bool tc_any_routed(int D, int64_t N, int64_t M);  // some operator of this shape takes the tensor-core path (scratch sizing)
-int64_t tc_scratch_bytes(int64_t N, int64_t M, int D);
+// B > 1: a batch of B problems of N rows x M columns each (the batched entry points)
+int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B = 1);
+// Shapes of the batched entry points: 8 < D <= 64 only (smaller dimensions batch through the ranges entry points)
+inline bool tc_batched_dims(int64_t B, int64_t N, int64_t M, int D) {
+  return B >= 1 && N > 0 && M > 0 && D > B200OT_MAX_D && tc_capable_dim(D);
+}
+// `batched`: x (B,N,D), y (B,M,D), element b of the rows reduced over element b of the columns only; the kernels'
+// batched instantiations even at B = 1
 int softmin_partial_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
                        const float* center, int64_t N, int64_t M, int D, float eps, void* scratch,
-                       float** part_out, int* n_part_out, cudaStream_t st);
+                       float** part_out, int* n_part_out, cudaStream_t st, int64_t B = 1, bool batched = false);
 
 int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
                    void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out,
-                   float clampq = 0.f, const float* coord_absmax = nullptr);
+                   float clampq = 0.f, const float* coord_absmax = nullptr, int64_t B = 1, bool batched = false);
 
 #define B200OT_STR2(x) #x
 #define B200OT_STR(x) B200OT_STR2(x)

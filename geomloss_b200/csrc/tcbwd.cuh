@@ -80,11 +80,12 @@ __device__ __forceinline__ float tc_norm_p(float s, float t, float w) {
   return q < t ? 0.f : p;
 }
 
-template <int MODE, int PT, bool MERGE, int DK>
+// BATCH: B problems side by side, laid out and mapped to rows and column tiles as in tc_reduce_kernel (tcconv.cuh).
+template <int MODE, int PT, bool MERGE, int DK, bool BATCH = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_bwd_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                   float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE, int D,
-                  int self_mode, float clampq, const float* __restrict__ coord_absmax) {
+                  int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe, int64_t n_local) {
   static_assert(MODE == 2 || MODE == 3 || MODE == 4 || MODE == 5, "row-gradient modes");
   static_assert(PT == 1 || PT == 2, "P is fed to GEMM 2 as one or two fp16 terms");
   static_assert(DK % 16 == 0 && DK <= 64, "padded dimension");
@@ -100,8 +101,9 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row_tile = blockIdx.x;
   const int split = blockIdx.y;
-  const int t0 = split * tiles_per_split;
-  const int t1 = min(ntiles_b, t0 + tiles_per_split);
+  const int elem = BATCH ? row_tile / rtpe : 0;
+  const int t0 = elem * ntiles_b + split * tiles_per_split;
+  const int t1 = min((elem + 1) * ntiles_b, t0 + tiles_per_split);
   const int nt = t1 - t0;
 
   if (threadIdx.x == 0) {
@@ -222,7 +224,11 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     float tot = sum[h];
     tot += __shfl_xor_sync(0xffffffffu, tot, 1);
     tot += __shfl_xor_sync(0xffffffffu, tot, 2);
-    const int64_t row = row0 + 8 * h;
+    int64_t row = row0 + 8 * h;
+    if constexpr (BATCH) {
+      const int64_t local = row - (int64_t)elem * rtpe * kTcM;
+      row = local < n_local ? (int64_t)elem * n_local + local : N;
+    }
     if (row < N) {
       float* dst = part + ((int64_t)split * N + row) * (D + 1);
       if (cq == 0) dst[0] = tot;

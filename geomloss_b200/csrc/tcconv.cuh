@@ -99,6 +99,9 @@ __device__ __forceinline__ uint4 pack8_f16(const __half* src) {
 // in the rank-one chunk, and the fp32 weight w_j (kernel conv) behind the bf16 data.  Padding columns get
 // c = -1e38 when h_a is given (softmin: they must vanish from the log-sum-exp) and w = 0 otherwise.
 // `coord_absmax` (energy kernel, see tc_energy_coord_scale): the coordinates are further multiplied by a power of two.
+// Batches (`nb` elements of n points each, stored back to back): every element is padded to whole tiles on its own, so
+// slot p belongs to element b = p / npad and reads point b n + (p - b npad); h_a, h_b, w and row_extra are indexed the
+// same way, and the weights of element b are normalised by w_absmax[b].
 static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float* __restrict__ w,
                                       const float* __restrict__ h_a, const float* __restrict__ h_b,
                                       float h_scale_b, float h_scale, const float* __restrict__ center,
@@ -106,17 +109,20 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
                                       unsigned char* __restrict__ out,
                                       const float* __restrict__ row_extra = nullptr,
                                       const float* __restrict__ w_absmax = nullptr,
-                                      const float* __restrict__ coord_absmax = nullptr) {
+                                      const float* __restrict__ coord_absmax = nullptr, int64_t nb = 1) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t npad = ((n + tile - 1) / tile) * tile;
-  if (p >= npad) return;
+  if (p >= npad * nb) return;
   if (coord_absmax != nullptr) scale *= tc_energy_coord_scale(*coord_absmax);
+  const int64_t b = p / npad;
+  const int64_t local = p - b * npad;
+  const int64_t src = b * n + local;
   const int64_t t = p / tile;
   const int pt = (int)(p % tile);
   const int dk = tc_dk(D);
   const int64_t img_bytes = (int64_t)tile * kp * 2 + (is_cols ? (int64_t)tile * 4 : 0);
   unsigned char* img = out + t * img_bytes;
-  const bool live = p < n;
+  const bool live = local < n;
   float sq = 0.f;
   for (int kc = 0; kc < dk / 8; ++kc) {
     __half term[kTcTerms][8];
@@ -124,7 +130,7 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
     for (int k = 0; k < 8; ++k) {
       const int d = kc * 8 + k;
       float X = 0.f;
-      if (live && d < D) X = scale * (pts[p * D + d] - (center ? center[d] : 0.f));
+      if (live && d < D) X = scale * (pts[src * D + d] - (center ? center[d] : 0.f));
       X = fminf(fmaxf(X, -60000.f), 60000.f);  // fp16 range (only reached when every exponent underflows anyway)
       sq = fmaf(X, X, sq);
       const __half h = __float2half_rn(X);
@@ -139,11 +145,11 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
   {
     float r = live ? -0.5f * sq : 0.f;
     // softmin backward: exponent - lse2_i + kTcPLog2 (P = 2^14 softmax weight, common.cuh)
-    if (!is_cols && row_extra != nullptr && live) r -= row_extra[p] - (float)kTcPLog2;
+    if (!is_cols && row_extra != nullptr && live) r -= row_extra[src] - (float)kTcPLog2;
     if (is_cols && h_a != nullptr) {
       if (live) {
-        float h = h_a[p];
-        if (h_b != nullptr) h = fmaf(h_scale_b, h_b[p], h);
+        float h = h_a[src];
+        if (h_b != nullptr) h = fmaf(h_scale_b, h_b[src], h);
         r = fmaf(h_scale, h, r);
       } else {
         r = -1.0e38f;
@@ -173,8 +179,8 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
   if (is_cols) {
     // (row-gradient kernels feed P = w e to an fp16 GEMM: weights are normalised to |w| <= kTcPScale = 2^14, which
     // keeps P out of fp16's subnormal range; undone in the finalize)
-    float wv = (live && w) ? w[p] : 0.f;
-    if (w_absmax != nullptr && *w_absmax > 0.f) wv = (wv / *w_absmax) * kTcPScale;
+    float wv = (live && w) ? w[src] : 0.f;
+    if (w_absmax != nullptr && w_absmax[b] > 0.f) wv = (wv / w_absmax[b]) * kTcPScale;
     reinterpret_cast<float*>(img + (int64_t)tile * kp * 2)[pt] = wv;
   }
 }
@@ -261,11 +267,18 @@ __device__ __forceinline__ float tc_norm_value(float s, float t, float clampq) {
 // row sums in the same registers: while one warpgroup runs its exponentials the tensor cores serve the other.
 // A thread holds two rows x 32 columns of every tile; q = lane % 4 picks which quarter of the columns it summed,
 // and the four quarters are kept as separate partial sets (no shuffles, merged by the finalize kernels).
-template <int MODE>
+//
+// BATCH: B problems of n_local rows against the same number of columns each, every element padded to whole tiles on
+// its own (tc_pack_kernel).  Row tile r belongs to element b = r / rtpe and reads only that element's column tiles
+// [b ntiles_b, (b + 1) ntiles_b) (ntiles_b = column tiles per element), cut into splits as without a batch; a live row
+// (local index < n_local) writes its partials at row b n_local + local of the N = B n_local rows, padding rows write
+// nothing.  Rows and columns of a self term are padded alike, so `row0 - column` still finds the diagonal.
+template <int MODE, bool BATCH = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_reduce_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                      float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE,
-                     int D, int self_mode, float clampq, const float* __restrict__ coord_absmax) {
+                     int D, int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe,
+                     int64_t n_local) {
   static_assert(MODE == 0 || MODE == 1 || MODE == 4 || MODE == 5, "row gradients live in tcbwd.cuh");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int a_bytes = kTcM * kp * 2;
@@ -279,8 +292,9 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row_tile = blockIdx.x;
   const int split = blockIdx.y;
-  const int t0 = split * tiles_per_split;
-  const int t1 = min(ntiles_b, t0 + tiles_per_split);
+  const int elem = BATCH ? row_tile / rtpe : 0;
+  const int t0 = elem * ntiles_b + split * tiles_per_split;
+  const int t1 = min((elem + 1) * ntiles_b, t0 + tiles_per_split);
   const int nt = t1 - t0;
 
   if (threadIdx.x == 0) {
@@ -394,7 +408,11 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   const int q = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int64_t row = row0 + 8 * h;
+    int64_t row = row0 + 8 * h;
+    if constexpr (BATCH) {
+      const int64_t local = row - (int64_t)elem * rtpe * kTcM;
+      row = local < n_local ? (int64_t)elem * n_local + local : N;
+    }
     if (row < N) {
       if constexpr (MODE != 1) {
         part[((int64_t)split * kTcParts + q) * N + row] = acc[h];

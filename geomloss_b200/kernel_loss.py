@@ -49,8 +49,9 @@ def kernel_points(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=Non
 
 
 def kernel_points_batched(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=None, keops=False, **_ignored):
-    """Batched kernel norms a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D), D <= 8: the three (four) matvecs are ranges-mode
-    reductions over the block-diagonal stacked problem — one launch group each for the whole batch.
+    """Batched kernel norms a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D): the three (four) matvecs take one launch group each
+    for the whole batch — for D <= 8 ranges-mode reductions over the block-diagonal stacked problem, for 8 < D <= 64
+    the batched tensor-core operators (ops.kernel_conv_batched).
     Reference: kernel_loss on (B, ...) inputs (kernel_samples.py:92-146)."""
     from . import ranges
 
@@ -64,9 +65,18 @@ def kernel_points_batched(a, x, b, y, name=None, blur=0.05, potentials=False, ke
     kid = ops.KERNEL_KINDS[name] | (ops.KERNEL_UNCLAMPED if keops else 0)
     xf, yf, af, bf = x.reshape(B * N, D), y.reshape(B * M, D), a.reshape(B * N), b.reshape(B * M)
     center = ops.default_center(xf.detach(), yf.detach())
+    dg = _TwiceGrad.apply
+    if D > ops.MAX_D:
+        cv = ops.kernel_conv_batched
+        a_x = cv(kid, dg(x), x.detach(), a.detach(), blur, center=center)
+        b_y = cv(kid, dg(y), y.detach(), b.detach(), blur, center=center)
+        b_x = cv(kid, x, y, b, blur, center=center)
+        if potentials:
+            a_y = cv(kid, y, x, a, blur, center=center)
+            return a_x - b_x, b_y - a_y
+        return 0.5 * (dg(a) * a_x).sum(1) + 0.5 * (dg(b) * b_y).sum(1) - (a * b_x).sum(1)
     p_xx, p_yy = ranges.batch_problem(B, N, N, dev), ranges.batch_problem(B, M, M, dev)
     p_xy, p_yx = ranges.batch_problem(B, N, M, dev), ranges.batch_problem(B, M, N, dev)
-    dg = _TwiceGrad.apply
     cv = ranges.kernel_conv_ranges
     a_x = cv(kid, dg(xf), xf.detach(), af.detach(), blur, p_xx, None, center=center)
     b_y = cv(kid, dg(yf), yf.detach(), bf.detach(), blur, p_yy, None, center=center)

@@ -353,3 +353,205 @@ class _KernelConv(torch.autograd.Function):
 def kernel_conv(kind, x, y, w, blur, *, center=None):
     fused = (FUSED_CONV_GRAD and torch.is_grad_enabled() and x.requires_grad and (kind_id(kind) & 0xFF) == 0)
     return _KernelConv.apply(x, y, w, kind, blur, center, bool(fused))
+
+
+# ------------------------------------------------------------------------------------------------
+# batches of B problems in the tensor-core dimensions (8 < D <= 64): x (B,N,D), y (B,M,D), per-column vectors (B,M),
+# per-row vectors (B,N); element b of the rows is reduced over element b of the columns only, the whole batch in one
+# launch group per call (b200ot_*_batched).  Same contracts as the one-problem operators above.
+# ------------------------------------------------------------------------------------------------
+def _check_batch(x, y):
+    if x.dim() != 3 or y.dim() != 3 or x.shape[0] != y.shape[0] or x.shape[2] != y.shape[2]:
+        raise ValueError(f"expected x:(B,N,D), y:(B,M,D); got {tuple(x.shape)}, {tuple(y.shape)}")
+    B, N, D = x.shape
+    M = y.shape[1]
+    if B == 0 or N == 0 or M == 0:
+        raise ValueError("empty batch or point cloud")
+    if not MAX_D < D <= MAX_D_TC:
+        raise NotImplementedError(f"the batched tensor-core operators serve {MAX_D} < D <= {MAX_D_TC}, got D = {D} "
+                                  f"(batches with D <= {MAX_D} run as block-diagonal ranges problems, ranges.py)")
+    if x.device != y.device:
+        raise ValueError("x and y must be on the same device")
+    return B, N, M, D
+
+
+def _per_point(t, n, name):
+    if t is not None and t.numel() != n:
+        raise ValueError(f"{name} must have one entry per point of its cloud ({n}), got {tuple(t.shape)}")
+
+
+def _batched_scratch(L, B, N, M, D, dev):
+    return _scratch(L.b200ot_batched_scratch_bytes(B, N, M, D), dev, "batched")
+
+
+def softmin_batched_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, out_old=None, alpha_old=0.0,
+                        beta=1.0, out=None, want_lse2=False):
+    """``softmin_raw`` on a batch: out (B,N) <- alpha_old*out_old + beta*softmin(eps, (x[b], y[b]), h[b]).  p = 2 only.
+    No autograd.  Returns ``(out, lse2 | None)``."""
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
+    B, N, M, D = _check_batch(x, y)
+    if (p & 0xFF) != 2:
+        raise NotImplementedError(f"p = {p & 0xFF}: the batched softmin exists for p = 2 only (tensor cores)")
+    _per_point(h_a, B * M, "h_a")
+    _per_point(h_b, B * M, "h_b")
+    _per_point(out_old, B * N, "out_old")
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev), nvtx_range(f"b200ot.softmin_batched B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
+        if out is None:
+            out = torch.empty(B, N, dtype=torch.float32, device=dev)
+        lse2 = torch.empty(B, N, dtype=torch.float32, device=dev) if want_lse2 else None
+        scratch = _batched_scratch(L, B, N, M, D, dev)
+        rc = L.b200ot_softmin_fwd_batched(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
+                                          _ptr(out_old), float(alpha_old), float(beta), _ptr(out), _ptr(lse2), B, N,
+                                          M, D, int(p), float(eps), _ptr(scratch), scratch.numel(), _stream(dev))
+    _lib.check(rc, "b200ot_softmin_fwd_batched")
+    count_launches(3)
+    return out, lse2
+
+
+def softmin_batched_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None):
+    """grad_x (B,N,D) of <grad_out, softmin_batched(eps, x, y, h)> with y, h constant (b200ot_softmin_bwd_x_batched)."""
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
+    B, N, M, D = _check_batch(x, y)
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        scratch = _batched_scratch(L, B, N, M, D, dev)
+        rc = L.b200ot_softmin_bwd_x_batched(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
+                                            _ptr(lse2), _ptr(grad_out), _ptr(gx), B, N, M, D, int(p), float(eps),
+                                            _ptr(scratch), scratch.numel(), _stream(dev))
+    _lib.check(rc, "b200ot_softmin_bwd_x_batched")
+    count_launches(3)
+    return gx
+
+
+class _SoftminBatched(torch.autograd.Function):
+    """softmin_batched with _Softmin's autograd contract: the gradient flows to the row clouds x only."""
+
+    @staticmethod
+    def forward(ctx, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out):
+        need_grad = ctx.needs_input_grad[0]
+        out, lse2 = softmin_batched_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out,
+                                        want_lse2=need_grad)
+        if need_grad:
+            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
+                                  lse2)
+            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), h_b is not None, center is not None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
+        h_scale_b, eps, p, scale_out, has_hb, has_center = ctx.meta
+        go = (grad_out * scale_out).contiguous()
+        gx = softmin_batched_grad_rows(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, lse2, go, p=p,
+                                       center=center if has_center else None)
+        return gx, None, None, None, None, None, None, None, None
+
+
+def softmin_batched(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
+    """Differentiable (w.r.t. x) batched softmin, (B,N): ``softmin`` element by element."""
+    return _SoftminBatched.apply(x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps,
+                                 p, center, scale_out)
+
+
+def _conv_batched_args(x, y, w, center):
+    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
+    B, N, M, D = _check_batch(x, y)
+    _per_point(w, B * M, "w")
+    return x, y, w, center, B, N, M, D
+
+
+def kernel_conv_batched_raw(kind, x, y, w, blur, *, center=None):
+    """out (B,N), out[b, i] = sum_j k(x[b, i], y[b, j]) w[b, j], no autograd."""
+    x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev), nvtx_range(f"b200ot.kernel_conv_batched kind={kind} B={B} N={N} M={M} D={D}"):
+        out = torch.empty(B, N, dtype=torch.float32, device=dev)
+        scratch = _batched_scratch(L, B, N, M, D, dev)
+        rc = L.b200ot_kernel_conv_fwd_batched(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(out), B, N, M, D,
+                                              kind_id(kind), float(blur), _ptr(scratch), scratch.numel(),
+                                              _stream(dev))
+    _lib.check(rc, "b200ot_kernel_conv_fwd_batched")
+    count_launches(3)
+    return out
+
+
+def kernel_conv_batched_grad_rows(kind, x, y, w, blur, grad_out, *, center=None):
+    x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
+    grad_out = _f32c(grad_out, "grad_out")
+    _per_point(grad_out, B * N, "grad_out")
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        scratch = _batched_scratch(L, B, N, M, D, dev)
+        rc = L.b200ot_kernel_conv_bwd_x_batched(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(grad_out), _ptr(gx), B,
+                                                N, M, D, kind_id(kind), float(blur), _ptr(scratch), scratch.numel(),
+                                                _stream(dev))
+    _lib.check(rc, "b200ot_kernel_conv_bwd_x_batched")
+    count_launches(3)
+    return gx
+
+
+def kernel_conv_batched_value_and_grad_rows(kind, x, y, w, blur, *, center=None):
+    """``kernel_conv_value_and_grad_rows`` on a batch (gaussian only): (out (B,N), grad_unit (B,N,D))."""
+    if (kind_id(kind) & 0xFF) != 0:
+        raise ValueError("the one-pass value + row gradient exists for the gaussian kernel only")
+    x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev), nvtx_range(f"b200ot.kernel_conv_batched value+grad B={B} N={N} M={M} D={D}"):
+        out = torch.empty(B, N, dtype=torch.float32, device=dev)
+        gunit = torch.empty_like(x)
+        scratch = _batched_scratch(L, B, N, M, D, dev)
+        rc = L.b200ot_kernel_conv_fwd_bwd_x_batched(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(out), _ptr(gunit),
+                                                    B, N, M, D, kind_id(kind), float(blur), _ptr(scratch),
+                                                    scratch.numel(), _stream(dev))
+    _lib.check(rc, "b200ot_kernel_conv_fwd_bwd_x_batched")
+    count_launches(3)
+    return out, gunit
+
+
+class _KernelConvBatched(torch.autograd.Function):
+    """kernel_conv_batched with _KernelConv's contract: gradients to x, y and w; `fused`: the gaussian value and unit
+    row gradient from one pass."""
+
+    @staticmethod
+    def forward(ctx, x, y, w, kind, blur, center, fused):
+        if fused:
+            out, gunit = kernel_conv_batched_value_and_grad_rows(kind, x, y, w, blur, center=center)
+        else:
+            out, gunit = kernel_conv_batched_raw(kind, x, y, w, blur, center=center), None
+        ctx.save_for_backward(x, y, w, center if center is not None else w, gunit if fused else w)
+        ctx.meta = (kind, float(blur), center is not None, fused)
+        return out
+
+    @staticmethod
+    def backward(ctx, go):
+        x, y, w, center, gunit = ctx.saved_tensors
+        kind, blur, has_center, fused = ctx.meta
+        center = center if has_center else None
+        go = go.contiguous()
+        gx = gy = gw = None
+        if ctx.needs_input_grad[0]:
+            if fused:
+                gx = go.unsqueeze(-1) * gunit
+            else:
+                gx = kernel_conv_batched_grad_rows(kind, x, y, w, blur, go, center=center)
+        if ctx.needs_input_grad[1]:
+            gy = kernel_conv_batched_grad_rows(kind, y, x, go, blur, w, center=center)
+        if ctx.needs_input_grad[2]:
+            gw = kernel_conv_batched_raw(kind, y, x, go, blur, center=center).view_as(w)
+        return gx, gy, gw, None, None, None, None
+
+
+def kernel_conv_batched(kind, x, y, w, blur, *, center=None):
+    """out (B,N) = K(x[b], y[b]) @ w[b] for every b, differentiable w.r.t. x, y and w."""
+    fused = (FUSED_CONV_GRAD and torch.is_grad_enabled() and x.requires_grad and (kind_id(kind) & 0xFF) == 0)
+    return _KernelConvBatched.apply(x, y, w, kind, blur, center, bool(fused))

@@ -15,7 +15,10 @@ exactly — and differ only where the reference's two backends differ numericall
 "tensorized" clamps |x-y|^2 at 1e-8 under the square root (utils.py:56-61) while "online" and "multiscale" use the
 pykeops norm (no clamp).  "multiscale" is the two-scale Sinkhorn with kernel truncation / the truncated kernel
 norms (multiscale.py) on the ranges mode of the same kernels, with exactly the reference's cluster blocks.
-Batched inputs (B, N, D) with D <= 8 run as ONE block-diagonal launch group per reduction (ranges.py).
+Batched inputs (B, N, D) run as ONE launch group per reduction for the whole batch: a block-diagonal ranges problem
+for D <= 8 (ranges.py), the batched tensor-core operators for 8 < D <= 64 (ops.softmin_batched / kernel_conv_batched;
+Sinkhorn with p = 2 only: p = 1 above D = 8 raises NotImplementedError, batched or not).  Column-sharded multi-GPU
+engines solve the batch element by element.
 Inputs must be float32 CUDA tensors: there is no CPU path.
 """
 from __future__ import annotations
@@ -27,11 +30,16 @@ import warnings
 
 from .kernel_loss import kernel_points, kernel_points_batched
 from .multiscale import kernel_multiscale, sinkhorn_multiscale
-from .ops import MAX_D
+from .ops import MAX_D, MAX_D_TC
 from . import kernel_small, sinkhorn_small
 from .sinkhorn import sinkhorn_points, sinkhorn_points_batched
 
 _LOSSES = ("sinkhorn", "hausdorff", "energy", "gaussian", "laplacian")
+
+# Batches above D = 8 take the batched tensor-core operators while one element has at most this many pairs.  A larger
+# element fills the GPU on its own, and the batched launch (B elements' column images streamed at once) is then no
+# faster than the per-element loop.  Measured with tools/bench_batched_tc.py (DESIGN.md section 3.5b).
+BATCHED_TC_MAX_PAIRS = 1e9
 _BACKENDS = ("auto", "tensorized", "online", "multiscale")
 
 
@@ -165,8 +173,12 @@ class SamplesLoss(Module):
             from .sinkhorn import max_diameter
 
             kw["diameter"] = max_diameter(x.reshape(-1, D), y.reshape(-1, D))
-        if B > 1 and D <= MAX_D and not self._engine and self.loss != "hausdorff":
-            # the whole batch in one launch group per reduction (block-diagonal ranges problem)
+        # (a p = 1 Sinkhorn above D = 8 has no batched operator: the loop below raises NotImplementedError)
+        one_group = D <= MAX_D or (D <= MAX_D_TC and (self.loss != "sinkhorn" or self.p == 2)
+                                   and N * M <= BATCHED_TC_MAX_PAIRS)
+        if B > 1 and one_group and not self._engine and self.loss != "hausdorff":
+            # the whole batch in one launch group per reduction (D <= 8: block-diagonal ranges problem; above: the
+            # batched tensor-core operators)
             batched = sinkhorn_points_batched if self.loss == "sinkhorn" else kernel_points_batched
             if self.loss != "sinkhorn":
                 kw["name"] = self.loss

@@ -190,8 +190,9 @@ def sinkhorn_cost_batched(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, B, debias=True
 
 def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scaling=0.5, debias=True,
                             potentials=False, keops=False, **_ignored):
-    """Batched Sinkhorn divergence a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D), D <= 8: every softmin of the loop is ONE
-    ranges-mode launch group over the whole batch (block-diagonal problem), not B launches.
+    """Batched Sinkhorn divergence a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D): every softmin of the loop is ONE launch group
+    over the whole batch, not B launches — for D <= 8 a ranges-mode block-diagonal problem, for 8 < D <= 64 (p = 2)
+    the batched tensor-core operators (ops.softmin_batched_raw / softmin_batched).
     Reference: sinkhorn_tensorized / sinkhorn_online on (B, ...) inputs, softmin_online_lazytensor
     (sinkhorn_samples.py:74-221, :229-290, :349-424); one shared eps-schedule (diameter over the flattened batch)."""
     from . import ranges
@@ -204,14 +205,28 @@ def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=Non
     xf, yf, af, bf = x.reshape(B * N, D), y.reshape(B * M, D), a.reshape(B * N), b.reshape(B * M)
     center = ops.default_center(xf.detach(), yf.detach())
     dev = x.device
-    problems = {"xy": ranges.batch_problem(B, N, M, dev), "yx": ranges.batch_problem(B, M, N, dev)}
-    if debias:
-        problems["xx"] = ranges.batch_problem(B, N, N, dev)
-        problems["yy"] = ranges.batch_problem(B, M, M, dev)
     pk = (p | ops.P_UNCLAMPED) if keops else p
+    loop = dict(p=pk, debias=debias, center=center)
+    if D > ops.MAX_D:
+        # the loop runs on the flattened clouds and potentials; the operators see the (B, n, D) views
+        def sm(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
+            out, lse2 = ops.softmin_batched_raw(eps, rows.view(B, -1, D), cols.view(B, -1, D), h_a, h_b, h_scale_b,
+                                                **kw)
+            return out.view(-1), None if lse2 is None else lse2.view(-1)
+
+        def smg(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
+            return ops.softmin_batched(eps, rows.view(B, -1, D), cols.view(B, -1, D), h_a, h_b, h_scale_b,
+                                       **kw).view(-1)
+
+        loop.update(softmin_raw=sm, softmin_grad=smg)
+    else:
+        problems = {"xy": ranges.batch_problem(B, N, M, dev), "yx": ranges.batch_problem(B, M, N, dev)}
+        if debias:
+            problems["xx"] = ranges.batch_problem(B, N, N, dev)
+            problems["yy"] = ranges.batch_problem(B, M, M, dev)
+        loop.update(problems=problems)
     f_aa, g_bb, g_ab, f_ba = sinkhorn_loop_points(log_weights(af.detach()), log_weights(bf.detach()), xf, yf,
-                                                  eps_list, rho, p=pk, debias=debias, center=center,
-                                                  problems=problems)
+                                                  eps_list, rho, **loop)
     out = sinkhorn_cost_batched(eps, rho, af, bf, f_aa, g_bb, g_ab, f_ba, B, debias=debias, potentials=potentials)
     if potentials:
         return out[0].view(B, N), out[1].view(B, M)

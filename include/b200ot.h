@@ -218,6 +218,40 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
                                  float* out, float* grad_unit, int64_t N, int64_t M, int32_t D, int32_t kind,
                                  float blur, void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Batched problems in the tensor-core dimensions (8 < D <= 64): B independent problems of the same shape in one
+ * launch group per call — the batched LazyTensor reductions of the reference (softmin_online_lazytensor,
+ * sinkhorn_samples.py:229-290; kernel_loss on (B, N, D) inputs).  x (B,N,D), y (B,M,D); h_a, h_b, w (B,M); out,
+ * lse2, grad_out (B,N); grad_x (B,N,D); center (D) shared by the whole batch.  Row i of element b is reduced over
+ * the columns of element b only.  Arguments and results are those of the one-problem entries above, element by
+ * element; p = 2 only (p = 1 has no tensor-core softmin); D <= 8 batches go through the ranges entry points.
+ * EINVAL for B < 1, D <= 8 or D > 64; scratch: b200ot_batched_scratch_bytes(B, N, M, D) bytes, 16-byte aligned.
+ * The batched row gradients run the default variant of the row-gradient kernel ($B200OT_TC_BWD is not read).
+ * ------------------------------------------------------------------------------------------- */
+B200OT_API int64_t b200ot_batched_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D);
+B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const float* h_a, const float* h_b,
+                                          float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                          float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
+                                          int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                          void* stream);
+B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, const float* h_a, const float* h_b,
+                                            float h_scale_b, const float* center, const float* lse2,
+                                            const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                            int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                            void* stream);
+B200OT_API int b200ot_kernel_conv_fwd_batched(const float* x, const float* y, const float* w, const float* center,
+                                              float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
+                                              float blur, void* scratch, int64_t scratch_bytes, void* stream);
+B200OT_API int b200ot_kernel_conv_bwd_x_batched(const float* x, const float* y, const float* w, const float* center,
+                                                const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                                int32_t D, int32_t kind, float blur, void* scratch,
+                                                int64_t scratch_bytes, void* stream);
+/* gaussian only, like b200ot_kernel_conv_fwd_bwd_x */
+B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float* y, const float* w,
+                                                    const float* center, float* out, float* grad_unit, int64_t B,
+                                                    int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                                                    void* scratch, int64_t scratch_bytes, void* stream);
+
 /* --- stages of the CUDA-core kernel convolutions (D <= B200OT_MAX_D), ranges mode: truncated block-sparse
  *     MMDs (kernel_multiscale, kernel_samples.py:177-271) and batched problems.  cols: gather-packed,
  *     b200ot_packed_cols_floats(n_slots, D, 2) floats.  part: (N) sums (backward = 0) or (N, width) sums

@@ -30,7 +30,7 @@ def check(name, got, ref, tol=2e-5):
     assert err < tol, name
 
 
-which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "grid", "loss"}
+which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "grid", "loss"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -130,6 +130,30 @@ if "tc" in which:
             check(f"tc_{name}_d{d}", out, (K @ w[:700].double()).float(), 1e-3)
             (gx,) = torch.autograd.grad(out.sum(), xg)
             assert torch.isfinite(gx).all()
+if "batched" in which:
+    # the batched tensor-core kernels (tc_reduce_kernel<0/1/4/5, BATCH>, tc_bwd_kernel<2/3/4/5, ..., BATCH>), each
+    # element checked against its own columns
+    B, n = 3, 300
+    for d in (16, 64):
+        x, y = torch.rand(B, n, d, generator=g), torch.rand(B, n, d, generator=g)
+        h, w = torch.randn(B, n, generator=g), torch.rand(B, n, generator=g)
+        xd, yd, hd, wd, ones = x.to(DEV), y.to(DEV), h.to(DEV), w.to(DEV), torch.ones(B, n, device=DEV)
+        center = ops.default_center(xd.view(-1, d), yd.view(-1, d))
+        d2 = ((x[:, :, None, :].double() - y[:, None, :, :].double()) ** 2).sum(-1)
+        out, lse2 = ops.softmin_batched_raw(1.0, xd, yd, hd, p=2, center=center, want_lse2=True)
+        check(f"batched_softmin_d{d}", out, (-torch.logsumexp(h.double()[:, None, :] - d2 / 2.0, dim=2)).float(), 1e-4)
+        gx = ops.softmin_batched_grad_rows(1.0, xd, yd, hd, None, 0.0, lse2, ones, p=2, center=center)
+        prob = torch.softmax(h.double()[:, None, :] - d2 / 2.0, dim=2)
+        check(f"batched_softmin_grad_d{d}", gx, x.double() - prob @ y.double(), 1e-4)
+        for kind, K in ((0, (-d2 / 8.0).exp()), (1, (-d2.clamp_min(1e-8).sqrt() / 2.0).exp()),
+                        (2, -d2.clamp_min(1e-8).sqrt())):
+            conv = ops.kernel_conv_batched_raw(kind, xd, yd, wd, 2.0, center=center)
+            check(f"batched_conv{kind}_d{d}", conv, (K @ w.double()[:, :, None])[..., 0], 1e-3)
+            gc = ops.kernel_conv_batched_grad_rows(kind, xd, yd, wd, 2.0, ones, center=center)
+            assert torch.isfinite(gc).all()
+        val, gu = ops.kernel_conv_batched_value_and_grad_rows(0, xd, yd, wd, 2.0, center=center)
+        check(f"batched_conv_value_d{d}", val, ((-d2 / 8.0).exp() @ w.double()[:, :, None])[..., 0], 1e-4)
+        assert torch.isfinite(gu).all()
 if "grid" in which:
     for shape in ((1, 2, 32, 32), (1, 1, 16, 16, 16), (1, 1, 1024, 1024)):
         h = torch.randn(*shape, generator=g)
