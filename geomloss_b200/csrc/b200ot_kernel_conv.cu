@@ -16,7 +16,9 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <type_traits>
+#include <vector>
 
 namespace b200ot {
 
@@ -366,7 +368,7 @@ int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, con
   auto launch = [&](auto kern) -> int {
     B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
     kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
-                                                   p.nstage, D, self_mode, clampq, coord_absmax, p.rtpe, N);
+                                                   p.nstage, D, self_mode, clampq, coord_absmax, p.rtpe, N, nullptr, nullptr, nullptr);
     B200OT_CUDA_TRY(cudaGetLastError());
     return B200OT_OK;
   };
@@ -436,10 +438,137 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
   kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
-                                                 p.nstage, D, 0, 0.f, nullptr, p.rtpe, N);
+                                                 p.nstage, D, 0, 0.f, nullptr, p.rtpe, N, nullptr, nullptr, nullptr);
   B200OT_CUDA_TRY(cudaGetLastError());
   *part_out = part;
   *n_part_out = p.n_split * kTcParts;
+  return B200OT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Block-sparse softmins (the fine phase of the two-scale Sinkhorn above D = 8): every row cluster and every column
+// cluster is padded to whole 128-point tiles on its own, slot -> point through row_src / col_src (-1: padding).  One
+// segment per row tile; the host descriptors are validated here and copied into the scratch behind the partials.
+// ---------------------------------------------------------------------------------------------------
+static_assert(kTcBlocksTile == kTcM && kTcBlocksTile == kTcBN, "segments are one row tile, pieces whole column tiles");
+
+int blocks_validate(int64_t n_row_slots, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
+                    const b200ot_piece* pieces, int* max_tiles, int64_t* n_pieces) {
+  if (n_row_slots <= 0 || n_col_slots <= 0 || n_row_slots % kTcM || n_col_slots % kTcBN ||
+      n_row_slots / kTcM != n_seg || n_col_slots / kTcBN > 0x7fffffff)
+    return B200OT_EINVAL;
+  int64_t np = 0;
+  for (int64_t s = 0; s < n_seg; ++s) {
+    const b200ot_segment& g = seg[s];
+    if (g.row_start < 0 || g.row_start % kTcM || g.row_start >= n_row_slots || g.row_count < 1 ||
+        g.row_count > kTcM || g.piece_begin < 0 || g.piece_end < g.piece_begin)
+      return B200OT_EINVAL;
+    np = std::max<int64_t>(np, g.piece_end);
+  }
+  // column tiles before piece q, so that a segment's tile count is one difference
+  std::vector<int64_t> before(np + 1, 0);
+  for (int64_t q = 0; q < np; ++q) {
+    const b200ot_piece& c = pieces[q];
+    if (c.col_start < 0 || c.col_start % kTcBN || c.col_count <= 0 || c.col_count % kTcBN ||
+        (int64_t)c.col_start + c.col_count > n_col_slots)
+      return B200OT_EINVAL;
+    before[q + 1] = before[q] + c.col_count / kTcBN;
+  }
+  // every row tile belongs to exactly one segment: each live row is written once per split
+  std::vector<char> seen(n_seg, 0);
+  int64_t mt = 0;
+  for (int64_t s = 0; s < n_seg; ++s) {
+    const int64_t t = seg[s].row_start / kTcM;
+    if (seen[t]) return B200OT_EINVAL;
+    seen[t] = 1;
+    mt = std::max(mt, before[seg[s].piece_end] - before[seg[s].piece_begin]);
+  }
+  if (mt > 0x7fffffff) return B200OT_EINVAL;
+  *max_tiles = (int)mt;
+  *n_pieces = np;
+  return B200OT_OK;
+}
+
+// The plan of one block-sparse problem: images of n_row_slots / n_col_slots points, segments cut into splits the way
+// make_tc_plan cuts a dense problem's column tiles (from the longest segment), then the descriptors.
+static TcPlan make_tc_blocks_plan(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
+                                  int max_tiles, int D, bool bwd) {
+  TcPlan p = make_tc_plan(kTcM, kTcBN, D, bwd);
+  p.a_tiles = n_row_slots / kTcM;
+  p.b_tiles = n_col_slots / kTcBN;
+  int64_t want = ceil_div64((int64_t)num_sms() * 4, n_seg);
+  const int forced = forced_splits();  // test hook (plan.cuh)
+  if (forced > 0) want = forced;
+  if (want < 1) want = 1;
+  if (want > 64) want = 64;
+  const int mt = std::max(max_tiles, 1);
+  if (want > mt) want = mt;
+  p.tiles_per_split = (int)ceil_div64(mt, want);
+  p.n_split = (int)ceil_div64(mt, p.tiles_per_split);
+  p.off_b = round_up64(p.a_tiles * p.a_bytes, 256);
+  p.off_part = p.off_b + round_up64(p.b_tiles * p.b_bytes, 256);
+  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? N * (D + 1) : kTcParts * N * 2) * 4, 256);
+  p.total = p.off_misc + round_up64(n_seg * 16, 256) + round_up64(std::max<int64_t>(n_pieces, 1) * 8, 256);
+  return p;
+}
+
+int64_t tc_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
+                                int max_tiles, int D) {
+  return std::max(make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, false).total,
+                  make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, true).total);
+}
+
+// Pack, descriptor copy and reduction of one block-sparse softmin (bwd: the row-gradient sums, lse2 = the forward's);
+// arguments already validated.  Leaves n_part partial sets of N rows in *part_out, like softmin_partial_tc (forward)
+// and bwd_partial_tc (backward).
+int softmin_blocks_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                      const float* center, const float* lse2, int64_t N, const int* row_src, int64_t n_row_slots,
+                      const int* col_src, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
+                      const b200ot_piece* pieces, int64_t n_pieces, int max_tiles, int D, float eps, void* scratch,
+                      float** part_out, int* n_part_out, cudaStream_t st) {
+  const TcPlan p = make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, bwd);
+  if (p.nstage < 1) return B200OT_EINVAL;
+  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
+  unsigned char* a_imgs = base;
+  unsigned char* b_imgs = base + p.off_b;
+  float* part = reinterpret_cast<float*>(base + p.off_part);
+  int4* d_seg = reinterpret_cast<int4*>(base + p.off_misc);
+  int2* d_pieces = reinterpret_cast<int2*>(base + p.off_misc + round_up64(n_seg * 16, 256));
+  const float scale = softmin_coord_scale(2, eps);
+  B200OT_CUDA_TRY(cudaMemcpyAsync(d_seg, seg, n_seg * 16, cudaMemcpyHostToDevice, st));
+  if (n_pieces > 0) B200OT_CUDA_TRY(cudaMemcpyAsync(d_pieces, pieces, n_pieces * 8, cudaMemcpyHostToDevice, st));
+  const int threads = 128;
+  tc_pack_kernel<<<(unsigned)ceil_div64(n_row_slots, threads), threads, 0, st>>>(
+      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, n_row_slots, D, p.kp, kTcM, 0, a_imgs,
+      bwd ? lse2 : nullptr, nullptr, nullptr, 1, row_src);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  tc_pack_kernel<<<(unsigned)ceil_div64(n_col_slots, threads), threads, 0, st>>>(
+      y, nullptr, h_a, h_b, h_scale_b, kLog2e, center, scale, n_col_slots, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr,
+      nullptr, 1, col_src);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  dim3 grid((unsigned)n_seg, (unsigned)p.n_split);
+  auto launch = [&](auto kern) -> int {
+    B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+    kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, 0, p.tiles_per_split, p.nstage, D, 0,
+                                                   0.f, nullptr, 0, 0, d_seg, d_pieces, row_src);
+    B200OT_CUDA_TRY(cudaGetLastError());
+    return B200OT_OK;
+  };
+  int rc;
+  if (!bwd) {
+    rc = launch(tc_reduce_kernel<1, false, true>);
+  } else {
+    // the default row-gradient variant (PT = 2, MERGE)
+    switch (tc_dk(D)) {
+      case 16: rc = launch(tc_bwd_kernel<3, 2, true, 16, false, true>); break;
+      case 32: rc = launch(tc_bwd_kernel<3, 2, true, 32, false, true>); break;
+      case 48: rc = launch(tc_bwd_kernel<3, 2, true, 48, false, true>); break;
+      default: rc = launch(tc_bwd_kernel<3, 2, true, 64, false, true>); break;
+    }
+  }
+  if (rc) return rc;
+  *part_out = part;
+  *n_part_out = bwd ? p.n_split : p.n_split * kTcParts;
   return B200OT_OK;
 }
 
@@ -491,7 +620,7 @@ static int conv_fwd_tc(int kind_flags, const float* x, const float* y, const flo
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
   dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
   kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
-                                                 p.nstage, D, self_mode, cs.clampq, coord_absmax, p.rtpe, N);
+                                                 p.nstage, D, self_mode, cs.clampq, coord_absmax, p.rtpe, N, nullptr, nullptr, nullptr);
   B200OT_CUDA_TRY(cudaGetLastError());
   conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
       part, p.n_split * kTcParts, kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, B * N, coord_absmax);

@@ -307,4 +307,43 @@ B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const 
   return b200ot_softmin_finalize(tc_part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
 }
 
+B200OT_API void b200ot_blocks_shape(int32_t* rows_per_segment, int32_t* col_align) {
+  if (rows_per_segment) *rows_per_segment = kTcBlocksTile;
+  if (col_align) *col_align = kTcBlocksTile;
+}
+
+B200OT_API int64_t b200ot_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots,
+                                               const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
+                                               int32_t D) {
+  int max_tiles = 0;
+  int64_t n_pieces = 0;
+  if (blocks_check(N, n_row_slots, n_col_slots, seg, n_seg, pieces, D, 2, 1.f, nullptr, &max_tiles, &n_pieces))
+    return 0;
+  return tc_blocks_scratch_bytes(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D);
+}
+
+B200OT_API int b200ot_softmin_fwd_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
+                                         float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                         float beta, float* out, float* lse2_out, int64_t N, const int32_t* row_src,
+                                         int64_t n_row_slots, const int32_t* col_src, int64_t n_col_slots,
+                                         const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
+                                         int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                         void* stream) {
+  if (!x || !y || !h_a || !row_src || !col_src || !scratch || (!out && !lse2_out)) return B200OT_EINVAL;
+  int max_tiles = 0;
+  int64_t n_pieces = 0;
+  const int rc =
+      blocks_check(N, n_row_slots, n_col_slots, seg, n_seg, pieces, D, p, eps, scratch, &max_tiles, &n_pieces);
+  if (rc) return rc;
+  if (scratch_bytes < tc_blocks_scratch_bytes(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D))
+    return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  const int rc2 = softmin_blocks_tc(false, x, y, h_a, h_b, h_scale_b, center, nullptr, N, row_src, n_row_slots, col_src,
+                                    n_col_slots, seg, n_seg, pieces, n_pieces, max_tiles, D, eps, scratch, &part,
+                                    &n_part, (cudaStream_t)stream);
+  if (rc2) return rc2;
+  return b200ot_softmin_finalize(part, n_part, out_old, alpha_old, beta, out, lse2_out, N, eps, stream);
+}
+
 }  // extern "C"

@@ -231,4 +231,29 @@ B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, cons
   return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, p, eps, stream);
 }
 
+B200OT_API int b200ot_softmin_bwd_x_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
+                                           float h_scale_b, const float* center, const float* lse2,
+                                           const float* grad_out, float* grad_x, int64_t N, const int32_t* row_src,
+                                           int64_t n_row_slots, const int32_t* col_src, int64_t n_col_slots,
+                                           const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
+                                           int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                           void* stream) {
+  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !row_src || !col_src || !scratch) return B200OT_EINVAL;
+  int max_tiles = 0;
+  int64_t n_pieces = 0;
+  const int rc =
+      blocks_check(N, n_row_slots, n_col_slots, seg, n_seg, pieces, D, p, eps, scratch, &max_tiles, &n_pieces);
+  if (rc) return rc;
+  if (scratch_bytes < tc_blocks_scratch_bytes(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D))
+    return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  // P carries kTcPScale, which cancels: the finalize divides by each row's sum of P
+  const int rc2 = softmin_blocks_tc(true, x, y, h_a, h_b, h_scale_b, center, lse2, N, row_src, n_row_slots, col_src,
+                                    n_col_slots, seg, n_seg, pieces, n_pieces, max_tiles, D, eps, scratch, &part,
+                                    &n_part, (cudaStream_t)stream);
+  if (rc2) return rc2;
+  return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
+}
+
 }  // extern "C"

@@ -64,6 +64,33 @@ int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, con
                    void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out,
                    float clampq = 0.f, const float* coord_absmax = nullptr, int64_t B = 1, bool batched = false);
 
+// Block-sparse softmins on the tensor cores (8 < D <= 64, p = 2; b200ot_*_blocks).  blocks_validate checks the host
+// descriptors (tile-aligned, one segment per row tile) and returns the longest segment in column tiles and the number
+// of pieces the segments reference.
+inline bool tc_blocks_dims(int D) { return D > B200OT_MAX_D && tc_capable_dim(D); }
+constexpr int kTcBlocksTile = 128;  // segment height and column alignment: the kernels' tile (kTcM = kTcBN, tcconv.cuh)
+int blocks_validate(int64_t n_row_slots, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
+                    const b200ot_piece* pieces, int* max_tiles, int64_t* n_pieces);
+int64_t tc_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
+                                int max_tiles, int D);
+int softmin_blocks_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                      const float* center, const float* lse2, int64_t N, const int* row_src, int64_t n_row_slots,
+                      const int* col_src, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
+                      const b200ot_piece* pieces, int64_t n_pieces, int max_tiles, int D, float eps, void* scratch,
+                      float** part_out, int* n_part_out, cudaStream_t st);
+// The checks every b200ot_*_blocks entry makes before any launch, in this order: EINVAL for a null descriptor array,
+// N <= 0, n_seg <= 0, D outside (8, 64], p other than 2 (| B200OT_P_UNCLAMPED) or eps <= 0; EALIGN for misaligned
+// descriptor arrays or scratch; EINVAL for descriptors off the tile grid (blocks_validate).
+inline int blocks_check(int64_t N, int64_t n_row_slots, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
+                        const b200ot_piece* pieces, int D, int p, float eps, const void* scratch, int* max_tiles,
+                        int64_t* n_pieces) {
+  if (!seg || !pieces || N <= 0 || n_seg <= 0 || n_seg > 0x7fffffff || !tc_blocks_dims(D) || !valid_p(p) ||
+      p_exponent(p) != 2 || !(eps > 0.f))
+    return B200OT_EINVAL;
+  if ((((uintptr_t)seg) & 15) || (((uintptr_t)pieces) & 7) || (((uintptr_t)scratch) & 15)) return B200OT_EALIGN;
+  return blocks_validate(n_row_slots, n_col_slots, seg, n_seg, pieces, max_tiles, n_pieces);
+}
+
 #define B200OT_STR2(x) #x
 #define B200OT_STR(x) B200OT_STR2(x)
 #define B200OT_CUDA_TRY(expr)                                                         \

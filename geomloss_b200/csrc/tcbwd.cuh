@@ -81,14 +81,19 @@ __device__ __forceinline__ float tc_norm_p(float s, float t, float w) {
 }
 
 // BATCH: B problems side by side, laid out and mapped to rows and column tiles as in tc_reduce_kernel (tcconv.cuh).
-template <int MODE, int PT, bool MERGE, int DK, bool BATCH = false>
+// BLOCKS: block-sparse softmin (MODE 3), segments, pieces and row_src as in tc_reduce_kernel; a split without a tile
+// writes zero sums.
+template <int MODE, int PT, bool MERGE, int DK, bool BATCH = false, bool BLOCKS = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_bwd_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                   float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE, int D,
-                  int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe, int64_t n_local) {
+                  int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe, int64_t n_local,
+                  const int4* __restrict__ bseg = nullptr, const int2* __restrict__ bpieces = nullptr,
+                  const int* __restrict__ row_src = nullptr) {
   static_assert(MODE == 2 || MODE == 3 || MODE == 4 || MODE == 5, "row-gradient modes");
   static_assert(PT == 1 || PT == 2, "P is fed to GEMM 2 as one or two fp16 terms");
   static_assert(DK % 16 == 0 && DK <= 64, "padded dimension");
+  static_assert(!BLOCKS || (MODE == 3 && !BATCH), "the block-sparse layout serves the softmin of one problem");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int a_bytes = kTcM * kp * 2;
   const int b_bytes = kTcBN * kp * 2 + kTcBN * 4;
@@ -99,12 +104,14 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   uint64_t* empty_b = full_b + kTcMaxStage;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row_tile = blockIdx.x;
   const int split = blockIdx.y;
+  TcBlockSpan bs{};
+  if constexpr (BLOCKS) bs = tc_block_span(bseg, bpieces, blockIdx.x, split, tiles_per_split);
+  const int row_tile = BLOCKS ? bs.row_tile : (int)blockIdx.x;
   const int elem = BATCH ? row_tile / rtpe : 0;
   const int t0 = elem * ntiles_b + split * tiles_per_split;
   const int t1 = min((elem + 1) * ntiles_b, t0 + tiles_per_split);
-  const int nt = t1 - t0;
+  const int nt = BLOCKS ? bs.nt : t1 - t0;
 
   if (threadIdx.x == 0) {
     mbar_init(bar_a, 1);
@@ -121,11 +128,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     if (lane == 0) {
       mbar_arrive_expect_tx(bar_a, a_bytes);
       tma_load_1d(sa, a_imgs + (int64_t)row_tile * a_bytes, a_bytes, bar_a);
+      int pc = bs.piece, off = bs.off;  // BLOCKS: position in the segment's pieces
       for (int k = 0; k < nt; ++k) {
         const int st = k % NSTAGE;
         if (k >= NSTAGE) mbar_wait(&empty_b[st], ((k / NSTAGE) + 1) & 1);
         mbar_arrive_expect_tx(&full_b[st], b_bytes);
-        tma_load_1d(sb + st * b_bytes, b_imgs + (int64_t)(t0 + k) * b_bytes, b_bytes, &full_b[st]);
+        int ct = t0 + k;
+        if constexpr (BLOCKS) {
+          const int2 pp = bpieces[pc];
+          ct = pp.x / kTcBN + off;
+          if (++off == pp.y / kTcBN) {
+            ++pc;
+            off = 0;
+          }
+        }
+        tma_load_1d(sb + st * b_bytes, b_imgs + (int64_t)ct * b_bytes, b_bytes, &full_b[st]);
       }
     }
     return;
@@ -228,6 +245,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     if constexpr (BATCH) {
       const int64_t local = row - (int64_t)elem * rtpe * kTcM;
       row = local < n_local ? (int64_t)elem * n_local + local : N;
+    }
+    if constexpr (BLOCKS) {
+      const int g = row_src[row];
+      row = g >= 0 ? g : N;
     }
     if (row < N) {
       float* dst = part + ((int64_t)split * N + row) * (D + 1);

@@ -102,6 +102,8 @@ __device__ __forceinline__ uint4 pack8_f16(const __half* src) {
 // Batches (`nb` elements of n points each, stored back to back): every element is padded to whole tiles on its own, so
 // slot p belongs to element b = p / npad and reads point b n + (p - b npad); h_a, h_b, w and row_extra are indexed the
 // same way, and the weights of element b are normalised by w_absmax[b].
+// Gather (block-sparse problems, n = number of slots, a multiple of the tile): slot p reads point gather[p], or is
+// padding when gather[p] < 0.
 static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float* __restrict__ w,
                                       const float* __restrict__ h_a, const float* __restrict__ h_b,
                                       float h_scale_b, float h_scale, const float* __restrict__ center,
@@ -109,20 +111,26 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
                                       unsigned char* __restrict__ out,
                                       const float* __restrict__ row_extra = nullptr,
                                       const float* __restrict__ w_absmax = nullptr,
-                                      const float* __restrict__ coord_absmax = nullptr, int64_t nb = 1) {
+                                      const float* __restrict__ coord_absmax = nullptr, int64_t nb = 1,
+                                      const int* __restrict__ gather = nullptr) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t npad = ((n + tile - 1) / tile) * tile;
   if (p >= npad * nb) return;
   if (coord_absmax != nullptr) scale *= tc_energy_coord_scale(*coord_absmax);
   const int64_t b = p / npad;
   const int64_t local = p - b * npad;
-  const int64_t src = b * n + local;
+  int64_t src = b * n + local;
   const int64_t t = p / tile;
   const int pt = (int)(p % tile);
   const int dk = tc_dk(D);
   const int64_t img_bytes = (int64_t)tile * kp * 2 + (is_cols ? (int64_t)tile * 4 : 0);
   unsigned char* img = out + t * img_bytes;
-  const bool live = local < n;
+  bool live = local < n;
+  if (gather != nullptr) {
+    const int g = gather[p];
+    live = g >= 0;
+    src = live ? g : 0;
+  }
   float sq = 0.f;
   for (int kc = 0; kc < dk / 8; ++kc) {
     __half term[kTcTerms][8];
@@ -254,6 +262,35 @@ __device__ __forceinline__ float tc_norm_value(float s, float t, float clampq) {
   return d;
 }
 
+// BLOCKS (block-sparse problems): CTA x runs segment x = (row_start, row_count, piece_begin, piece_end) of `bseg`, one
+// 128-row tile of one row cluster; its columns are the pieces [piece_begin, piece_end) of `bpieces`, (col_start,
+// col_count) runs of whole column tiles.  Rows, columns and pieces are in slots, multiples of 128 (validated by the
+// host).  The split's tiles are [split tps, split tps + tps) of the concatenation of the segment's pieces; `piece` /
+// `off` locate the first of them.  A split past the segment's last tile has nt = 0.
+struct TcBlockSpan {
+  int row_tile, nt, piece, off;
+};
+__device__ __forceinline__ TcBlockSpan tc_block_span(const int4* __restrict__ seg, const int2* __restrict__ pieces,
+                                                     int s, int split, int tps) {
+  const int4 sg = seg[s];
+  TcBlockSpan r;
+  r.row_tile = sg.x / kTcM;
+  const int first = split * tps;
+  int pc = sg.z, acc = 0;
+  while (pc < sg.w) {
+    const int n = pieces[pc].y / kTcBN;
+    if (acc + n > first) break;
+    acc += n;
+    ++pc;
+  }
+  r.piece = pc;
+  r.off = first - acc;
+  int total = acc;
+  for (int q = pc; q < sg.w && total < first + tps; ++q) total += pieces[q].y / kTcBN;
+  r.nt = max(0, min(tps, total - first));
+  return r;
+}
+
 // MODE 0: gaussian kernel conv  part[(split*kTcParts + q)*N + row]   = sum_j w_j 2^S_ij
 // MODE 1: softmin               part2[(split*kTcParts + q)*N + row]  = (m, s) with sum_j 2^S_ij = s 2^m  (lazy max,
 //         sum-guarded exactly like softmin.cuh; same partial format as softmin_partial_kernel)
@@ -273,13 +310,18 @@ __device__ __forceinline__ float tc_norm_value(float s, float t, float clampq) {
 // [b ntiles_b, (b + 1) ntiles_b) (ntiles_b = column tiles per element), cut into splits as without a batch; a live row
 // (local index < n_local) writes its partials at row b n_local + local of the N = B n_local rows, padding rows write
 // nothing.  Rows and columns of a self term are padded alike, so `row0 - column` still finds the diagonal.
-template <int MODE, bool BATCH = false>
+// BLOCKS (softmin only): CTA x runs segment x (tc_block_span); row slot r writes its partials at row row_src[r], padding
+// slots (row_src < 0) write nothing.  Every split writes every live row of its segment, (kNegBig, 0) when it has no
+// tile, so the finalize merges without knowing the layout.
+template <int MODE, bool BATCH = false, bool BLOCKS = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_reduce_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                      float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE,
                      int D, int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe,
-                     int64_t n_local) {
+                     int64_t n_local, const int4* __restrict__ bseg = nullptr,
+                     const int2* __restrict__ bpieces = nullptr, const int* __restrict__ row_src = nullptr) {
   static_assert(MODE == 0 || MODE == 1 || MODE == 4 || MODE == 5, "row gradients live in tcbwd.cuh");
+  static_assert(!BLOCKS || (MODE == 1 && !BATCH), "the block-sparse layout serves the softmin of one problem");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int a_bytes = kTcM * kp * 2;
   const int b_bytes = kTcBN * kp * 2 + kTcBN * 4;
@@ -290,12 +332,14 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   uint64_t* empty_b = full_b + kTcMaxStage;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row_tile = blockIdx.x;
   const int split = blockIdx.y;
+  TcBlockSpan bs{};
+  if constexpr (BLOCKS) bs = tc_block_span(bseg, bpieces, blockIdx.x, split, tiles_per_split);
+  const int row_tile = BLOCKS ? bs.row_tile : (int)blockIdx.x;
   const int elem = BATCH ? row_tile / rtpe : 0;
   const int t0 = elem * ntiles_b + split * tiles_per_split;
   const int t1 = min((elem + 1) * ntiles_b, t0 + tiles_per_split);
-  const int nt = t1 - t0;
+  const int nt = BLOCKS ? bs.nt : t1 - t0;
 
   if (threadIdx.x == 0) {
     mbar_init(bar_a, 1);
@@ -312,11 +356,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     if (lane == 0) {
       mbar_arrive_expect_tx(bar_a, a_bytes);
       tma_load_1d(sa, a_imgs + (int64_t)row_tile * a_bytes, a_bytes, bar_a);
+      int pc = bs.piece, off = bs.off;  // BLOCKS: position in the segment's pieces
       for (int k = 0; k < nt; ++k) {
         const int st = k % NSTAGE;
         if (k >= NSTAGE) mbar_wait(&empty_b[st], ((k / NSTAGE) + 1) & 1);
         mbar_arrive_expect_tx(&full_b[st], b_bytes);
-        tma_load_1d(sb + st * b_bytes, b_imgs + (int64_t)(t0 + k) * b_bytes, b_bytes, &full_b[st]);
+        int ct = t0 + k;
+        if constexpr (BLOCKS) {
+          const int2 pp = bpieces[pc];
+          ct = pp.x / kTcBN + off;
+          if (++off == pp.y / kTcBN) {
+            ++pc;
+            off = 0;
+          }
+        }
+        tma_load_1d(sb + st * b_bytes, b_imgs + (int64_t)ct * b_bytes, b_bytes, &full_b[st]);
       }
     }
     return;
@@ -412,6 +466,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     if constexpr (BATCH) {
       const int64_t local = row - (int64_t)elem * rtpe * kTcM;
       row = local < n_local ? (int64_t)elem * n_local + local : N;
+    }
+    if constexpr (BLOCKS) {
+      const int g = row_src[row];
+      row = g >= 0 ? g : N;
     }
     if (row < N) {
       if constexpr (MODE != 1) {

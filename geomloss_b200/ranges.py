@@ -14,6 +14,12 @@ A problem is described to libb200ot.so (include/b200ot.h, "ranges mode") by
 The kernels then visit exactly the (row group, column group) pairs of the boolean ``keep`` matrix — the same blocks
 as the reference, not a tile-level superset.  Everything below is vectorised torch on the device (no Python loop
 over clusters); the only host syncs are the sizes of the descriptor arrays.
+
+These are the CUDA-core kernels, D <= 8.  For 8 < D <= 64 the same ``keep`` matrix is run by the tensor-core kernels
+(``variant=TC``, the b200ot_*_blocks entries): every row cluster AND every column cluster is padded to whole 128-point
+tiles, segments are single 128-row tiles of one row cluster and pieces runs of whole column tiles.  Padding slots cost
+computation (a cluster of 1 point fills a tile) but no accuracy: padding columns vanish from the log-sum-exp and
+padding rows write nothing.
 """
 from __future__ import annotations
 
@@ -24,12 +30,20 @@ import torch
 from . import _lib, ops
 
 BIG, SMALL = 0, 1
+TC = 2  # block-sparse tensor-core problems, 8 < D <= 64
 
 
 def shape(variant):
     r, c, al = ctypes.c_int32(0), ctypes.c_int32(0), ctypes.c_int32(0)
     _lib.lib().b200ot_ranges_shape(int(variant), ctypes.byref(r), ctypes.byref(c), ctypes.byref(al))
     return r.value, c.value, al.value
+
+
+def blocks_shape():
+    """(rows per segment, column alignment) of the tensor-core block-sparse problems: both 128."""
+    r, al = ctypes.c_int32(0), ctypes.c_int32(0)
+    _lib.lib().b200ot_blocks_shape(ctypes.byref(r), ctypes.byref(al))
+    return r.value, al.value
 
 
 def _excl_cumsum(t):
@@ -44,6 +58,7 @@ class ColumnLayout:
     def __init__(self, counts, align=16):
         counts = counts.to(torch.int64)
         dev = counts.device
+        self.align = align
         self.counts = counts
         self.padded = (counts + align - 1) // align * align
         self.col_start = _excl_cumsum(counts)
@@ -61,11 +76,15 @@ class ColumnLayout:
 class RangesProblem:
     """Descriptor arrays of one reduction problem (rows x grouped columns restricted to ``keep``)."""
 
-    def __init__(self, seg, pieces, layout, variant, n_rows, density):
+    def __init__(self, seg, pieces, layout, variant, n_rows, density, row_layout=None, computed=None):
         self.seg, self.pieces, self.layout, self.variant = seg, pieces, layout, variant
         self.n_seg = int(seg.shape[0])
         self.n_rows = n_rows
         self.density = density  # kept (row, column) pairs / all pairs
+        # TC: the row slot layout, and the (row slot, column slot) pairs the kernels compute / all pairs
+        self.row_layout = row_layout
+        self.computed = density if computed is None else computed
+        self._scratch_bytes = {}
 
 
 def pick_variant(row_counts, col_counts):
@@ -84,7 +103,14 @@ def build_problem(keep, row_counts, layout, variant=None, rank=0, world=1):
     R, C = row_counts.numel(), layout.counts.numel()
     if variant is None:
         variant = pick_variant(row_counts, layout.counts)
-    max_rows, max_cols, _ = shape(variant)
+    tc = variant == TC
+    if tc:
+        max_rows, align = blocks_shape()
+        if layout.align != align or world > 1:
+            raise ValueError(f"tensor-core block problems need a ColumnLayout(counts, align={align}) and one GPU")
+        max_cols = max(layout.n_slots, 1)  # a run of kept column clusters is one piece
+    else:
+        max_rows, max_cols, _ = shape(variant)
     if keep is None:
         keep = torch.ones(R, C, dtype=torch.bool, device=dev)
     keep = keep.to(torch.bool)
@@ -118,20 +144,33 @@ def build_problem(keep, row_counts, layout, variant=None, rank=0, world=1):
     pieces = torch.stack([col_start, col_count], dim=1).to(torch.int32).contiguous()
     per_row = torch.zeros(R, dtype=torch.int64, device=dev).index_add_(0, run_row, n_piece)
     piece_ptr = _excl_cumsum(per_row)
-    # segments: every row group is cut into CTA-sized runs of rows sharing its piece list
+    # segments: every row group is cut into CTA-sized runs of rows sharing its piece list (TC: whole row tiles of the
+    # row slot layout, every row cluster padded to a multiple of 128 rows on its own)
+    row_layout = ColumnLayout(row_counts, align=max_rows) if tc else None
     row_off = _excl_cumsum(row_counts)
     n_seg_r = (row_counts + max_rows - 1) // max_rows
     seg_grp = torch.repeat_interleave(torch.arange(R, device=dev), n_seg_r)
     k_seg = torch.arange(seg_grp.numel(), device=dev) - (n_seg_r.cumsum(0) - n_seg_r)[seg_grp]
-    row_start = row_off[seg_grp] + k_seg * max_rows
-    row_count = torch.minimum(torch.full_like(row_start, max_rows), row_off[seg_grp + 1] - row_start)
+    row_base = row_layout.slot_start if tc else row_off
+    row_start = row_base[seg_grp] + k_seg * max_rows
+    row_count = torch.minimum(torch.full_like(row_start, max_rows), row_off[seg_grp + 1] - (row_off[seg_grp] +
+                                                                                             k_seg * max_rows))
     seg = torch.stack([row_start, row_count, piece_ptr[seg_grp], piece_ptr[seg_grp + 1]], dim=1)
     # heaviest segments first: shortens the tail of the last wave
-    work = (seg[:, 3] - seg[:, 2]) * max_cols
+    if tc:
+        slots = torch.zeros(R, dtype=torch.int64, device=dev).index_add_(0, run_row, run_hi - run_lo)
+        work = slots[seg_grp]
+    else:
+        work = (seg[:, 3] - seg[:, 2]) * max_cols
     seg = seg[torch.argsort(work, descending=True, stable=True)].to(torch.int32).contiguous()
     if pieces.shape[0] == 0:
         pieces = torch.zeros(1, 2, dtype=torch.int32, device=dev)
-    return RangesProblem(seg, pieces, layout, variant, int(row_off[-1].item()), density)
+    if not tc:
+        return RangesProblem(seg, pieces, layout, variant, int(row_off[-1].item()), density)
+    # the tensor-core entries read the descriptors on the host
+    computed = float((slots.double() * max_rows * n_seg_r.double()).sum().item()) / max(pairs_all, 1.0)
+    return RangesProblem(seg.cpu(), pieces.cpu(), layout, variant, int(row_off[-1].item()), density,
+                         row_layout=row_layout, computed=computed)
 
 
 def batch_problem(B, N, M, device, variant=None):
@@ -146,11 +185,26 @@ def batch_problem(B, N, M, device, variant=None):
 # ------------------------------------------------------------------------------------------------------
 # softmin
 # ------------------------------------------------------------------------------------------------------
+def _check_path(prob, D):
+    """A problem is built for one family of kernels: CUDA-core ranges (BIG / SMALL, D <= 8) or tensor-core blocks
+    (TC, 8 < D <= 64).  The other one refuses it."""
+    if prob.variant == TC:
+        if not ops.MAX_D < D <= ops.MAX_D_TC:
+            raise ValueError(f"a tensor-core block problem (variant TC) serves {ops.MAX_D} < D <= {ops.MAX_D_TC}, "
+                             f"got D = {D}")
+    elif D > ops.MAX_D:
+        raise ValueError(f"a ranges problem (variant BIG / SMALL) serves D <= {ops.MAX_D}, got D = {D}: build it with "
+                         "variant=ranges.TC and ColumnLayout(counts, align=128)")
+
+
 def softmin_shard_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None, part=None):
     """pack (gather) + partial reduction: the (N, 2) (m, s) partials of this problem's pieces."""
     x, y, h_a, h_b, center = (ops._f32c(t, n) for t, n in ((x, "x"), (y, "y"), (h_a, "h_a"), (h_b, "h_b"),
                                                            (center, "center")))
     N, D = x.shape
+    _check_path(prob, D)
+    if prob.variant == TC:
+        raise ValueError("tensor-core block problems run as one call (softmin_ranges_raw), without exposed partials")
     if N != prob.n_rows or y.shape[0] != prob.layout.n_cols:
         raise ValueError("point clouds do not match the ranges problem they are reduced with")
     dev = x.device
@@ -186,8 +240,71 @@ def softmin_finalize(parts, n_part, eps, out_old, alpha_old, beta, want_lse2, ou
     return out, lse2
 
 
+def _blocks_args(prob, x, y):
+    """Shared arguments of the b200ot_*_blocks entries: row / column gather and the host descriptors."""
+    N, D = x.shape
+    if N != prob.n_rows or y.shape[0] != prob.layout.n_cols:
+        raise ValueError("point clouds do not match the block problem they are reduced with")
+    rl, cl = prob.row_layout, prob.layout
+    nbytes = prob._scratch_bytes.get(D)
+    if nbytes is None:
+        nbytes = _lib.lib().b200ot_blocks_scratch_bytes(N, rl.n_slots, cl.n_slots, ops._ptr(prob.seg), prob.n_seg,
+                                                        ops._ptr(prob.pieces), D)
+        if nbytes <= 0:
+            raise ValueError("invalid tensor-core block problem")
+        prob._scratch_bytes[D] = nbytes
+    return (N, ops._ptr(rl.src), rl.n_slots, ops._ptr(cl.src), cl.n_slots, ops._ptr(prob.seg), prob.n_seg,
+            ops._ptr(prob.pieces), D), nbytes
+
+
+def softmin_blocks_raw(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None, out_old=None, alpha_old=0.0,
+                       beta=1.0, want_lse2=False, out=None):
+    """One block-sparse softmin on the tensor cores (8 < D <= 64): pack + reduction + finalize in one C call."""
+    x, y, h_a, h_b, center, out_old = (ops._f32c(t, n) for t, n in ((x, "x"), (y, "y"), (h_a, "h_a"), (h_b, "h_b"),
+                                                                    (center, "center"), (out_old, "out_old")))
+    _check_path(prob, x.shape[1])
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        (N, *rest), nbytes = _blocks_args(prob, x, y)
+        if out is None:
+            out = torch.empty(N, dtype=torch.float32, device=dev)
+        lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
+        scratch = ops._scratch(nbytes, dev, "blocks")
+        _lib.check(L.b200ot_softmin_fwd_blocks(ops._ptr(x), ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b),
+                                               float(h_scale_b), ops._ptr(center), ops._ptr(out_old),
+                                               float(alpha_old), float(beta), ops._ptr(out), ops._ptr(lse2), N, *rest,
+                                               int(p), float(eps), ops._ptr(scratch), nbytes, ops._stream(dev)),
+                   "b200ot_softmin_fwd_blocks")
+    ops.count_launches(4)
+    return out, lse2
+
+
+def softmin_blocks_bwd_x(eps, x, y, h_a, h_b, h_scale_b, prob, lse2, grad_out, *, p=2, center=None):
+    x, y, h_a, h_b, center, lse2, grad_out = (
+        ops._f32c(t, n) for t, n in ((x, "x"), (y, "y"), (h_a, "h_a"), (h_b, "h_b"), (center, "center"),
+                                     (lse2, "lse2"), (grad_out, "grad_out")))
+    _check_path(prob, x.shape[1])
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        (N, *rest), nbytes = _blocks_args(prob, x, y)
+        gx = torch.empty_like(x)
+        scratch = ops._scratch(nbytes, dev, "blocks")
+        _lib.check(L.b200ot_softmin_bwd_x_blocks(ops._ptr(x), ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b),
+                                                 float(h_scale_b), ops._ptr(center), ops._ptr(lse2),
+                                                 ops._ptr(grad_out), ops._ptr(gx), N, *rest, int(p), float(eps),
+                                                 ops._ptr(scratch), nbytes, ops._stream(dev)),
+                   "b200ot_softmin_bwd_x_blocks")
+    ops.count_launches(4)
+    return gx
+
+
 def softmin_ranges_raw(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None, out_old=None, alpha_old=0.0,
                        beta=1.0, want_lse2=False, out=None):
+    if x.shape[1] > ops.MAX_D:
+        return softmin_blocks_raw(eps, x, y, h_a, h_b, h_scale_b, prob, p=p, center=center, out_old=out_old,
+                                  alpha_old=alpha_old, beta=beta, want_lse2=want_lse2, out=out)
     part = softmin_shard_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, p=p, center=center)
     return softmin_finalize(part, 1, eps, out_old, alpha_old, beta, want_lse2, out=out)
 
@@ -197,6 +314,9 @@ def softmin_bwd_shard_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, lse2, *, p=2,
     x, y, h_a, h_b, center, lse2 = (ops._f32c(t, n) for t, n in ((x, "x"), (y, "y"), (h_a, "h_a"), (h_b, "h_b"),
                                                                  (center, "center"), (lse2, "lse2")))
     N, D = x.shape
+    _check_path(prob, D)
+    if prob.variant == TC:
+        raise ValueError("tensor-core block problems run as one call (softmin_blocks_bwd_x), without exposed sums")
     dev = x.device
     L = _lib.lib()
     lay = prob.layout
@@ -249,6 +369,10 @@ class _RangesSoftmin(torch.autograd.Function):
         x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
         h_scale_b, eps, p, scale_out, prob, has_hb, has_center = ctx.meta
         center = center if has_center else None
+        if prob.variant == TC:
+            gx = softmin_blocks_bwd_x(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, prob, lse2,
+                                      (grad_out * scale_out).contiguous(), p=p, center=center)
+            return gx, None, None, None, None, None, None, None, None, None
         sums = softmin_bwd_shard_ranges(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, prob, lse2, p=p,
                                         center=center)
         gx = softmin_bwd_finalize(sums, eps, x, center, (grad_out * scale_out).contiguous(), p)

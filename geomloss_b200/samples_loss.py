@@ -14,7 +14,11 @@ the dense path).  "tensorized" and "online" are ONE engine — the never-materia
 exactly — and differ only where the reference's two backends differ numerically: for p = 1 / laplacian / energy
 "tensorized" clamps |x-y|^2 at 1e-8 under the square root (utils.py:56-61) while "online" and "multiscale" use the
 pykeops norm (no clamp).  "multiscale" is the two-scale Sinkhorn with kernel truncation / the truncated kernel
-norms (multiscale.py) on the ranges mode of the same kernels, with exactly the reference's cluster blocks.
+norms (multiscale.py) on the ranges mode of the same kernels, with exactly the reference's cluster blocks.  With
+explicit labels for both clouds (the 6-tensor call form) the two-scale Sinkhorn also runs for 3 < D <= 64, like the
+reference, whose ``clusterize`` takes labels in any dimension: the CUDA-core ranges kernels up to D = 8, the
+tensor-core block-sparse softmins above (p = 2; p = 1 above D = 8 raises NotImplementedError).  Column-sharded
+multi-GPU engines keep the single-scale route for such calls.
 Batched inputs (B, N, D) run as ONE launch group per reduction for the whole batch: a block-diagonal ranges problem
 for D <= 8 (ranges.py), the batched tensor-core operators for 8 < D <= 64 (ops.softmin_batched / kernel_conv_batched;
 Sinkhorn with p = 2 only: p = 1 above D = 8 raises NotImplementedError, batched or not).  Column-sharded multi-GPU
@@ -130,7 +134,10 @@ class SamplesLoss(Module):
                 F, G = values
                 return F.view_as(a), G.view_as(b)
             return values if B == 0 else values.view(-1)
-        if backend == "multiscale" and self.loss == "sinkhorn" and D <= 3:
+        # user labels above D = 3 (the voxel grid stops there): the two-scale Sinkhorn on one GPU, up to D = 64
+        labelled = (l_x is not None and l_y is not None and D <= MAX_D_TC and not self._engine
+                    and self._multiscale_engine is None)
+        if backend == "multiscale" and self.loss == "sinkhorn" and (D <= 3 or labelled):
             # single problem (B == 0, or B == 1 squeezed like the reference does, samples_loss.py:249-251)
             sq = (lambda t: t[0]) if B == 1 else (lambda t: t)
             values = sinkhorn_multiscale(sq(a), sq(x), sq(b), sq(y), p=self.p, blur=self.blur, reach=self.reach,

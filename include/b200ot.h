@@ -252,6 +252,47 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float*
                                                     int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
                                                     void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Block-sparse softmins in the tensor-core dimensions (8 < D <= 64, p = 2 or 2 | B200OT_P_UNCLAMPED): the fine phase
+ * of the two-scale Sinkhorn with user cluster labels (sinkhorn_multiscale, sinkhorn_samples.py:547-681), the
+ * counterpart of the ranges entries above, which serve D <= B200OT_MAX_D.  A separate family with its own layout:
+ *   slots     every row cluster and every column cluster is padded to whole tiles of `col_align` (128) points on its
+ *             own; row slot r holds row row_src[r] of x, column slot s column col_src[s] of y (-1: padding, a neutral
+ *             column / a row that writes nothing).  row_src (n_row_slots) and col_src (n_col_slots) are device arrays;
+ *   segment   one tile of `rows_per_segment` (128) row slots of one row cluster: row_start = the first slot (a multiple
+ *             of 128), row_count = its live rows (1..128), [piece_begin, piece_end) its pieces.  Exactly one segment per
+ *             row tile (n_seg = n_row_slots / 128); launch order = array order, so list the heaviest first;
+ *   piece     (col_start, col_count): a run of whole column tiles (both multiples of 128);
+ *   seg, pieces are HOST arrays (16- / 8-byte aligned).  Every call validates them and copies them into the scratch on
+ *             `stream` (from pageable memory that copy waits for the stream's earlier work).
+ * Each row is reduced over exactly the columns of its segment's pieces.  Results are indexed by row (x, lse2, out,
+ * grad_x: N rows), h_a / h_b by column of y.  The column tiles of a segment are cut into splits like a dense problem's
+ * ($B200OT_FORCE_SPLITS applies); the row gradients run the default variant of the row-gradient kernel.
+ * EINVAL (before any launch) for null pointers, N <= 0, n_seg <= 0, D <= 8 or D > 64, p other than 2, and descriptors
+ * off the tile grid; EALIGN for misaligned descriptor arrays or scratch; ESCRATCH below b200ot_blocks_scratch_bytes
+ * (0 for invalid descriptors).
+ * ------------------------------------------------------------------------------------------- */
+B200OT_API void b200ot_blocks_shape(int32_t* rows_per_segment, int32_t* col_align);
+B200OT_API int64_t b200ot_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots,
+                                               const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
+                                               int32_t D);
+/* b200ot_softmin_fwd on the listed blocks: out, lse2_out (N), out_old, alpha_old, beta as there */
+B200OT_API int b200ot_softmin_fwd_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
+                                         float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                         float beta, float* out, float* lse2_out, int64_t N, const int32_t* row_src,
+                                         int64_t n_row_slots, const int32_t* col_src, int64_t n_col_slots,
+                                         const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
+                                         int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                         void* stream);
+/* b200ot_softmin_bwd_x on the listed blocks (lse2: the forward's) */
+B200OT_API int b200ot_softmin_bwd_x_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
+                                           float h_scale_b, const float* center, const float* lse2,
+                                           const float* grad_out, float* grad_x, int64_t N, const int32_t* row_src,
+                                           int64_t n_row_slots, const int32_t* col_src, int64_t n_col_slots,
+                                           const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
+                                           int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                           void* stream);
+
 /* --- stages of the CUDA-core kernel convolutions (D <= B200OT_MAX_D), ranges mode: truncated block-sparse
  *     MMDs (kernel_multiscale, kernel_samples.py:177-271) and batched problems.  cols: gather-packed,
  *     b200ot_packed_cols_floats(n_slots, D, 2) floats.  part: (N) sums (backward = 0) or (N, width) sums

@@ -30,7 +30,7 @@ def check(name, got, ref, tol=2e-5):
     assert err < tol, name
 
 
-which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "grid", "loss"}
+which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "blocks", "grid", "loss"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -154,6 +154,35 @@ if "batched" in which:
         val, gu = ops.kernel_conv_batched_value_and_grad_rows(0, xd, yd, wd, 2.0, center=center)
         check(f"batched_conv_value_d{d}", val, ((-d2 / 8.0).exp() @ w.double()[:, :, None])[..., 0], 1e-4)
         assert torch.isfinite(gu).all()
+if "blocks" in which:
+    # the block-sparse tensor-core softmins (tc_reduce_kernel<1, false, BLOCKS>, tc_bwd_kernel<3, 2, true, dk, false,
+    # BLOCKS>): clusters of 1, 127, 128, 129 and 300 points, a row cluster that keeps nothing, a self problem
+    for d in (16, 64):
+        rc, cc = torch.tensor([1, 129, 300, 128]), torch.tensor([127, 1, 300, 129, 128])
+        keep = torch.rand(4, 5, generator=g) < 0.6
+        keep[0], keep[1] = True, False
+        prob = ranges.build_problem(keep.to(DEV), rc.to(DEV), ranges.ColumnLayout(cc.to(DEV), align=128),
+                                    variant=ranges.TC)
+        x, y, h = torch.rand(int(rc.sum()), d, generator=g), torch.rand(int(cc.sum()), d, generator=g), torch.randn(
+            int(cc.sum()), generator=g)
+        xg = x.to(DEV).requires_grad_(True)
+        out = ranges.softmin_ranges(1.0, xg, y.to(DEV), h.to(DEV), None, 0.0, prob)
+        mask = keep[torch.repeat_interleave(torch.arange(4), rc)][:, torch.repeat_interleave(torch.arange(5), cc)]
+        d2 = ((x[:, None, :].double() - y[None, :, :].double()) ** 2).sum(-1) / 2
+        ref = -torch.logsumexp((h.double()[None, :] - d2).masked_fill(~mask, -float("inf")), dim=1)
+        live = mask.any(1)
+        check(f"blocks_softmin_d{d}", out[live.to(DEV)], ref[live].float(), 1e-4)
+        (gx,) = torch.autograd.grad(out[live.to(DEV)].sum(), xg)
+        assert torch.isfinite(gx).all()
+        kxx = torch.rand(4, 4, generator=g) < 0.5
+        kxx[torch.arange(4), torch.arange(4)] = True
+        pxx = ranges.build_problem(kxx.to(DEV), rc.to(DEV), ranges.ColumnLayout(rc.to(DEV), align=128),
+                                   variant=ranges.TC)
+        hx = torch.randn(int(rc.sum()), generator=g).to(DEV)
+        sxx = ranges.softmin_ranges(1.0, xg, xg.detach(), hx, None, 0.0, pxx)
+        (gx,) = torch.autograd.grad(sxx.sum(), xg)
+        assert torch.isfinite(sxx).all() and torch.isfinite(gx).all()
+        print(f"blocks_self_d{d} ok")
 if "grid" in which:
     for shape in ((1, 2, 32, 32), (1, 1, 16, 16, 16), (1, 1, 1024, 1024)):
         h = torch.randn(*shape, generator=g)
