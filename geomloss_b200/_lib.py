@@ -81,12 +81,12 @@ _SIGNATURES = {
     "b200ot_softmin_bwd_x_blocks": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, _P, _P, c_int64, _P, c_int64, _P,
                                               c_int64, _P, c_int64, _P, c_int32, c_int32, c_float, _P, c_int64, _P]),
     "b200ot_sinkhorn_iteration_small": (c_int32, [_P] * 13 + [c_int64, c_int64, c_int64, c_int32, c_int32, c_float,
-                                                  c_float, c_float, c_int32, _P]),
+                                                  c_float, c_float, c_int32, _P, _P]),
     "b200ot_sinkhorn_loop_small": (c_int32, [_P, _P, _P, _P, c_int32, ctypes.POINTER(ctypes.c_double), c_int32,
                                              ctypes.c_double, c_int32, _P, _P, ctypes.POINTER(c_int32), c_int64,
-                                             c_int64, c_int64, c_int32, c_int32, _P]),
+                                             c_int64, c_int64, c_int32, c_int32, _P, _P]),
     "b200ot_sinkhorn_final_bwd_small": (c_int32, [_P] * 15 + [c_int64, c_int64, c_int64, c_int32, c_int32, c_float,
-                                                  c_float, _P, c_int32, _P]),
+                                                  c_float, _P, c_int32, _P, _P]),
     "b200ot_sinkhorn_cost_small": (c_int32, [_P] * 6 + [c_int64, c_int64, c_int64, c_float, c_float] + [_P] * 8),
     "b200ot_kernel_mmd_value_small": (c_int32, [_P] * 5 + [c_int64, c_int64, c_int64, _P, _P]),
     "b200ot_cloud_extent_scratch_bytes": (c_int64, []),

@@ -46,8 +46,18 @@ struct SmallProblemSet {
   const float* lse2_in[4];   // backward: saved lse2 of the forward final step
   const float* gout[4];      // backward: upstream gradient per row (nullable = zero)
   const float* go_scale;     // backward: per-batch-element factor on every gout (nullable = 1)
+  const float* lo_hi;        // (2, D) bounding box of the batch: coordinates are taken from its mid-point (nullable)
   int nrows[4], ncols[4];
 };
+
+// Mid-point of the bounding box, subtracted from every coordinate before the scaling, as the tiled kernels do: the
+// scaled differences then keep the bits of clouds that lie far from the origin (x - c is exact when x and c agree
+// to within a factor of two, the rounded product of a large coordinate is not)
+template <int D>
+__device__ __forceinline__ void box_centre(const float* __restrict__ lo_hi, float (&C)[D]) {
+#pragma unroll
+  for (int d = 0; d < D; ++d) C[d] = lo_hi ? 0.5f * (lo_hi[d] + lo_hi[D + d]) : 0.f;
+}
 
 // Scaled coordinates are ROUNDED products (__fmul_rn is never contracted).  With a plain `scale * x` the compiler fuses
 // the row side into the difference, df = fma(x, scale, -Y), while the column side Y = round(scale * y) went through
@@ -98,9 +108,10 @@ __global__ void __launch_bounds__(WARPS * 32)
   const float* __restrict__ pot = S.pot[q] ? S.pot[q] + (int64_t)b * ncols : nullptr;
 
   const int i = min(row0 + lane, nrows - 1);
-  float X[D];
+  float X[D], C[D];
+  box_centre<D>(S.lo_hi, C);
 #pragma unroll
-  for (int d = 0; d < D; ++d) X[d] = __fmul_rn(scale, rows[(int64_t)i * D + d]);  // (never contracted: see scaled_coord)
+  for (int d = 0; d < D; ++d) X[d] = __fmul_rn(scale, rows[(int64_t)i * D + d] - C[d]);  // (never contracted: see above)
 
   float m = kNegBig, s = 0.f;
   for (int j0 = 0; j0 < ncols; j0 += kSmallTile) {
@@ -111,7 +122,7 @@ __global__ void __launch_bounds__(WARPS * 32)
       if (e < nt) {
         const int j = j0 + e;
 #pragma unroll
-        for (int d = 0; d < D; ++d) dst[d] = __fmul_rn(scale, cols[(int64_t)j * D + d]);
+        for (int d = 0; d < D; ++d) dst[d] = __fmul_rn(scale, cols[(int64_t)j * D + d] - C[d]);
         float h = column_log2_weight(logw[j], w_linear);
         if (pot) h = fmaf(pot[j], inv_eps_log2e, h);
         dst[D] = h;
@@ -184,10 +195,11 @@ __global__ void __launch_bounds__(kSmallWarps * 32)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const float* __restrict__ rows = S.rows[side] + (int64_t)b * nrows * D;
   const int i = min(row0 + lane, nrows - 1);
-  float X[D], G[D];
+  float X[D], G[D], C[D];
+  box_centre<D>(S.lo_hi, C);
 #pragma unroll
   for (int d = 0; d < D; ++d) {
-    X[d] = __fmul_rn(scale, rows[(int64_t)i * D + d]);  // (never contracted: see scaled_coord)
+    X[d] = __fmul_rn(scale, rows[(int64_t)i * D + d] - C[d]);  // (never contracted: see scaled_coord)
     G[d] = 0.f;
   }
   for (int term = 0; term < n_terms; ++term) {
@@ -212,7 +224,7 @@ __global__ void __launch_bounds__(kSmallWarps * 32)
         if (e < nt) {
           const int j = j0 + e;
 #pragma unroll
-          for (int d = 0; d < D; ++d) dst[d] = __fmul_rn(scale, cols[(int64_t)j * D + d]);
+          for (int d = 0; d < D; ++d) dst[d] = __fmul_rn(scale, cols[(int64_t)j * D + d] - C[d]);
           float h = column_log2_weight(logw[j], w_linear);
           if (pot) h = fmaf(pot[j], inv_eps_log2e, h);
           dst[D] = h;
@@ -332,6 +344,45 @@ static int launch_bwd(int pe, const SmallProblemSet& S, dim3 grid, float scale, 
     default: return B200OT_EINVAL;            \
   }
 
+// The batch is gridDim.z of the small kernels, at most 65535 elements per launch: a larger batch runs as consecutive
+// launches over slices of it.  launch(b0, nb) enqueues the elements [b0, b0 + nb), every per-element array offset to b0.
+constexpr int64_t kMaxGridZ = 65535;
+constexpr int64_t kMaxGridX = 0x7fffffff;  // the cost kernels: one block per batch element, gridDim.x
+
+template <class F>
+static int for_batch_slices(int64_t B, F&& launch) {
+  for (int64_t b0 = 0; b0 < B; b0 += kMaxGridZ) {
+    const int rc = launch(b0, B - b0 < kMaxGridZ ? B - b0 : kMaxGridZ);
+    if (rc != B200OT_OK) return rc;
+  }
+  return B200OT_OK;
+}
+
+template <class T>
+static T* skip(T* p, int64_t n) {
+  return p ? p + n : p;
+}
+
+// the problems of batch elements [b0, B) of S (lse2 / lse2_in point into their own [f_ba | g_ab | f_aa | g_bb] block,
+// whose offsets already account for the whole batch)
+static SmallProblemSet batch_slice(const SmallProblemSet& S, int64_t b0, int D) {
+  SmallProblemSet T = S;
+  for (int q = 0; q < 4; ++q) {
+    const int64_t r = b0 * S.nrows[q], c = b0 * S.ncols[q];
+    T.rows[q] = skip(S.rows[q], r * D);
+    T.cols[q] = skip(S.cols[q], c * D);
+    T.logw[q] = skip(S.logw[q], c);
+    T.pot[q] = skip(S.pot[q], c);
+    T.old[q] = skip(S.old[q], r);
+    T.out[q] = skip(S.out[q], r);
+    T.lse2[q] = skip(S.lse2[q], r);
+    T.lse2_in[q] = skip(S.lse2_in[q], r);
+    T.gout[q] = skip(S.gout[q], r);
+  }
+  T.go_scale = skip(S.go_scale, b0);
+  return T;
+}
+
 static void fill_problems(SmallProblemSet& S, const float* x, const float* y, const float* a_log, const float* b_log,
                           const float* f_ba, const float* g_ab, const float* f_aa, const float* g_bb, int N, int M) {
   const float* rows[4] = {x, y, x, y};
@@ -353,6 +404,7 @@ static void fill_problems(SmallProblemSet& S, const float* x, const float* y, co
     S.gout[q] = nullptr;
   }
   S.go_scale = nullptr;
+  S.lo_hi = nullptr;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -726,8 +778,8 @@ B200OT_API int b200ot_sinkhorn_iteration_small(const float* x, const float* y, c
                                                const float* g_bb, float* f_ba_out, float* g_ab_out, float* f_aa_out,
                                                float* g_bb_out, float* lse2_out, int64_t B, int64_t N, int64_t M,
                                                int32_t D, int32_t p, float eps, float alpha_old, float beta,
-                                               int32_t weights_linear, void* stream) {
-  if (!x || !y || !a_log || !b_log || !f_ba_out || !g_ab_out || B <= 0 || N <= 0 || M <= 0 || B > 65535 ||
+                                               int32_t weights_linear, const float* lo_hi, void* stream) {
+  if (!x || !y || !a_log || !b_log || !f_ba_out || !g_ab_out || B <= 0 || N <= 0 || M <= 0 ||
       N > B200OT_SMALL_MAX_POINTS || M > B200OT_SMALL_MAX_POINTS || !supported_simt_dim(D) || !valid_p(p) ||
       !(eps > 0.f) || ((f_aa_out == nullptr) != (g_bb_out == nullptr)))
     return B200OT_EINVAL;
@@ -738,6 +790,7 @@ B200OT_API int b200ot_sinkhorn_iteration_small(const float* x, const float* y, c
   if (has_old && debias && (!f_aa || !g_bb)) return B200OT_EINVAL;
   SmallProblemSet S;
   fill_problems(S, x, y, a_log, b_log, f_ba, g_ab, f_aa, g_bb, (int)N, (int)M);
+  S.lo_hi = lo_hi;
   const float* old[4] = {f_ba, g_ab, f_aa, g_bb};
   float* out[4] = {f_ba_out, g_ab_out, f_aa_out, g_bb_out};
   for (int q = 0; q < 4; ++q) {
@@ -750,12 +803,15 @@ B200OT_API int b200ot_sinkhorn_iteration_small(const float* x, const float* y, c
   const float scale = softmin_coord_scale(pe, eps);
   const float clampq = scale * scale * cost_clamp(p);
   const int64_t tiles = ceil_div64(N > M ? N : M, kSmallRows);
-  dim3 grid((unsigned)tiles, debias ? 4u : 2u, (unsigned)B);
   const float bneg = -beta * eps * kLn2;
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(DD) launch_iter<DD>(pe, S, grid, scale, kLog2e / eps, clampq, alpha_old, bneg, weights_linear, st)
-  B200OT_DISPATCH_D(D, CALL)
+  return for_batch_slices(B, [&](int64_t b0, int64_t nb) {
+    const SmallProblemSet T = batch_slice(S, b0, D);
+    const dim3 grid((unsigned)tiles, debias ? 4u : 2u, (unsigned)nb);
+#define CALL(DD) launch_iter<DD>(pe, T, grid, scale, kLog2e / eps, clampq, alpha_old, bneg, weights_linear, st)
+    B200OT_DISPATCH_D(D, CALL)
 #undef CALL
+  });
 }
 
 B200OT_API int b200ot_sinkhorn_final_bwd_small(const float* x, const float* y, const float* a_log, const float* b_log,
@@ -764,8 +820,9 @@ B200OT_API int b200ot_sinkhorn_final_bwd_small(const float* x, const float* y, c
                                                const float* go_g_ab, const float* go_f_aa, const float* go_g_bb,
                                                float* grad_x, float* grad_y, int64_t B, int64_t N, int64_t M,
                                                int32_t D, int32_t p, float eps, float scale_out,
-                                               const float* go_scale, int32_t weights_linear, void* stream) {
-  if (!x || !y || !a_log || !b_log || !lse2 || !grad_x || !grad_y || B <= 0 || N <= 0 || M <= 0 || B > 65535 ||
+                                               const float* go_scale, int32_t weights_linear, const float* lo_hi,
+                                               void* stream) {
+  if (!x || !y || !a_log || !b_log || !lse2 || !grad_x || !grad_y || B <= 0 || N <= 0 || M <= 0 ||
       N > B200OT_SMALL_MAX_POINTS || M > B200OT_SMALL_MAX_POINTS || !supported_simt_dim(D) || !valid_p(p) ||
       !(eps > 0.f))
     return B200OT_EINVAL;
@@ -778,24 +835,29 @@ B200OT_API int b200ot_sinkhorn_final_bwd_small(const float* x, const float* y, c
     S.lse2_in[q] = lse2 + off[q];
   }
   S.go_scale = go_scale;
+  S.lo_hi = lo_hi;
   const int n_terms = (go_f_aa || go_g_bb) ? 2 : 1;
   const int pe = p_exponent(p);
   const float scale = softmin_coord_scale(pe, eps);
   const float clampq = scale * scale * cost_clamp(p);
   const int64_t tiles = ceil_div64(N > M ? N : M, kSmallRows);
-  dim3 grid((unsigned)tiles, 2u, (unsigned)B);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(DD) \
-  launch_bwd<DD>(pe, S, grid, scale, kLog2e / eps, clampq, scale_out, grad_x, grad_y, n_terms, weights_linear, st)
-  B200OT_DISPATCH_D(D, CALL)
+  return for_batch_slices(B, [&](int64_t b0, int64_t nb) {
+    const SmallProblemSet T = batch_slice(S, b0, D);
+    float* gx = grad_x + b0 * N * D;
+    float* gy = grad_y + b0 * M * D;
+    const dim3 grid((unsigned)tiles, 2u, (unsigned)nb);
+#define CALL(DD) launch_bwd<DD>(pe, T, grid, scale, kLog2e / eps, clampq, scale_out, gx, gy, n_terms, weights_linear, st)
+    B200OT_DISPATCH_D(D, CALL)
 #undef CALL
+  });
 }
 
 B200OT_API int b200ot_sinkhorn_cost_small(const float* a, const float* b, const float* f_ba, const float* g_ab,
                                           const float* f_aa, const float* g_bb, int64_t B, int64_t N, int64_t M,
                                           float rho, float eps, float* value, float* go_f_ba, float* go_g_ab,
                                           float* go_f_aa, float* go_g_bb, float* phi, float* psi, void* stream) {
-  if (!a || !b || !f_ba || !g_ab || !value || B <= 0 || N <= 0 || M <= 0 || B > 65535 ||
+  if (!a || !b || !f_ba || !g_ab || !value || B <= 0 || N <= 0 || M <= 0 || B > kMaxGridX ||
       N > B200OT_SMALL_MAX_POINTS || M > B200OT_SMALL_MAX_POINTS || (f_aa == nullptr) != (g_bb == nullptr))
     return B200OT_EINVAL;
   SmallCostSet S;
@@ -816,7 +878,7 @@ B200OT_API int b200ot_sinkhorn_cost_small(const float* a, const float* b, const 
 B200OT_API int b200ot_kernel_mmd_value_small(const float* a, const float* b, const float* a_x, const float* b_y,
                                              const float* b_x, int64_t B, int64_t N, int64_t M, float* value,
                                              void* stream) {
-  if (!a || !b || !a_x || !b_y || !b_x || !value || B <= 0 || N <= 0 || M <= 0 || B > 65535 ||
+  if (!a || !b || !a_x || !b_y || !b_x || !value || B <= 0 || N <= 0 || M <= 0 || B > kMaxGridX ||
       N > B200OT_SMALL_MAX_POINTS || M > B200OT_SMALL_MAX_POINTS)
     return B200OT_EINVAL;
   // 1/2 <a, a_x> + 1/2 <b, b_y> - <a, b_x>  =  <a, 1/2 a_x - b_x> + <b, 1/2 b_y>: coefficients (1/2, 1), the `self` slot
@@ -855,7 +917,8 @@ B200OT_API int b200ot_cloud_extent(const float* x, int64_t n, const float* y, in
 B200OT_API int b200ot_sinkhorn_loop_small(const float* x, const float* y, const float* a, const float* b,
                                           int32_t weights_linear, const double* eps_list, int32_t n_eps, double rho,
                                           int32_t debias, float* pots_a, float* pots_b, int32_t* result_in_a,
-                                          int64_t B, int64_t N, int64_t M, int32_t D, int32_t p, void* stream) {
+                                          int64_t B, int64_t N, int64_t M, int32_t D, int32_t p,
+                                          const float* lo_hi, void* stream) {
   if (!eps_list || n_eps <= 0 || !pots_a || !pots_b || !result_in_a || pots_a == pots_b) return B200OT_EINVAL;
   auto view = [&](float* base, float** f_ba, float** g_ab, float** f_aa, float** g_bb) {
     *f_ba = base;
@@ -871,7 +934,7 @@ B200OT_API int b200ot_sinkhorn_loop_small(const float* x, const float* y, const 
   // initialisation at the first temperature (sinkhorn_divergence.py:461-465): h = log-weights only
   int rc = b200ot_sinkhorn_iteration_small(x, y, a, b, nullptr, nullptr, nullptr, nullptr, c0, c1, c2, c3, nullptr, B, N, M,
                                            D, p, (float)eps_list[0], 0.f, (float)damp(eps_list[0]), weights_linear,
-                                           stream);
+                                           lo_hi, stream);
   if (rc) return rc;
   // eps-scaling descent (:468-493): symmetric, averaged updates
   for (int i = 0; i < n_eps; ++i) {
@@ -879,7 +942,7 @@ B200OT_API int b200ot_sinkhorn_loop_small(const float* x, const float* y, const 
     view(cur, &c0, &c1, &c2, &c3);
     view(nxt, &n0, &n1, &n2, &n3);
     rc = b200ot_sinkhorn_iteration_small(x, y, a, b, c0, c1, c2, c3, n0, n1, n2, n3, nullptr, B, N, M, D, p, (float)eps,
-                                         0.5f, (float)(0.5 * damp(eps)), weights_linear, stream);
+                                         0.5f, (float)(0.5 * damp(eps)), weights_linear, lo_hi, stream);
     if (rc) return rc;
     float* t = cur;
     cur = nxt;
@@ -893,7 +956,7 @@ B200OT_API int b200ot_kernel_mmd_small(const float* x, const float* y, const flo
                                        float* b_y, float* b_x, float* a_y, int64_t B, int64_t N, int64_t M, int32_t D,
                                        int32_t kind, float blur, void* stream) {
   const int kb = kind & 0xff;
-  if (!x || !y || !a || !b || !a_x || !b_y || !b_x || B <= 0 || N <= 0 || M <= 0 || B > 65535 ||
+  if (!x || !y || !a || !b || !a_x || !b_y || !b_x || B <= 0 || N <= 0 || M <= 0 ||
       N > B200OT_SMALL_MAX_POINTS || M > B200OT_SMALL_MAX_POINTS || !supported_simt_dim(D) || kb < 0 || kb > 2 ||
       (kind & ~(0xff | B200OT_KERNEL_UNCLAMPED)) != 0 || (kb != B200OT_KERNEL_ENERGY && !(blur > 0.f)))
     return B200OT_EINVAL;
@@ -913,18 +976,28 @@ B200OT_API int b200ot_kernel_mmd_small(const float* x, const float* y, const flo
   }
   float scale, clampq;
   mmd_scales(kind, blur, &scale, &clampq);
-  dim3 grid((unsigned)ceil_div64(N > M ? N : M, kSmallRows), a_y ? 4u : 3u, (unsigned)B);
+  const int64_t tiles = ceil_div64(N > M ? N : M, kSmallRows);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(DD) launch_mmd<DD>(kb, S, grid, scale, clampq, st)
-  B200OT_DISPATCH_D(D, CALL)
+  return for_batch_slices(B, [&](int64_t b0, int64_t nb) {
+    SmallConvSet T = S;
+    for (int q = 0; q < 4; ++q) {
+      T.rows[q] = S.rows[q] + b0 * S.nrows[q] * D;
+      T.cols[q] = S.cols[q] + b0 * S.ncols[q] * D;
+      T.w[q] = S.w[q] + b0 * S.ncols[q];
+      T.out[q] = skip(S.out[q], b0 * S.nrows[q]);
+    }
+    const dim3 grid((unsigned)tiles, a_y ? 4u : 3u, (unsigned)nb);
+#define CALL(DD) launch_mmd<DD>(kb, T, grid, scale, clampq, st)
+    B200OT_DISPATCH_D(D, CALL)
 #undef CALL
+  });
 }
 
 B200OT_API int b200ot_kernel_mmd_bwd_small(const float* x, const float* y, const float* a, const float* b,
                                            const float* grad_value, float* grad_x, float* grad_y, int64_t B, int64_t N,
                                            int64_t M, int32_t D, int32_t kind, float blur, void* stream) {
   const int kb = kind & 0xff;
-  if (!x || !y || !a || !b || !grad_value || !grad_x || !grad_y || B <= 0 || N <= 0 || M <= 0 || B > 65535 ||
+  if (!x || !y || !a || !b || !grad_value || !grad_x || !grad_y || B <= 0 || N <= 0 || M <= 0 ||
       N > B200OT_SMALL_MAX_POINTS || M > B200OT_SMALL_MAX_POINTS || !supported_simt_dim(D) || kb < 0 || kb > 2 ||
       (kind & ~(0xff | B200OT_KERNEL_UNCLAMPED)) != 0 || (kb != B200OT_KERNEL_ENERGY && !(blur > 0.f)))
     return B200OT_EINVAL;
@@ -944,11 +1017,22 @@ B200OT_API int b200ot_kernel_mmd_bwd_small(const float* x, const float* y, const
   // = -(k (X - Y)/|X - Y|) / blur; energy -(x - y)/|x - y|
   const float coef = kb == B200OT_KERNEL_GAUSSIAN ? -1.0f / (scale * blur * blur)
                                                   : (kb == B200OT_KERNEL_LAPLACIAN ? -1.0f / blur : -1.0f);
-  dim3 grid((unsigned)ceil_div64(N > M ? N : M, kSmallRows), 2u, (unsigned)B);
+  const int64_t tiles = ceil_div64(N > M ? N : M, kSmallRows);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(DD) launch_mmd_bwd<DD>(kb, S, grid, scale, clampq, coef, st)
-  B200OT_DISPATCH_D(D, CALL)
+  return for_batch_slices(B, [&](int64_t b0, int64_t nb) {
+    SmallConvBwd T = S;
+    T.x = x + b0 * N * D;
+    T.y = y + b0 * M * D;
+    T.a = a + b0 * N;
+    T.b = b + b0 * M;
+    T.go = grad_value + b0;
+    T.gx = grad_x + b0 * N * D;
+    T.gy = grad_y + b0 * M * D;
+    const dim3 grid((unsigned)tiles, 2u, (unsigned)nb);
+#define CALL(DD) launch_mmd_bwd<DD>(kb, T, grid, scale, clampq, coef, st)
+    B200OT_DISPATCH_D(D, CALL)
 #undef CALL
+  });
 }
 
 }  // extern "C"

@@ -31,11 +31,16 @@ def max_diameter(x, y):
     """Length of the diagonal of the joint bounding box (one host sync).     sinkhorn_divergence.py:96-112"""
     lh = ops.cloud_extent(x, y)
     if lh is not None:  # one launch + one 2D-float copy; the norm of D numbers is taken on the host
-        lo, hi = lh.cpu().double().unbind(0)
-        return float(torch.sqrt(((hi - lo) ** 2).sum()).float())
+        return extent_diameter(lh)
     lo = torch.minimum(x.min(0).values, y.min(0).values)
     hi = torch.maximum(x.max(0).values, y.max(0).values)
     return (hi - lo).norm().item()
+
+
+def extent_diameter(lh):
+    """Diagonal of a (2, D) [minima; maxima] box from ops.cloud_extent."""
+    lo, hi = lh.cpu().double().unbind(0)
+    return float(torch.sqrt(((hi - lo) ** 2).sum()).float())
 
 
 def epsilon_schedule(p, diameter, blur, scaling):

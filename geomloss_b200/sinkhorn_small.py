@@ -15,7 +15,7 @@ import ctypes
 import torch
 
 from . import _lib, ops
-from .sinkhorn import damping, scaling_parameters, sinkhorn_cost_batched
+from .sinkhorn import damping, extent_diameter, scaling_parameters, sinkhorn_cost_batched
 
 # largest cloud served by the one-launch-per-iteration kernels; beyond, the tiled TMA kernels win
 SMALL_MAX = 6000
@@ -33,7 +33,7 @@ def _views(buf, B, N, M, debias):
     return f_ba, g_ab, buf[B * (N + M): B * (2 * N + M)].view(B, N), buf[B * (2 * N + M):].view(B, M)
 
 
-def _descent(x, y, a, b, eps_list, rho, p, debias):
+def _descent(x, y, a, b, eps_list, rho, p, debias, lh):
     """Initialisation + every eps-scaling step in ONE C call (n_eps + 1 launches enqueued back to back); weights are
     passed as they are, their logarithm (with the reference's -100000 floor) is taken inside the kernel."""
     B, N, D = x.shape
@@ -47,7 +47,7 @@ def _descent(x, y, a, b, eps_list, rho, p, debias):
     with torch.cuda.device(dev):
         rc = L.b200ot_sinkhorn_loop_small(P(x), P(y), P(a), P(b), 1, eps_arr, len(eps_list),
                                           -1.0 if rho is None else float(rho), 1 if debias else 0, P(bufs[0]),
-                                          P(bufs[1]), ctypes.byref(which), B, N, M, D, int(p), ops._stream(dev))
+                                          P(bufs[1]), ctypes.byref(which), B, N, M, D, int(p), P(lh), ops._stream(dev))
     _lib.check(rc, "b200ot_sinkhorn_loop_small")
     ops.count_launches(len(eps_list) + 1)
     return _views(bufs[0] if which.value else bufs[1], B, N, M, debias)
@@ -57,7 +57,7 @@ class _FinalStep(torch.autograd.Function):
     """The last, non-averaged update (sinkhorn_divergence.py:612-623): potentials detached, gradient to x and y only."""
 
     @staticmethod
-    def forward(ctx, x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, p, debias):
+    def forward(ctx, x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, p, debias, lh):
         B, N, D = x.shape
         M = y.shape[1]
         dev = x.device
@@ -70,11 +70,11 @@ class _FinalStep(torch.autograd.Function):
         with torch.cuda.device(dev):
             rc = L.b200ot_sinkhorn_iteration_small(P(x), P(y), P(a), P(b), P(f_ba), P(g_ab), P(f_aa), P(g_bb),
                                                    P(n_f_ba), P(n_g_ab), P(n_f_aa), P(n_g_bb), P(lse2), B, N, M, D,
-                                                   int(p), float(eps), 0.0, float(lam), 1, ops._stream(dev))
+                                                   int(p), float(eps), 0.0, float(lam), 1, P(lh), ops._stream(dev))
         _lib.check(rc, "b200ot_sinkhorn_iteration_small")
         ops.count_launches(1)
         if need:
-            ctx.save_for_backward(x, y, a, b, f_ba, g_ab, f_aa if debias else f_ba, g_bb if debias else g_ab, lse2)
+            ctx.save_for_backward(x, y, a, b, f_ba, g_ab, f_aa if debias else f_ba, g_bb if debias else g_ab, lse2, lh)
             ctx.meta = (float(eps), float(lam), int(p), bool(debias))
         if debias:
             return n_f_ba, n_g_ab, n_f_aa, n_g_bb
@@ -82,7 +82,7 @@ class _FinalStep(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *gos):
-        x, y, a, b, f_ba, g_ab, f_aa, g_bb, lse2 = ctx.saved_tensors
+        x, y, a, b, f_ba, g_ab, f_aa, g_bb, lse2, lh = ctx.saved_tensors
         eps, lam, p, debias = ctx.meta
         B, N, D = x.shape
         M = y.shape[1]
@@ -94,10 +94,10 @@ class _FinalStep(torch.autograd.Function):
             rc = L.b200ot_sinkhorn_final_bwd_small(P(x), P(y), P(a), P(b), P(f_ba), P(g_ab),
                                                    P(f_aa) if debias else None, P(g_bb) if debias else None, P(lse2),
                                                    P(gos[0]), P(gos[1]), P(gos[2]), P(gos[3]), P(gx), P(gy), B, N, M,
-                                                   D, p, eps, lam, None, 1, ops._stream(x.device))
+                                                   D, p, eps, lam, None, 1, P(lh), ops._stream(x.device))
         _lib.check(rc, "b200ot_sinkhorn_final_bwd_small")
         ops.count_launches(1)
-        return (gx, gy) + (None,) * 10
+        return (gx, gy) + (None,) * 11
 
 
 class _FinalValue(torch.autograd.Function):
@@ -106,7 +106,7 @@ class _FinalValue(torch.autograd.Function):
     kernel — no elementwise torch kernels, no autograd graph between the potentials and the value."""
 
     @staticmethod
-    def forward(ctx, x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, p, debias, rho, eps_final):
+    def forward(ctx, x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, p, debias, rho, eps_final, lh):
         B, N, D = x.shape
         M = y.shape[1]
         dev = x.device
@@ -127,7 +127,7 @@ class _FinalValue(torch.autograd.Function):
             rc = L.b200ot_sinkhorn_iteration_small(P(x), P(y), P(ad), P(bd), P(f_ba), P(g_ab), P(f_aa), P(g_bb),
                                                    P(n_f_ba), P(n_g_ab), P(n_f_aa), P(n_g_bb),
                                                    P(lse2) if need_xy else None, B, N, M, D, int(p), float(eps), 0.0,
-                                                   float(lam), 1, st)
+                                                   float(lam), 1, P(lh), st)
             _lib.check(rc, "b200ot_sinkhorn_iteration_small")
             rc = L.b200ot_sinkhorn_cost_small(P(ad), P(bd), P(n_f_ba), P(n_g_ab), P(n_f_aa), P(n_g_bb), B, N, M,
                                               -1.0 if rho is None else float(rho), float(eps_final), P(value),
@@ -139,13 +139,14 @@ class _FinalValue(torch.autograd.Function):
             _lib.check(rc, "b200ot_sinkhorn_cost_small")
         ops.count_launches(2)
         if need_xy or need_w:
-            ctx.save_for_backward(x, y, ad, bd, f_ba, g_ab, f_aa if debias else f_ba, g_bb if debias else g_ab, work)
+            ctx.save_for_backward(x, y, ad, bd, f_ba, g_ab, f_aa if debias else f_ba, g_bb if debias else g_ab, work,
+                                  lh)
             ctx.meta = (float(eps), float(lam), int(p), bool(debias), need_xy, need_w)
         return value
 
     @staticmethod
     def backward(ctx, gv):
-        x, y, a, b, f_ba, g_ab, f_aa, g_bb, work = ctx.saved_tensors
+        x, y, a, b, f_ba, g_ab, f_aa, g_bb, work, lh = ctx.saved_tensors
         eps, lam, p, debias, need_xy, need_w = ctx.meta
         B, N, D = x.shape
         M = y.shape[1]
@@ -162,7 +163,8 @@ class _FinalValue(torch.autograd.Function):
                 rc = L.b200ot_sinkhorn_final_bwd_small(P(x), P(y), P(a), P(b), P(f_ba), P(g_ab),
                                                        P(f_aa) if debias else None, P(g_bb) if debias else None,
                                                        P(lse2), P(go_f_ba), P(go_g_ab), P(go_f_aa), P(go_g_bb), P(gx),
-                                                       P(gy), B, N, M, D, p, eps, lam, P(gv), 1, ops._stream(x.device))
+                                                       P(gy), B, N, M, D, p, eps, lam, P(gv), 1, P(lh),
+                                                       ops._stream(x.device))
             _lib.check(rc, "b200ot_sinkhorn_final_bwd_small")
             ops.count_launches(1)
         if need_w:
@@ -171,7 +173,7 @@ class _FinalValue(torch.autograd.Function):
                 ga = terms[: B * N].view(B, N) * gv[:, None]
             if ctx.needs_input_grad[3]:
                 gb = terms[B * N:].view(B, M) * gv[:, None]
-        return (gx, gy, ga, gb) + (None,) * 10
+        return (gx, gy, ga, gb) + (None,) * 11
 
 
 def sinkhorn_small(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scaling=0.5, debias=True, potentials=False,
@@ -183,16 +185,21 @@ def sinkhorn_small(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scalin
     a, b = ops._f32c(a, "a"), ops._f32c(b, "b")
     B, N, D = x.shape
     M = y.shape[1]
+    # the batch's bounding box, in one launch: its mid-point is the origin of the kernels' coordinates (whatever the
+    # diameter), its diagonal the default diameter (one over the flattened batch, as the reference measures it)
+    lh = ops.cloud_extent(x.view(-1, D), y.view(-1, D))
+    if diameter is None:
+        diameter = extent_diameter(lh)
     diameter, eps_final, eps_list, rho = scaling_parameters(x, y, p, blur, reach, diameter, scaling)
     pk = (p | ops.P_UNCLAMPED) if keops else p
     ad, bd = a.detach(), b.detach()
     with torch.no_grad():
-        f_ba, g_ab, f_aa, g_bb = _descent(x.detach(), y.detach(), ad, bd, eps_list, rho, pk, debias)
+        f_ba, g_ab, f_aa, g_bb = _descent(x.detach(), y.detach(), ad, bd, eps_list, rho, pk, debias, lh)
     eps = eps_list[-1]
     lam = damping(eps, rho)
     if not potentials:
-        return _FinalValue.apply(x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, pk, debias, rho, eps_final)
-    outs = _FinalStep.apply(x, y, ad, bd, f_ba, g_ab, f_aa, g_bb, eps, lam, pk, debias)
+        return _FinalValue.apply(x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, pk, debias, rho, eps_final, lh)
+    outs = _FinalStep.apply(x, y, ad, bd, f_ba, g_ab, f_aa, g_bb, eps, lam, pk, debias, lh)
     if debias:
         n_f_ba, n_g_ab, n_f_aa, n_g_bb = outs
     else:

@@ -317,7 +317,8 @@ B200OT_API int b200ot_kernel_conv_bwd_finalize(const float* part, int32_t n_part
  * Small problems: one launch per symmetric Sinkhorn iteration
  * replaces the four softmin calls of the loop body of sinkhorn_loop (sinkhorn_divergence.py:468-493) — and of its
  * initialisation (:461-465) and final gradient-carrying step (:612-623) — for B stacked problems
- * x:(B,N,D) y:(B,M,D) a_log:(B,N) b_log:(B,M) with N, M <= B200OT_SMALL_MAX_POINTS, D <= B200OT_MAX_D:
+ * x:(B,N,D) y:(B,M,D) a_log:(B,N) b_log:(B,M) with N, M <= B200OT_SMALL_MAX_POINTS, D <= B200OT_MAX_D and any B >= 1
+ * (a batch above 65535 elements, the grid's z limit, is enqueued as consecutive launches over slices of it):
  *     f_ba_out <- alpha_old f_ba + beta softmin(eps, (x, y), b_log + g_ab/eps)      (B,N)
  *     g_ab_out <- alpha_old g_ab + beta softmin(eps, (y, x), a_log + f_ba/eps)      (B,M)
  *     f_aa_out <- alpha_old f_aa + beta softmin(eps, (x, x), a_log + f_aa/eps)      (B,N)   (debiasing; nullable pair)
@@ -330,6 +331,10 @@ B200OT_API int b200ot_kernel_conv_bwd_finalize(const float* part, int32_t n_part
  *     grad_y <- scale_out * ( go_g_ab[j] d softmin_yx / d y_j + go_g_bb[j] d softmin_yy / d y_j )     (B,M,D)
  * with columns and potentials held constant (the reference's autograd contract); f_ba .. g_bb are the potentials
  * that entered the final step; go_* nullable (zero upstream gradient).
+ * lo_hi (nullable, 2*D floats on the device: minima then maxima, as written by b200ot_cloud_extent): the coordinates are
+ * taken relative to the mid-point of this box before they are scaled by the temperature — pass the box of the whole
+ * batch, or the costs of clouds far from the origin lose the low bits of their differences.  Every call of one descent
+ * and its gradient must see the same box.
  * ------------------------------------------------------------------------------------------- */
 #define B200OT_SMALL_MAX_POINTS 65536
 B200OT_API int b200ot_sinkhorn_iteration_small(const float* x, const float* y, const float* a_log, const float* b_log,
@@ -337,7 +342,7 @@ B200OT_API int b200ot_sinkhorn_iteration_small(const float* x, const float* y, c
                                                const float* g_bb, float* f_ba_out, float* g_ab_out, float* f_aa_out,
                                                float* g_bb_out, float* lse2_out, int64_t B, int64_t N, int64_t M,
                                                int32_t D, int32_t p, float eps, float alpha_old, float beta,
-                                               int32_t weights_linear, void* stream);
+                                               int32_t weights_linear, const float* lo_hi, void* stream);
 /* The whole descent in ONE host call: initialisation at eps_list[0] (potentials <- damped softmins of the log-weights)
  * followed by one averaged symmetric update per temperature of eps_list (host array of n_eps doubles) — n_eps + 1
  * launches enqueued back to back, no Python / FFI round trip between them.  rho <= 0: balanced (damping 1), else
@@ -347,14 +352,16 @@ B200OT_API int b200ot_sinkhorn_iteration_small(const float* x, const float* y, c
 B200OT_API int b200ot_sinkhorn_loop_small(const float* x, const float* y, const float* a, const float* b,
                                           int32_t weights_linear, const double* eps_list, int32_t n_eps, double rho,
                                           int32_t debias, float* pots_a, float* pots_b, int32_t* result_in_a,
-                                          int64_t B, int64_t N, int64_t M, int32_t D, int32_t p, void* stream);
+                                          int64_t B, int64_t N, int64_t M, int32_t D, int32_t p,
+                                          const float* lo_hi, void* stream);
 B200OT_API int b200ot_sinkhorn_final_bwd_small(const float* x, const float* y, const float* a_log, const float* b_log,
                                                const float* f_ba, const float* g_ab, const float* f_aa,
                                                const float* g_bb, const float* lse2, const float* go_f_ba,
                                                const float* go_g_ab, const float* go_f_aa, const float* go_g_bb,
                                                float* grad_x, float* grad_y, int64_t B, int64_t N, int64_t M,
                                                int32_t D, int32_t p, float eps, float scale_out,
-                                               const float* go_scale, int32_t weights_linear, void* stream);
+                                               const float* go_scale, int32_t weights_linear, const float* lo_hi,
+                                               void* stream);
 /* go_scale (nullable): (B,) per-problem factor applied to every go_* — the upstream gradient of the B loss values when
  * go_* hold d value / d potential as written by b200ot_sinkhorn_cost_small.
  *

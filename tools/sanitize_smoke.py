@@ -30,7 +30,7 @@ def check(name, got, ref, tol=2e-5):
     assert err < tol, name
 
 
-which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "blocks", "grid", "loss"}
+which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "blocks", "grid", "loss", "small"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -209,5 +209,23 @@ if "loss" in which:
     print("multiscale sinkhorn", v.item())
     v = SamplesLoss("gaussian", blur=0.1, backend="multiscale", truncate=2)(x[0], y[0])
     print("multiscale gaussian", v.item())
+if "small" in which:
+    # the small-cloud kernels at D = 8 (csrc/b200ot_small.cu): the iteration kernel with 8 warps (one problem: 10 row
+    # tiles x 4 problems = 40 CTAs) and with 4 (40 elements: 1600 CTAs), the final backward, both MMD kernels
+    d, n, m = 8, 300, 260
+    for B in (1, 40):
+        x, y = torch.rand(B, n, d, generator=g), torch.rand(B, m, d, generator=g)
+        xg = x.to(DEV).requires_grad_(True)
+        v = SamplesLoss("sinkhorn", blur=0.3)(xg, y.to(DEV))
+        (gx,) = torch.autograd.grad(v.sum(), xg)
+        assert torch.isfinite(v).all() and torch.isfinite(gx).all()
+        print(f"small sinkhorn B={B} d={d}", v[:2].tolist())
+        xg = x.to(DEV).requires_grad_(True)
+        v = SamplesLoss("gaussian", blur=0.5)(xg, y.to(DEV))
+        (gx,) = torch.autograd.grad(v.sum(), xg)
+        assert torch.isfinite(gx).all()
+        K = lambda u, w: (-((u[:, :, None].double() - w[:, None].double()) ** 2).sum(-1) / 0.5).exp()  # noqa: E731
+        ref = 0.5 * K(x, x).mean((1, 2)) + 0.5 * K(y, y).mean((1, 2)) - K(x, y).mean((1, 2))
+        check(f"small_gaussian_B{B}_d{d}", v, ref, 1e-4)
 torch.cuda.synchronize()
 print("sanitize_smoke: all launches completed")
