@@ -35,6 +35,9 @@ static bool valid_kind(int kind) {
   return kind_base(kind) >= 0 && kind_base(kind) <= 2 && (kind & ~(0xff | B200OT_KERNEL_UNCLAMPED)) == 0;
 }
 
+// blur is the length scale of the gaussian and laplacian kernels; the energy kernel has none
+static bool blur_ok(int kind, float blur) { return kind_base(kind) == B200OT_KERNEL_ENERGY || blur > 0.f; }
+
 static ConvScales conv_scales(int kind_flags, float blur) {
   ConvScales c;
   const int kind = kind_base(kind_flags);
@@ -208,10 +211,12 @@ static float conv_bwd_coef(int kind_flags, const ConvScales& cs, float blur) {
 // ---------------------------------------------------------------------------------------------------
 // tensor-core path (gaussian, and laplacian / energy for 8 < D <= 64): see tcconv.cuh
 // ---------------------------------------------------------------------------------------------------
+// A launch group: `ctas` x n_split CTAs over a_tiles row images and b_tiles column images, then the partials and a misc
+// block in the scratch
 struct TcPlan {
   int kp, nstage, n_split, tiles_per_split;
-  int rtpe, ctpe;  // row / column tiles per batch element
-  int64_t a_tiles, b_tiles, a_bytes, b_bytes, smem;
+  int rtpe, ctpe;  // row / column tiles per batch element (0 for a block-sparse problem)
+  int64_t a_tiles, b_tiles, ctas, smem;
   int64_t off_b, off_part, off_misc, total;
 };
 
@@ -290,38 +295,47 @@ static TcBwdTuning tc_bwd_tuning() {
   return t;
 }
 
-// B > 1 (the batched entry points): B problems of N rows x M columns side by side, each element padded to whole tiles on
-// its own (tc_pack_kernel).  The split count is chosen for the whole grid, as without a batch, and cuts each element's
-// ctpe column tiles (so it is capped at ctpe); a CTA never reads another element's columns.  B = 1 is the plan of one
-// problem.
-static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd = false, int64_t B = 1) {
+// The plan of a launch group: `ctas` row CTAs, each reading up to `tiles` (>= 1) column tiles.  The split count is
+// chosen for the whole grid and cuts those tiles.  Behind the images: the partials of `rows` rows ((m, s) pairs forward, D+1
+// sums per row backward), then a misc block of misc_bytes.
+static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, int64_t ctas, int64_t tiles, int64_t rows,
+                           int64_t misc_bytes) {
   TcPlan p;
   p.kp = tc_kp(D);
-  p.rtpe = (int)ceil_div64(N, kTcM);
-  p.ctpe = (int)ceil_div64(M, kTcBN);
-  p.a_tiles = B * p.rtpe;
-  p.b_tiles = B * p.ctpe;
-  p.a_bytes = tc_a_img_bytes(p.kp);
-  p.b_bytes = tc_b_img_bytes(p.kp, kTcBN);
+  p.rtpe = p.ctpe = 0;
+  p.a_tiles = a_tiles;
+  p.b_tiles = b_tiles;
+  p.ctas = ctas;
+  const int64_t b_bytes = tc_b_img_bytes(p.kp, kTcBN);
   const int64_t bar_bytes = 256;  // mbarriers behind the column ring
   // the CTA's row image stays in shared memory; the rest of the 227 KB a block may use holds the column ring
   const int64_t avail = 227 * 1024 - bar_bytes - tc_a_span(p.kp);
-  int64_t ns = avail / p.b_bytes;
+  int64_t ns = avail / b_bytes;
   p.nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
-  p.smem = tc_a_span(p.kp) + p.nstage * p.b_bytes + bar_bytes;
-  int64_t want = ceil_div64((int64_t)num_sms() * 4, p.a_tiles);
+  p.smem = tc_a_span(p.kp) + p.nstage * b_bytes + bar_bytes;
+  int64_t want = ceil_div64((int64_t)num_sms() * 4, ctas);
   const int forced = forced_splits();  // test hook (plan.cuh)
   if (forced > 0) want = forced;
   if (want < 1) want = 1;
   if (want > 64) want = 64;
-  if (want > p.ctpe) want = p.ctpe;
-  p.tiles_per_split = (int)ceil_div64(p.ctpe, want);
-  p.n_split = (int)ceil_div64(p.ctpe, p.tiles_per_split);
-  p.off_b = round_up64(p.a_tiles * p.a_bytes, 256);
-  p.off_part = p.off_b + round_up64(p.b_tiles * p.b_bytes, 256);
-  // partials: (m, s) pairs forward, D+1 sums per row backward
-  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? B * N * (D + 1) : kTcParts * B * N * 2) * 4, 256);
-  p.total = p.off_misc + round_up64((B + 1) * 4, 256);  // [0]: energy coordinate max, [1 + b]: max|w| of element b
+  if (want > tiles) want = tiles;
+  p.tiles_per_split = (int)ceil_div64(tiles, want);
+  p.n_split = (int)ceil_div64(tiles, p.tiles_per_split);
+  p.off_b = round_up64(a_tiles * tc_a_img_bytes(p.kp), 256);
+  p.off_part = p.off_b + round_up64(b_tiles * b_bytes, 256);
+  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? rows * (D + 1) : kTcParts * rows * 2) * 4, 256);
+  p.total = p.off_misc + round_up64(misc_bytes, 256);
+  return p;
+}
+
+// B problems of N rows x M columns side by side (B = 1: one problem), each element padded to whole tiles on its own
+// (tc_pack_kernel).  The splits cut each element's ctpe column tiles, so a CTA never reads another element's columns.
+// Misc block: [0] the energy coordinate maximum, [1 + b] max|w| of element b.
+static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B = 1) {
+  const int rtpe = (int)ceil_div64(N, kTcM), ctpe = (int)ceil_div64(M, kTcBN);
+  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4);
+  p.rtpe = rtpe;
+  p.ctpe = ctpe;
   return p;
 }
 
@@ -330,86 +344,131 @@ int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
   return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B).total);
 }
 
+// What the images of a launch group hold (tc_pack_kernel): the row cloud x and the column cloud y, centred at `center`
+// and multiplied by `scale`; B elements of N rows / M columns, or N / M block-sparse slots gathered through row_src /
+// col_src.  Besides the coordinates: the column weights w, the softmin's column terms h_a + h_scale_b h_b and the
+// softmin row gradient's row term lse2.
+struct TcOperands {
+  const float *x, *y, *center;
+  float scale;
+  int64_t N, M;
+  int D;
+  int64_t B = 1;
+  const float *w = nullptr, *h_a = nullptr, *h_b = nullptr;
+  float h_scale_b = 0.f;
+  const float* lse2 = nullptr;
+  const int *row_src = nullptr, *col_src = nullptr;
+};
+
+// Packs both images of plan p.  Asked for through a non-null out pointer, it first computes into the misc block:
+//   * w_absmax (row gradients): P = w_j e_ij feeds an fp16 GEMM, so the weights are normalised to max|w| = kTcPScale
+//     (undone by the finalize kernel), one maximum per batch element, so that a heavy element cannot push a light
+//     one's P into fp16's subnormal range;
+//   * coord_absmax (energy): the largest centred coordinate of both clouds (of every batch element: one scale for the
+//     whole batch, a power of two that the finalize undoes exactly), from which every kernel of the pass derives the
+//     same power-of-two coordinate scale (tc_energy_coord_scale).
+static int tc_pack(const TcPlan& p, unsigned char* base, const TcOperands& o, cudaStream_t st,
+                   const float** w_absmax = nullptr, const float** coord_absmax = nullptr) {
+  float* misc = reinterpret_cast<float*>(base + p.off_misc);
+  const float* cmax = nullptr;
+  if (coord_absmax) {
+    B200OT_CUDA_TRY(cudaMemsetAsync(misc, 0, sizeof(float), st));
+    const int64_t n = o.B * o.N, m = o.B * o.M;
+    coord_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((n + m) * o.D, 256), 1024), 256, 0, st>>>(
+        o.x, n, o.y, m, o.D, o.center, misc);
+    B200OT_CUDA_TRY(cudaGetLastError());
+    cmax = *coord_absmax = misc;
+  }
+  const float* wmax = nullptr;
+  if (w_absmax) {
+    if (o.w != nullptr) {
+      B200OT_CUDA_TRY(cudaMemsetAsync(misc + 1, 0, o.B * sizeof(float), st));
+      const dim3 g((unsigned)std::min<int64_t>(ceil_div64(o.M, 256), 1024), (unsigned)o.B);
+      absmax_kernel<<<g, 256, 0, st>>>(o.w, o.M, misc + 1);
+      B200OT_CUDA_TRY(cudaGetLastError());
+      wmax = misc + 1;
+    }
+    *w_absmax = wmax;
+  }
+  const int threads = 128;
+  tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
+      o.x, nullptr, nullptr, nullptr, 0.f, 0.f, o.center, o.scale, o.N, o.D, p.kp, kTcM, 0, base, o.lse2, nullptr, cmax,
+      o.B, o.row_src);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
+      o.y, o.w, o.h_a, o.h_b, o.h_scale_b, kLog2e, o.center, o.scale, o.M, o.D, p.kp, kTcBN, 1, base + p.off_b, nullptr,
+      wmax, cmax, o.B, o.col_src);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// The parameter list of tc_reduce_kernel and tc_bwd_kernel
+using TcKernel = void (*)(const unsigned char*, const unsigned char*, float*, int64_t, int, int, int, int, int, int,
+                          float, const float*, int, int64_t, const int4*, const int2*, const int*);
+
+// One launch of a reduction or row-gradient kernel over plan p, into the plan's partials: `rows` rows (n_local per
+// batch element; block-sparse problems: seg / pieces / row_src)
+static int tc_launch(TcKernel kern, const TcPlan& p, unsigned char* base, int64_t rows, int64_t n_local, int D,
+                     int self_mode, float clampq, const float* coord_absmax, cudaStream_t st,
+                     const int4* seg = nullptr, const int2* pieces = nullptr, const int* row_src = nullptr) {
+  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+  const dim3 grid((unsigned)p.ctas, (unsigned)p.n_split);
+  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(base, base + p.off_b, reinterpret_cast<float*>(base + p.off_part),
+                                                 rows, p.kp, p.ctpe, p.tiles_per_split, p.nstage, D, self_mode, clampq,
+                                                 coord_absmax, p.rtpe, n_local, seg, pieces, row_src);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// tc_bwd_kernel at the padded dimension of D
+template <int MODE, int PT, bool MERGE, bool BATCH, bool BLOCKS = false>
+static TcKernel tc_bwd_dk(int D) {
+  switch (tc_dk(D)) {
+    case 16: return tc_bwd_kernel<MODE, PT, MERGE, 16, BATCH, BLOCKS>;
+    case 32: return tc_bwd_kernel<MODE, PT, MERGE, 32, BATCH, BLOCKS>;
+    case 48: return tc_bwd_kernel<MODE, PT, MERGE, 48, BATCH, BLOCKS>;
+    default: return tc_bwd_kernel<MODE, PT, MERGE, 64, BATCH, BLOCKS>;
+  }
+}
+
+// The row-gradient instantiation of MODE: the $B200OT_TC_BWD variant for the gaussian and the softmin of one problem,
+// the default variant (PT = 2, MERGE) for the laplacian, the energy and every batch
+template <int MODE>
+static TcKernel tc_bwd_variant(int D, bool batched) {
+  if (batched) return tc_bwd_dk<MODE, 2, true, true>(D);
+  if constexpr (MODE == 2 || MODE == 3) {
+    const TcBwdTuning tn = tc_bwd_tuning();
+    if (tn.merge) return tn.p_terms == 1 ? tc_bwd_dk<MODE, 1, true, false>(D) : tc_bwd_dk<MODE, 2, true, false>(D);
+    return tn.p_terms == 1 ? tc_bwd_dk<MODE, 1, false, false>(D) : tc_bwd_dk<MODE, 2, false, false>(D);
+  }
+  return tc_bwd_dk<MODE, 2, true, false>(D);
+}
+
 // Row gradients on the tensor-core path; `mode` is the MODE of tc_bwd_kernel (2 gaussian conv, 3 softmin p = 2,
-// 4 laplacian, 5 energy; clampq and coord_absmax: see there).  Leaves n_part sets of (B N, D+1) partial sums in
-// *part_out.  `batched`: B elements of N rows / M columns (make_tc_plan), the weights normalised per element.
+// 4 laplacian, 5 energy; clampq: see there).  Leaves n_part sets of (B N, D+1) partial sums in *part_out, and the
+// scales the finalize undoes in *w_absmax_out and *coord_absmax_out (tc_pack; null when the pass has none).
+// `batched`: B elements of N rows / M columns (make_tc_plan), the weights normalised per element.
 int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
-                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out,
-                   float clampq, const float* coord_absmax, int64_t B, bool batched) {
+                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, int64_t B, bool batched,
+                   const float** w_absmax_out, float clampq, const float** coord_absmax_out) {
   const TcPlan p = make_tc_plan(N, M, D, true, B);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  unsigned char* a_imgs = base;
-  unsigned char* b_imgs = base + p.off_b;
-  float* part = reinterpret_cast<float*>(base + p.off_part);
-  float* w_absmax = nullptr;
-  if (w != nullptr) {
-    // P = w_j e_ij feeds an fp16 GEMM: normalise the weights to max|w| = kTcPScale (undone by the finalize kernel),
-    // one maximum per batch element, so that a heavy element cannot push a light one's P into fp16's subnormal range
-    w_absmax = reinterpret_cast<float*>(base + p.off_misc) + 1;
-    B200OT_CUDA_TRY(cudaMemsetAsync(w_absmax, 0, B * sizeof(float), st));
-    const dim3 g((unsigned)std::min<int64_t>(ceil_div64(M, 256), 1024), (unsigned)B);
-    absmax_kernel<<<g, 256, 0, st>>>(w, M, w_absmax);
-    B200OT_CUDA_TRY(cudaGetLastError());
-  }
-  if (w_absmax_out) *w_absmax_out = w_absmax;
-  const int threads = 128;
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, lse2, nullptr, coord_absmax,
-      B);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, w, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, w_absmax,
-      coord_absmax, B);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
-  const int self_mode = (mode != 3 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
-  auto launch = [&](auto kern) -> int {
-    B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
-                                                   p.nstage, D, self_mode, clampq, coord_absmax, p.rtpe, N, nullptr, nullptr, nullptr);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    return B200OT_OK;
-  };
-  const TcBwdTuning tn = tc_bwd_tuning();
-  // (MODE, PT, MERGE, padded dimension, batch) -> instantiation
-  auto pick_dk = [&](auto mode_tag, auto pt_tag, auto merge_tag, auto batch_tag) -> int {
-    constexpr int MODE = decltype(mode_tag)::value, PT = decltype(pt_tag)::value;
-    constexpr bool MG = decltype(merge_tag)::value, BT = decltype(batch_tag)::value;
-    switch (tc_dk(D)) {
-      case 16: return launch(tc_bwd_kernel<MODE, PT, MG, 16, BT>);
-      case 32: return launch(tc_bwd_kernel<MODE, PT, MG, 32, BT>);
-      case 48: return launch(tc_bwd_kernel<MODE, PT, MG, 48, BT>);
-      default: return launch(tc_bwd_kernel<MODE, PT, MG, 64, BT>);
-    }
-  };
-  // the default variant (PT = 2, MERGE): the only one of the laplacian and energy row gradients and of every batched
-  // row gradient
-  using T2 = std::integral_constant<int, 2>;
-  auto pick_default = [&](auto mode_tag) -> int {
-    return batched ? pick_dk(mode_tag, T2{}, std::true_type{}, std::true_type{})
-                   : pick_dk(mode_tag, T2{}, std::true_type{}, std::false_type{});
-  };
-  auto pick = [&](auto mode_tag) -> int {
-    using T1 = std::integral_constant<int, 1>;
-    using NB = std::false_type;
-    if (batched) return pick_default(mode_tag);
-    if (tn.merge)
-      return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::true_type{}, NB{})
-                             : pick_dk(mode_tag, T2{}, std::true_type{}, NB{});
-    return tn.p_terms == 1 ? pick_dk(mode_tag, T1{}, std::false_type{}, NB{})
-                           : pick_dk(mode_tag, T2{}, std::false_type{}, NB{});
-  };
-  int rc;
-  switch (mode) {
-    case 2: rc = pick(std::integral_constant<int, 2>{}); break;
-    case 3: rc = pick(std::integral_constant<int, 3>{}); break;
-    case 4: rc = pick_default(std::integral_constant<int, 4>{}); break;
-    default: rc = pick_default(std::integral_constant<int, 5>{}); break;
-  }
+  const float *w_absmax = nullptr, *coord_absmax = nullptr;
+  int rc = tc_pack(p, base, {x, y, center, scale, N, M, D, B, w, h_a, h_b, h_scale_b, lse2}, st, &w_absmax,
+                   mode == 5 ? &coord_absmax : nullptr);
   if (rc) return rc;
-  *part_out = part;
+  const TcKernel kern = mode == 2   ? tc_bwd_variant<2>(D, batched)
+                        : mode == 3 ? tc_bwd_variant<3>(D, batched)
+                        : mode == 4 ? tc_bwd_variant<4>(D, batched)
+                                    : tc_bwd_variant<5>(D, batched);
+  const int self_mode = (mode != 3 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
+  rc = tc_launch(kern, p, base, B * N, N, D, self_mode, clampq, coord_absmax, st);
+  if (rc) return rc;
+  if (w_absmax_out) *w_absmax_out = w_absmax;
+  if (coord_absmax_out) *coord_absmax_out = coord_absmax;
+  *part_out = reinterpret_cast<float*>(base + p.off_part);
   *n_part_out = p.n_split;  // G of a CTA is complete over its column split (both column halves feed one GEMM)
   return B200OT_OK;
 }
@@ -422,25 +481,11 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
   const TcPlan p = make_tc_plan(N, M, D, false, B);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  unsigned char* a_imgs = base;
-  unsigned char* b_imgs = base + p.off_b;
-  float* part = reinterpret_cast<float*>(base + p.off_part);
-  const float scale = softmin_coord_scale(2, eps);
-  const int threads = 128;
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, nullptr, nullptr, nullptr, B);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, nullptr, h_a, h_b, h_scale_b, kLog2e, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr, nullptr,
-      B);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  auto kern = batched ? tc_reduce_kernel<1, true> : tc_reduce_kernel<1>;
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
-  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
-                                                 p.nstage, D, 0, 0.f, nullptr, p.rtpe, N, nullptr, nullptr, nullptr);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  *part_out = part;
+  int rc = tc_pack(p, base, {x, y, center, softmin_coord_scale(2, eps), N, M, D, B, nullptr, h_a, h_b, h_scale_b}, st);
+  if (rc) return rc;
+  rc = tc_launch(batched ? tc_reduce_kernel<1, true> : tc_reduce_kernel<1>, p, base, B * N, N, D, 0, 0.f, nullptr, st);
+  if (rc) return rc;
+  *part_out = reinterpret_cast<float*>(base + p.off_part);
   *n_part_out = p.n_split * kTcParts;
   return B200OT_OK;
 }
@@ -489,27 +534,13 @@ int blocks_validate(int64_t n_row_slots, int64_t n_col_slots, const b200ot_segme
   return B200OT_OK;
 }
 
-// The plan of one block-sparse problem: images of n_row_slots / n_col_slots points, segments cut into splits the way
-// make_tc_plan cuts a dense problem's column tiles (from the longest segment), then the descriptors.
+// The plan of one block-sparse problem: a CTA per segment, images of n_row_slots / n_col_slots points, segments cut
+// into splits from the longest one.  Misc block: the segment descriptors, then the pieces.
+static int64_t tc_blocks_seg_bytes(int64_t n_seg) { return round_up64(n_seg * 16, 256); }
 static TcPlan make_tc_blocks_plan(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
                                   int max_tiles, int D, bool bwd) {
-  TcPlan p = make_tc_plan(kTcM, kTcBN, D, bwd);
-  p.a_tiles = n_row_slots / kTcM;
-  p.b_tiles = n_col_slots / kTcBN;
-  int64_t want = ceil_div64((int64_t)num_sms() * 4, n_seg);
-  const int forced = forced_splits();  // test hook (plan.cuh)
-  if (forced > 0) want = forced;
-  if (want < 1) want = 1;
-  if (want > 64) want = 64;
-  const int mt = std::max(max_tiles, 1);
-  if (want > mt) want = mt;
-  p.tiles_per_split = (int)ceil_div64(mt, want);
-  p.n_split = (int)ceil_div64(mt, p.tiles_per_split);
-  p.off_b = round_up64(p.a_tiles * p.a_bytes, 256);
-  p.off_part = p.off_b + round_up64(p.b_tiles * p.b_bytes, 256);
-  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? N * (D + 1) : kTcParts * N * 2) * 4, 256);
-  p.total = p.off_misc + round_up64(n_seg * 16, 256) + round_up64(std::max<int64_t>(n_pieces, 1) * 8, 256);
-  return p;
+  return make_tc_plan(D, bwd, n_row_slots / kTcM, n_col_slots / kTcBN, n_seg, std::max(max_tiles, 1), N,
+                      tc_blocks_seg_bytes(n_seg) + std::max<int64_t>(n_pieces, 1) * 8);
 }
 
 int64_t tc_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
@@ -529,101 +560,75 @@ int softmin_blocks_tc(bool bwd, const float* x, const float* y, const float* h_a
   const TcPlan p = make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, bwd);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  unsigned char* a_imgs = base;
-  unsigned char* b_imgs = base + p.off_b;
-  float* part = reinterpret_cast<float*>(base + p.off_part);
   int4* d_seg = reinterpret_cast<int4*>(base + p.off_misc);
-  int2* d_pieces = reinterpret_cast<int2*>(base + p.off_misc + round_up64(n_seg * 16, 256));
-  const float scale = softmin_coord_scale(2, eps);
+  int2* d_pieces = reinterpret_cast<int2*>(base + p.off_misc + tc_blocks_seg_bytes(n_seg));
   B200OT_CUDA_TRY(cudaMemcpyAsync(d_seg, seg, n_seg * 16, cudaMemcpyHostToDevice, st));
   if (n_pieces > 0) B200OT_CUDA_TRY(cudaMemcpyAsync(d_pieces, pieces, n_pieces * 8, cudaMemcpyHostToDevice, st));
-  const int threads = 128;
-  tc_pack_kernel<<<(unsigned)ceil_div64(n_row_slots, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, n_row_slots, D, p.kp, kTcM, 0, a_imgs,
-      bwd ? lse2 : nullptr, nullptr, nullptr, 1, row_src);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  tc_pack_kernel<<<(unsigned)ceil_div64(n_col_slots, threads), threads, 0, st>>>(
-      y, nullptr, h_a, h_b, h_scale_b, kLog2e, center, scale, n_col_slots, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr,
-      nullptr, 1, col_src);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  dim3 grid((unsigned)n_seg, (unsigned)p.n_split);
-  auto launch = [&](auto kern) -> int {
-    B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, N, p.kp, 0, p.tiles_per_split, p.nstage, D, 0,
-                                                   0.f, nullptr, 0, 0, d_seg, d_pieces, row_src);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    return B200OT_OK;
-  };
-  int rc;
-  if (!bwd) {
-    rc = launch(tc_reduce_kernel<1, false, true>);
-  } else {
-    // the default row-gradient variant (PT = 2, MERGE)
-    switch (tc_dk(D)) {
-      case 16: rc = launch(tc_bwd_kernel<3, 2, true, 16, false, true>); break;
-      case 32: rc = launch(tc_bwd_kernel<3, 2, true, 32, false, true>); break;
-      case 48: rc = launch(tc_bwd_kernel<3, 2, true, 48, false, true>); break;
-      default: rc = launch(tc_bwd_kernel<3, 2, true, 64, false, true>); break;
-    }
-  }
+  int rc = tc_pack(p, base,
+                   {x, y, center, softmin_coord_scale(2, eps), n_row_slots, n_col_slots, D, 1, nullptr, h_a, h_b,
+                    h_scale_b, bwd ? lse2 : nullptr, row_src, col_src},
+                   st);
   if (rc) return rc;
-  *part_out = part;
+  // the row gradient runs its default variant (PT = 2, MERGE)
+  const TcKernel kern = bwd ? tc_bwd_dk<3, 2, true, false, true>(D) : tc_reduce_kernel<1, false, true>;
+  rc = tc_launch(kern, p, base, N, 0, D, 0, 0.f, nullptr, st, d_seg, d_pieces, row_src);
+  if (rc) return rc;
+  *part_out = reinterpret_cast<float*>(base + p.off_part);
   *n_part_out = bwd ? p.n_split : p.n_split * kTcParts;
   return B200OT_OK;
 }
 
-// Energy on the tensor cores: the largest centred coordinate of both clouds (of every batch element: one scale for the
-// whole batch, a power of two that the finalize undoes exactly), from which every kernel of the pass derives the same
-// power-of-two coordinate scale (tc_energy_coord_scale).  Kept in the scratch's misc block, [0].
-static int energy_coord_absmax(const float* x, int64_t N, const float* y, int64_t M, int D, const float* center,
-                               unsigned char* misc, cudaStream_t st, const float** out) {
-  float* a = reinterpret_cast<float*>(misc);
-  B200OT_CUDA_TRY(cudaMemsetAsync(a, 0, sizeof(float), st));
-  coord_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((N + M) * D, 256), 1024), 256, 0, st>>>(x, N, y, M, D,
-                                                                                                       center, a);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  *out = a;
-  return B200OT_OK;
-}
-
 static int conv_fwd_tc(int kind_flags, const float* x, const float* y, const float* w, const float* center, float* out,
-                       int64_t N, int64_t M, int D, float blur, void* scratch, cudaStream_t st, int64_t B = 1,
-                       bool batched = false) {
+                       int64_t N, int64_t M, int D, float blur, void* scratch, cudaStream_t st, int64_t B,
+                       bool batched) {
   const int kind = kind_base(kind_flags);
-  const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
   const TcPlan p = make_tc_plan(N, M, D, false, B);
   if (p.nstage < 1) return B200OT_EINVAL;
   unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  unsigned char* a_imgs = base;
-  unsigned char* b_imgs = base + p.off_b;
-  float* part = reinterpret_cast<float*>(base + p.off_part);
   // gaussian: 2^(-|X-Y|^2/2) with X = x sqrt(log2e) / blur; laplacian / energy: conv_scales' coordinates and clamp
   const ConvScales cs = conv_scales(kind_flags, blur);
-  const float scale = kind == B200OT_KERNEL_GAUSSIAN ? sqrtf(kLog2e) / blur : cs.scale;
   const float* coord_absmax = nullptr;
-  if (kind == B200OT_KERNEL_ENERGY) {
-    const int rc = energy_coord_absmax(x, B * N, y, B * M, D, center, base + p.off_misc, st, &coord_absmax);
-    if (rc) return rc;
-  }
-  const int threads = 128;
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      x, nullptr, nullptr, nullptr, 0.f, 0.f, center, scale, N, D, p.kp, kTcM, 0, a_imgs, nullptr, nullptr,
-      coord_absmax, B);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      y, w, nullptr, nullptr, 0.f, 0.f, center, scale, M, D, p.kp, kTcBN, 1, b_imgs, nullptr, nullptr, coord_absmax,
-      B);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  auto kern = kind == B200OT_KERNEL_GAUSSIAN ? (batched ? tc_reduce_kernel<0, true> : tc_reduce_kernel<0>)
-              : kind == B200OT_KERNEL_LAPLACIAN ? (batched ? tc_reduce_kernel<4, true> : tc_reduce_kernel<4>)
-                                                : (batched ? tc_reduce_kernel<5, true> : tc_reduce_kernel<5>);
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  dim3 grid((unsigned)p.a_tiles, (unsigned)p.n_split);
-  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(a_imgs, b_imgs, part, B * N, p.kp, p.ctpe, p.tiles_per_split,
-                                                 p.nstage, D, self_mode, cs.clampq, coord_absmax, p.rtpe, N, nullptr, nullptr, nullptr);
-  B200OT_CUDA_TRY(cudaGetLastError());
+  int rc = tc_pack(p, base, {x, y, center, cs.scale, N, M, D, B, w}, st, nullptr,
+                   kind == B200OT_KERNEL_ENERGY ? &coord_absmax : nullptr);
+  if (rc) return rc;
+  const TcKernel kern = kind == B200OT_KERNEL_GAUSSIAN    ? (batched ? tc_reduce_kernel<0, true> : tc_reduce_kernel<0>)
+                        : kind == B200OT_KERNEL_LAPLACIAN ? (batched ? tc_reduce_kernel<4, true> : tc_reduce_kernel<4>)
+                                                          : (batched ? tc_reduce_kernel<5, true> : tc_reduce_kernel<5>);
+  const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
+  rc = tc_launch(kern, p, base, B * N, N, D, self_mode, cs.clampq, coord_absmax, st);
+  if (rc) return rc;
   conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-      part, p.n_split * kTcParts, kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, B * N, coord_absmax);
+      reinterpret_cast<const float*>(base + p.off_part), p.n_split * kTcParts,
+      kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, B * N, coord_absmax);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// Row gradients on the tensor cores (and, with value_out, the forward values from the same pass: gaussian only), of one
+// problem or (`batched`) of B elements of N rows / M columns.  Arguments already validated.  Every kernel leaves the
+// gaussian's sums: grad = coef (sum_j P Y_j - X_i sum_j P) with coef = 1 / (scale blur^2) for the gaussian; the
+// laplacian and energy P = w k'(d) / d carries 2^-kTcNormPLog2 (tcbwd.cuh), so coef = 2^kTcNormPLog2 / blur (laplacian,
+// X = x log2e / blur) or 2^kTcNormPLog2 (energy).
+static int conv_bwd_tc(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
+                       float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                       void* scratch, void* stream, int64_t B, bool batched) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const int kb = kind_base(kind);
+  const ConvScales cs = conv_scales(kind, blur);
+  const int mode = kb == B200OT_KERNEL_GAUSSIAN ? 2 : (kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5);
+  const float coef = kb == B200OT_KERNEL_GAUSSIAN
+                         ? 1.0f / (cs.scale * blur * blur)
+                         : (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
+  float* tc_part = nullptr;
+  int n_part = 0;
+  const float *w_absmax = nullptr, *coord_absmax = nullptr;
+  const int rc = bwd_partial_tc(mode, x, y, w, nullptr, nullptr, 0.f, nullptr, center, cs.scale, N, M, D, scratch,
+                                &tc_part, &n_part, st, B, batched, &w_absmax, cs.clampq, &coord_absmax);
+  if (rc) return rc;
+  const int64_t n_per = batched ? N : 0;  // rows per element: the finalize undoes each element's weight scale
+  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
+      tc_part, n_part, x, center, grad_out, grad_x, B * N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax,
+      value_out, coord_absmax, n_per);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
@@ -660,7 +665,7 @@ B200OT_API int b200ot_kernel_conv_bwd_finalize(const float* part, int32_t n_part
                                                int32_t kind, float blur, void* stream) {
   if (!part || !x || !grad_out || !grad_x || n_part <= 0 || N <= 0 || !supported_simt_dim(D) || !valid_kind(kind))
     return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  if (!blur_ok(kind, blur)) return B200OT_EINVAL;
   const ConvScales cs = conv_scales(kind, blur);
   const int threads = 256;
   conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, threads), threads, 0, (cudaStream_t)stream>>>(
@@ -675,7 +680,7 @@ B200OT_API int b200ot_kernel_conv_pack_gather(const float* y, const float* w, co
                                               float blur, float* cols_out, void* stream) {
   if (!y || !w || !src_index || !cols_out || n_slots <= 0 || !supported_simt_dim(D) || !valid_kind(kind))
     return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  if (!blur_ok(kind, blur)) return B200OT_EINVAL;
   if (((uintptr_t)cols_out) & 15) return B200OT_EALIGN;
   return conv_pack(y, w, center, n_slots, D, conv_scales(kind, blur), cols_out, (cudaStream_t)stream,
                    reinterpret_cast<const int*>(src_index));
@@ -691,25 +696,28 @@ B200OT_API int b200ot_kernel_conv_partial_ranges(const float* x, const float* ce
       !supported_simt_dim(D) || !valid_kind(kind) ||
       (variant != B200OT_RANGES_BIG && variant != B200OT_RANGES_SMALL))
     return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  if (!blur_ok(kind, blur)) return B200OT_EINVAL;
   if ((((uintptr_t)cols) & 15) || (((uintptr_t)seg) & 15) || (((uintptr_t)pieces) & 7)) return B200OT_EALIGN;
   return conv_partial(kind, backward != 0, ranges_plan(variant, n_seg), (cudaStream_t)stream, x, center,
                       conv_scales(kind, blur), cols, part, N, D, reinterpret_cast<const int4*>(seg),
                       reinterpret_cast<const int2*>(pieces));
 }
 
-B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
-                                      float* out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
-                                      void* scratch, int64_t scratch_bytes, void* stream) {
+// The kernel convolution of one problem, or (`batched`, 8 < D <= 64) of B problems of N rows / M columns side by side.
+// The two differ only in the shapes they accept and in their routing.
+static int conv_fwd_impl(const float* x, const float* y, const float* w, const float* center, float* out, int64_t B,
+                         int64_t N, int64_t M, int32_t D, int32_t kind, float blur, void* scratch,
+                         int64_t scratch_bytes, void* stream, bool batched) {
   // laplacian / energy: the tensor cores serve 8 < D <= 64 only (no measured cross-over below)
-  const bool tc = (kind_base(kind) == B200OT_KERNEL_GAUSSIAN) ? tc_routed(kTcConvFwd, D, N, M)
-                                                              : (D > B200OT_MAX_D && tc_capable_dim(D));
-  if (!x || !y || !w || !out || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) || !valid_kind(kind))
-    return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  const bool tc = batched || ((kind_base(kind) == B200OT_KERNEL_GAUSSIAN) ? tc_routed(kTcConvFwd, D, N, M)
+                                                                          : (D > B200OT_MAX_D && tc_capable_dim(D)));
+  const bool shape = batched ? tc_batched_dims(B, N, M, D) : (N > 0 && M > 0 && (supported_simt_dim(D) || tc));
+  if (!x || !y || !w || !out || !scratch || !shape || !valid_kind(kind)) return B200OT_EINVAL;
+  if (!blur_ok(kind, blur)) return B200OT_EINVAL;
   if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_kernel_conv_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
-  if (tc) return conv_fwd_tc(kind, x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream);
+  if (scratch_bytes < (batched ? b200ot_batched_scratch_bytes(B, N, M, D) : b200ot_kernel_conv_scratch_bytes(N, M, D)))
+    return B200OT_ESCRATCH;
+  if (tc) return conv_fwd_tc(kind, x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream, B, batched);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -723,66 +731,29 @@ B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const floa
   return b200ot_kernel_conv_finalize(part, pl.n_split, out, N, kind, stream);
 }
 
-// Row gradients on the tensor cores (and, with value_out, the forward values from the same pass: gaussian only), of one
-// problem or (`batched`) of B elements of N rows / M columns.  Arguments already validated.
-static int conv_bwd_tc(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
-                       float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
-                       void* scratch, void* stream, int64_t B = 1, bool batched = false) {
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t n_per = batched ? N : 0;  // rows per element: the finalize undoes each element's weight scale
-  if (kind_base(kind) != B200OT_KERNEL_GAUSSIAN) {
-    // grad = coef (sum_j P Y_j - X_i sum_j P) with P = w k'(d) / d scaled by 2^-kTcNormPLog2 (tcbwd.cuh): the
-    // gaussian's finalize with coef = 2^kTcNormPLog2 / blur (laplacian, X = x log2e / blur) or 2^kTcNormPLog2 (energy)
-    const int kb = kind_base(kind);
-    const ConvScales cs = conv_scales(kind, blur);
-    const float* coord_absmax = nullptr;
-    if (kb == B200OT_KERNEL_ENERGY) {
-      const TcPlan p = make_tc_plan(N, M, D, true, B);
-      const int rc = energy_coord_absmax(x, B * N, y, B * M, D, center,
-                                         reinterpret_cast<unsigned char*>(scratch) + p.off_misc, st, &coord_absmax);
-      if (rc) return rc;
-    }
-    float* tc_part = nullptr;
-    int n_part = 0;
-    const float* w_absmax = nullptr;
-    const int rc = bwd_partial_tc(kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5, x, y, w, nullptr, nullptr, 0.f, nullptr,
-                                  center, cs.scale, N, M, D, scratch, &tc_part, &n_part, st, &w_absmax, cs.clampq,
-                                  coord_absmax, B, batched);
-    if (rc) return rc;
-    const float coef = (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
-    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-        tc_part, n_part, x, center, grad_out, grad_x, B * N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax,
-        nullptr, coord_absmax, n_per);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    return B200OT_OK;
-  }
-  float* tc_part = nullptr;
-  int n_part = 0;
-  const float scale = sqrtf(kLog2e) / blur;
-  const float* w_absmax = nullptr;
-  const int rc = bwd_partial_tc(2, x, y, w, nullptr, nullptr, 0.f, nullptr, center, scale, N, M, D, scratch, &tc_part,
-                                &n_part, st, &w_absmax, 0.f, nullptr, B, batched);
-  if (rc) return rc;
-  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-      tc_part, n_part, x, center, grad_out, grad_x, B * N, D, 0, scale, 1.0f / (scale * blur * blur), w_absmax,
-      value_out, nullptr, n_per);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
+B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
+                                      float* out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                                      void* scratch, int64_t scratch_bytes, void* stream) {
+  return conv_fwd_impl(x, y, w, center, out, 1, N, M, D, kind, blur, scratch, scratch_bytes, stream, false);
 }
 
-// Row gradients (and, with value_out, the forward values from the same pass: gaussian only).
+// Row gradients (and, with value_out, the forward values from the same pass: gaussian only), of one problem or
+// (`batched`) of B problems, as conv_fwd_impl.
 static int conv_bwd_x_impl(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
-                           float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
-                           void* scratch, int64_t scratch_bytes, void* stream) {
+                           float* grad_x, float* value_out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
+                           float blur, void* scratch, int64_t scratch_bytes, void* stream, bool batched) {
   const bool gauss = kind_base(kind) == B200OT_KERNEL_GAUSSIAN;
-  const bool tc = gauss ? tc_routed(kTcConvBwd, D, N, M) : (D > B200OT_MAX_D && tc_capable_dim(D));
-  if (!x || !y || !w || !grad_x || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) ||
-      !valid_kind(kind) || (value_out && !gauss))
+  const bool tc =
+      batched || (gauss ? tc_routed(kTcConvBwd, D, N, M) : (D > B200OT_MAX_D && tc_capable_dim(D)));
+  const bool shape = batched ? tc_batched_dims(B, N, M, D) : (N > 0 && M > 0 && (supported_simt_dim(D) || tc));
+  if (!x || !y || !w || !grad_x || !scratch || !shape || !valid_kind(kind) || (value_out && !gauss))
     return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
+  if (!blur_ok(kind, blur)) return B200OT_EINVAL;
   if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_kernel_conv_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
-  if (tc) return conv_bwd_tc(x, y, w, center, grad_out, grad_x, value_out, N, M, D, kind, blur, scratch, stream);
+  if (scratch_bytes < (batched ? b200ot_batched_scratch_bytes(B, N, M, D) : b200ot_kernel_conv_scratch_bytes(N, M, D)))
+    return B200OT_ESCRATCH;
+  if (tc)
+    return conv_bwd_tc(x, y, w, center, grad_out, grad_x, value_out, N, M, D, kind, blur, scratch, stream, B, batched);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -805,8 +776,8 @@ B200OT_API int b200ot_kernel_conv_bwd_x(const float* x, const float* y, const fl
                                         int32_t kind, float blur, void* scratch, int64_t scratch_bytes,
                                         void* stream) {
   if (!grad_out) return B200OT_EINVAL;
-  return conv_bwd_x_impl(x, y, w, center, grad_out, grad_x, nullptr, N, M, D, kind, blur, scratch, scratch_bytes,
-                         stream);
+  return conv_bwd_x_impl(x, y, w, center, grad_out, grad_x, nullptr, 1, N, M, D, kind, blur, scratch, scratch_bytes,
+                         stream, false);
 }
 
 B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, const float* w, const float* center,
@@ -814,8 +785,8 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
                                             int32_t kind, float blur, void* scratch, int64_t scratch_bytes,
                                             void* stream) {
   if (!out) return B200OT_EINVAL;
-  return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, N, M, D, kind, blur, scratch, scratch_bytes,
-                         stream);
+  return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, 1, N, M, D, kind, blur, scratch, scratch_bytes,
+                         stream, false);
 }
 
 // ---- batches of B problems in the tensor-core dimensions (tc_reduce_kernel / tc_bwd_kernel with BATCH) ----
@@ -826,24 +797,7 @@ B200OT_API int64_t b200ot_batched_scratch_bytes(int64_t B, int64_t N, int64_t M,
 B200OT_API int b200ot_kernel_conv_fwd_batched(const float* x, const float* y, const float* w, const float* center,
                                               float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
                                               float blur, void* scratch, int64_t scratch_bytes, void* stream) {
-  if (!x || !y || !w || !out || !scratch || !tc_batched_dims(B, N, M, D) || !valid_kind(kind)) return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  return conv_fwd_tc(kind, x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream, B, true);
-}
-
-static int conv_bwd_x_batched_impl(const float* x, const float* y, const float* w, const float* center,
-                                   const float* grad_out, float* grad_x, float* value_out, int64_t B, int64_t N,
-                                   int64_t M, int32_t D, int32_t kind, float blur, void* scratch,
-                                   int64_t scratch_bytes, void* stream) {
-  if (!x || !y || !w || !grad_x || !scratch || !tc_batched_dims(B, N, M, D) || !valid_kind(kind) ||
-      (value_out && kind_base(kind) != B200OT_KERNEL_GAUSSIAN))
-    return B200OT_EINVAL;
-  if (kind_base(kind) != B200OT_KERNEL_ENERGY && !(blur > 0.f)) return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  return conv_bwd_tc(x, y, w, center, grad_out, grad_x, value_out, N, M, D, kind, blur, scratch, stream, B, true);
+  return conv_fwd_impl(x, y, w, center, out, B, N, M, D, kind, blur, scratch, scratch_bytes, stream, true);
 }
 
 B200OT_API int b200ot_kernel_conv_bwd_x_batched(const float* x, const float* y, const float* w, const float* center,
@@ -851,8 +805,8 @@ B200OT_API int b200ot_kernel_conv_bwd_x_batched(const float* x, const float* y, 
                                                 int32_t D, int32_t kind, float blur, void* scratch,
                                                 int64_t scratch_bytes, void* stream) {
   if (!grad_out) return B200OT_EINVAL;
-  return conv_bwd_x_batched_impl(x, y, w, center, grad_out, grad_x, nullptr, B, N, M, D, kind, blur, scratch,
-                                 scratch_bytes, stream);
+  return conv_bwd_x_impl(x, y, w, center, grad_out, grad_x, nullptr, B, N, M, D, kind, blur, scratch, scratch_bytes,
+                         stream, true);
 }
 
 B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float* y, const float* w,
@@ -860,8 +814,8 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float*
                                                     int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
                                                     void* scratch, int64_t scratch_bytes, void* stream) {
   if (!out) return B200OT_EINVAL;
-  return conv_bwd_x_batched_impl(x, y, w, center, nullptr, grad_unit, out, B, N, M, D, kind, blur, scratch,
-                                 scratch_bytes, stream);
+  return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, B, N, M, D, kind, blur, scratch, scratch_bytes,
+                         stream, true);
 }
 
 }  // extern "C"

@@ -170,7 +170,7 @@ static int softmin_bwd_partials(const float* x, const float* y, const float* h_a
   *scale_out = tc ? kTcPScale : 1.f;
   if (tc)
     return bwd_partial_tc(3, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M, D,
-                          scratch, part_out, n_part_out, (cudaStream_t)stream, nullptr);
+                          scratch, part_out, n_part_out, (cudaStream_t)stream);
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
@@ -226,7 +226,7 @@ B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, cons
   int n_part = 0;
   // P carries kTcPScale, which cancels: the finalize divides by each row's sum of P
   const int rc = bwd_partial_tc(3, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M,
-                                D, scratch, &part, &n_part, (cudaStream_t)stream, nullptr, 0.f, nullptr, B, true);
+                                D, scratch, &part, &n_part, (cudaStream_t)stream, B, true);
   if (rc) return rc;
   return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, p, eps, stream);
 }

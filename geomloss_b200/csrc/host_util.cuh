@@ -61,8 +61,9 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
 
 int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
-                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, const float** w_absmax_out,
-                   float clampq = 0.f, const float* coord_absmax = nullptr, int64_t B = 1, bool batched = false);
+                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, int64_t B = 1,
+                   bool batched = false, const float** w_absmax_out = nullptr, float clampq = 0.f,
+                   const float** coord_absmax_out = nullptr);
 
 // Block-sparse softmins on the tensor cores (8 < D <= 64, p = 2; b200ot_*_blocks).  blocks_validate checks the host
 // descriptors (tile-aligned, one segment per row tile) and returns the longest segment in column tiles and the number

@@ -95,89 +95,38 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   static_assert(DK % 16 == 0 && DK <= 64, "padded dimension");
   static_assert(!BLOCKS || (MODE == 3 && !BATCH), "the block-sparse layout serves the softmin of one problem");
   extern __shared__ __align__(1024) unsigned char smem[];
-  const int a_bytes = kTcM * kp * 2;
-  const int b_bytes = kTcBN * kp * 2 + kTcBN * 4;
-  unsigned char* sa = smem;
-  unsigned char* sb = smem + tc_a_span(kp);
-  uint64_t* bar_a = reinterpret_cast<uint64_t*>(sb + NSTAGE * b_bytes);
-  uint64_t* full_b = bar_a + 1;
-  uint64_t* empty_b = full_b + kTcMaxStage;
-
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int split = blockIdx.y;
-  TcBlockSpan bs{};
-  if constexpr (BLOCKS) bs = tc_block_span(bseg, bpieces, blockIdx.x, split, tiles_per_split);
-  const int row_tile = BLOCKS ? bs.row_tile : (int)blockIdx.x;
-  const int elem = BATCH ? row_tile / rtpe : 0;
-  const int t0 = elem * ntiles_b + split * tiles_per_split;
-  const int t1 = min((elem + 1) * ntiles_b, t0 + tiles_per_split);
-  const int nt = BLOCKS ? bs.nt : t1 - t0;
-
-  if (threadIdx.x == 0) {
-    mbar_init(bar_a, 1);
-    for (int s = 0; s < NSTAGE; ++s) {
-      mbar_init(&full_b[s], 1);
-      mbar_init(&empty_b[s], 4 * kTcWG);  // every consumer warp, once GEMM 2 and the weight reads are done
-    }
-    mbar_fence_init();
-  }
-  __syncthreads();
-
+  const TcCta c = tc_cta_prologue<BATCH, BLOCKS>(smem, kp, NSTAGE, ntiles_b, tiles_per_split, rtpe, bseg, bpieces);
   if (warp == 4 * kTcWG) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      mbar_arrive_expect_tx(bar_a, a_bytes);
-      tma_load_1d(sa, a_imgs + (int64_t)row_tile * a_bytes, a_bytes, bar_a);
-      int pc = bs.piece, off = bs.off;  // BLOCKS: position in the segment's pieces
-      for (int k = 0; k < nt; ++k) {
-        const int st = k % NSTAGE;
-        if (k >= NSTAGE) mbar_wait(&empty_b[st], ((k / NSTAGE) + 1) & 1);
-        mbar_arrive_expect_tx(&full_b[st], b_bytes);
-        int ct = t0 + k;
-        if constexpr (BLOCKS) {
-          const int2 pp = bpieces[pc];
-          ct = pp.x / kTcBN + off;
-          if (++off == pp.y / kTcBN) {
-            ++pc;
-            off = 0;
-          }
-        }
-        tma_load_1d(sb + st * b_bytes, b_imgs + (int64_t)ct * b_bytes, b_bytes, &full_b[st]);
-      }
-    }
+    tc_produce<BLOCKS>(c, a_imgs, b_imgs, bpieces, NSTAGE, lane);
     return;
   }
   // ===== consumer warpgroups =====
   const int wg = warp >> 2;
-  const uint32_t a_addr = smem_u32(sa) + wg * 64 * 16;
-  const int64_t row0 = (int64_t)row_tile * kTcM + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // and row0 + 8
+  const uint32_t a_addr = smem_u32(c.sa) + wg * 64 * 16;
+  const int64_t row0 = (int64_t)c.row_tile * kTcM + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // and row0 + 8
   const int cq = 2 * (lane & 3);
   float g[DK];  // [G_a | G_b]: columns 0..DK-1 in g[0 .. DK/2), DK..2DK-1 in g[DK/2 .. DK)
 #pragma unroll
   for (int i = 0; i < DK; ++i) g[i] = 0.f;
   float sum[2] = {0.f, 0.f};
-  mbar_wait(bar_a, 0);
+  mbar_wait(c.bar_a, 0);
   float tb[2] = {0.f, 0.f};  // MODE 4 / 5: coincidence bound of each row
-  if constexpr (MODE >= 4) {
-    clampq = tc_norm_clampq(clampq, coord_absmax);
-    const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    tb[0] = tc_norm_row_bound(sa, kp, lr, clampq);
-    tb[1] = tc_norm_row_bound(sa, kp, lr + 8, clampq);
-  }
-  for (int k = 0; k < nt; ++k) {
+  if constexpr (MODE >= 4) tc_norm_row_bounds(tb, clampq, coord_absmax, c.sa, kp, wg, warp, lane);
+  for (int k = 0; k < c.nt; ++k) {
     const int st = k % NSTAGE;
-    mbar_wait(&full_b[st], (k / NSTAGE) & 1);
-    const uint32_t b_addr = smem_u32(sb + st * b_bytes);
+    mbar_wait(&c.full_b[st], (k / NSTAGE) & 1);
+    const uint32_t b_addr = smem_u32(c.sb + st * c.b_bytes);
     // ---- GEMM 1: S ----
     float s[64];
     tc_exponent_gemm(s, a_addr, b_addr, DK / 8);
     wgmma_wait<0>();
     reg_fence(s);
     if constexpr (MODE != 3) {
-      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(t0 + k) * kTcBN, cq);
+      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
     }
     // ---- S -> P, packed as the A fragments of GEMM 2 (ph[2 n8 + h] = the pair of row h in 8-column block n8) ----
-    const float* wts = reinterpret_cast<const float*>(sb + st * b_bytes + kTcBN * kp * 2);
+    const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
     uint32_t ph[32], pl[PT == 2 ? 32 : 1];
     float ts[2] = {0.f, 0.f};
 #pragma unroll
@@ -233,7 +182,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     wgmma_wait<0>();
     reg_fence(g);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_b[st]);  // the column tile may be overwritten
+    if (lane == 0) mbar_arrive(&c.empty_b[st]);  // the column tile may be overwritten
   }
   // ---- row sums over the quad, gradient sums out ----
 #pragma unroll
@@ -241,17 +190,9 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     float tot = sum[h];
     tot += __shfl_xor_sync(0xffffffffu, tot, 1);
     tot += __shfl_xor_sync(0xffffffffu, tot, 2);
-    int64_t row = row0 + 8 * h;
-    if constexpr (BATCH) {
-      const int64_t local = row - (int64_t)elem * rtpe * kTcM;
-      row = local < n_local ? (int64_t)elem * n_local + local : N;
-    }
-    if constexpr (BLOCKS) {
-      const int g = row_src[row];
-      row = g >= 0 ? g : N;
-    }
+    const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, c.elem, rtpe, n_local, row_src, N);
     if (row < N) {
-      float* dst = part + ((int64_t)split * N + row) * (D + 1);
+      float* dst = part + ((int64_t)c.split * N + row) * (D + 1);
       if (cq == 0) dst[0] = tot;
 #pragma unroll
       for (int j = 0; j < DK / 2; ++j) {

@@ -252,9 +252,19 @@ __device__ __forceinline__ float tc_norm_clampq(float clampq, const float* coord
   }
   return fmaxf(clampq, 1e-30f);
 }
-// k(d) of one pair from its exponent s: d^2 = clamp for a pair below the row bound t (and the diagonal), else -2 s
+// MODE 4 / 5: the clamp (scaled in place) and the coincidence bounds tb of the thread's two rows of the row image
+__device__ __forceinline__ void tc_norm_row_bounds(float (&tb)[2], float& clampq, const float* coord_absmax,
+                                                   const unsigned char* sa, int kp, int wg, int warp, int lane) {
+  clampq = tc_norm_clampq(clampq, coord_absmax);
+  const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  tb[0] = tc_norm_row_bound(sa, kp, lr, clampq);
+  tb[1] = tc_norm_row_bound(sa, kp, lr + 8, clampq);
+}
+// The weighted value of one pair from its exponent s: 2^s (MODE 0), or k(d) with d^2 = clamp for a pair below the row
+// bound t (and the diagonal), else -2 s (MODE 4 / 5)
 template <int MODE>
-__device__ __forceinline__ float tc_norm_value(float s, float t, float clampq) {
+__device__ __forceinline__ float tc_pair_value(float s, float t, float clampq) {
+  if constexpr (MODE == 0) return ex2_approx(s);
   const float q = -2.f * s;
   const float d2 = q < t ? clampq : q;
   const float d = d2 * rsqrt_approx(d2);
@@ -291,6 +301,95 @@ __device__ __forceinline__ TcBlockSpan tc_block_span(const int4* __restrict__ se
   return r;
 }
 
+// What tc_reduce_kernel and tc_bwd_kernel share before their consumer loops.  Shared memory: the row image `sa`, the
+// ring of NSTAGE column slots `sb` and the mbarriers behind it.  The CTA's work: row tile `row_tile` (of batch element
+// `elem`) against the nt column tiles of split `split` from tile t0 (BLOCKS: from tile bs.off of piece bs.piece).
+struct TcCta {
+  unsigned char *sa, *sb;
+  uint64_t *bar_a, *full_b, *empty_b;
+  int a_bytes, b_bytes;
+  int split, row_tile, elem, t0, nt;
+  TcBlockSpan bs;
+};
+// Carves the shared memory, finds the CTA's tiles and initialises the barriers (the CTA's threads all call it)
+template <bool BATCH, bool BLOCKS>
+__device__ __forceinline__ TcCta tc_cta_prologue(unsigned char* smem, int kp, int NSTAGE, int ntiles_b,
+                                                 int tiles_per_split, int rtpe, const int4* __restrict__ bseg,
+                                                 const int2* __restrict__ bpieces) {
+  TcCta c;
+  c.a_bytes = kTcM * kp * 2;
+  c.b_bytes = kTcBN * kp * 2 + kTcBN * 4;
+  c.sa = smem;
+  c.sb = smem + tc_a_span(kp);
+  c.bar_a = reinterpret_cast<uint64_t*>(c.sb + NSTAGE * c.b_bytes);
+  c.full_b = c.bar_a + 1;
+  c.empty_b = c.full_b + kTcMaxStage;
+
+  c.split = blockIdx.y;
+  c.bs = TcBlockSpan{};
+  if constexpr (BLOCKS) c.bs = tc_block_span(bseg, bpieces, blockIdx.x, c.split, tiles_per_split);
+  c.row_tile = BLOCKS ? c.bs.row_tile : (int)blockIdx.x;
+  c.elem = BATCH ? c.row_tile / rtpe : 0;
+  c.t0 = c.elem * ntiles_b + c.split * tiles_per_split;
+  const int t1 = min((c.elem + 1) * ntiles_b, c.t0 + tiles_per_split);
+  c.nt = BLOCKS ? c.bs.nt : t1 - c.t0;
+
+  if (threadIdx.x == 0) {
+    mbar_init(c.bar_a, 1);
+    for (int s = 0; s < NSTAGE; ++s) {
+      mbar_init(&c.full_b[s], 1);
+      mbar_init(&c.empty_b[s], 4 * kTcWG);  // every consumer warp, once its MMAs and weight reads are done
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  return c;
+}
+
+// The TMA producer (one lane of the warp behind the warpgroups): the row image once, then the CTA's column tiles
+// through the ring
+template <bool BLOCKS>
+__device__ __forceinline__ void tc_produce(const TcCta& c, const unsigned char* __restrict__ a_imgs,
+                                           const unsigned char* __restrict__ b_imgs,
+                                           const int2* __restrict__ bpieces, int NSTAGE, int lane) {
+  if (lane == 0) {
+    mbar_arrive_expect_tx(c.bar_a, c.a_bytes);
+    tma_load_1d(c.sa, a_imgs + (int64_t)c.row_tile * c.a_bytes, c.a_bytes, c.bar_a);
+    int pc = c.bs.piece, off = c.bs.off;  // BLOCKS: position in the segment's pieces
+    for (int k = 0; k < c.nt; ++k) {
+      const int st = k % NSTAGE;
+      if (k >= NSTAGE) mbar_wait(&c.empty_b[st], ((k / NSTAGE) + 1) & 1);
+      mbar_arrive_expect_tx(&c.full_b[st], c.b_bytes);
+      int ct = c.t0 + k;
+      if constexpr (BLOCKS) {
+        const int2 pp = bpieces[pc];
+        ct = pp.x / kTcBN + off;
+        if (++off == pp.y / kTcBN) {
+          ++pc;
+          off = 0;
+        }
+      }
+      tma_load_1d(c.sb + st * c.b_bytes, b_imgs + (int64_t)ct * c.b_bytes, c.b_bytes, &c.full_b[st]);
+    }
+  }
+}
+
+// The output row of tile row `row`: BATCH, row b n_local + local of a live row of element b; BLOCKS, row_src of the
+// slot.  N for a padding row, which writes nothing.
+template <bool BATCH, bool BLOCKS>
+__device__ __forceinline__ int64_t tc_out_row(int64_t row, int elem, int rtpe, int64_t n_local,
+                                              const int* __restrict__ row_src, int64_t N) {
+  if constexpr (BATCH) {
+    const int64_t local = row - (int64_t)elem * rtpe * kTcM;
+    row = local < n_local ? (int64_t)elem * n_local + local : N;
+  }
+  if constexpr (BLOCKS) {
+    const int g = row_src[row];
+    row = g >= 0 ? g : N;
+  }
+  return row;
+}
+
 // MODE 0: gaussian kernel conv  part[(split*kTcParts + q)*N + row]   = sum_j w_j 2^S_ij
 // MODE 1: softmin               part2[(split*kTcParts + q)*N + row]  = (m, s) with sum_j 2^S_ij = s 2^m  (lazy max,
 //         sum-guarded exactly like softmin.cuh; same partial format as softmin_partial_kernel)
@@ -323,107 +422,41 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   static_assert(MODE == 0 || MODE == 1 || MODE == 4 || MODE == 5, "row gradients live in tcbwd.cuh");
   static_assert(!BLOCKS || (MODE == 1 && !BATCH), "the block-sparse layout serves the softmin of one problem");
   extern __shared__ __align__(1024) unsigned char smem[];
-  const int a_bytes = kTcM * kp * 2;
-  const int b_bytes = kTcBN * kp * 2 + kTcBN * 4;
-  unsigned char* sa = smem;
-  unsigned char* sb = smem + tc_a_span(kp);
-  uint64_t* bar_a = reinterpret_cast<uint64_t*>(sb + NSTAGE * b_bytes);
-  uint64_t* full_b = bar_a + 1;
-  uint64_t* empty_b = full_b + kTcMaxStage;
-
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int split = blockIdx.y;
-  TcBlockSpan bs{};
-  if constexpr (BLOCKS) bs = tc_block_span(bseg, bpieces, blockIdx.x, split, tiles_per_split);
-  const int row_tile = BLOCKS ? bs.row_tile : (int)blockIdx.x;
-  const int elem = BATCH ? row_tile / rtpe : 0;
-  const int t0 = elem * ntiles_b + split * tiles_per_split;
-  const int t1 = min((elem + 1) * ntiles_b, t0 + tiles_per_split);
-  const int nt = BLOCKS ? bs.nt : t1 - t0;
-
-  if (threadIdx.x == 0) {
-    mbar_init(bar_a, 1);
-    for (int s = 0; s < NSTAGE; ++s) {
-      mbar_init(&full_b[s], 1);
-      mbar_init(&empty_b[s], 4 * kTcWG);  // every consumer warp (it reads the weights after its MMAs)
-    }
-    mbar_fence_init();
-  }
-  __syncthreads();
-
+  const TcCta c = tc_cta_prologue<BATCH, BLOCKS>(smem, kp, NSTAGE, ntiles_b, tiles_per_split, rtpe, bseg, bpieces);
   if (warp == 4 * kTcWG) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      mbar_arrive_expect_tx(bar_a, a_bytes);
-      tma_load_1d(sa, a_imgs + (int64_t)row_tile * a_bytes, a_bytes, bar_a);
-      int pc = bs.piece, off = bs.off;  // BLOCKS: position in the segment's pieces
-      for (int k = 0; k < nt; ++k) {
-        const int st = k % NSTAGE;
-        if (k >= NSTAGE) mbar_wait(&empty_b[st], ((k / NSTAGE) + 1) & 1);
-        mbar_arrive_expect_tx(&full_b[st], b_bytes);
-        int ct = t0 + k;
-        if constexpr (BLOCKS) {
-          const int2 pp = bpieces[pc];
-          ct = pp.x / kTcBN + off;
-          if (++off == pp.y / kTcBN) {
-            ++pc;
-            off = 0;
-          }
-        }
-        tma_load_1d(sb + st * b_bytes, b_imgs + (int64_t)ct * b_bytes, b_bytes, &full_b[st]);
-      }
-    }
+    tc_produce<BLOCKS>(c, a_imgs, b_imgs, bpieces, NSTAGE, lane);
     return;
   }
   // ===== consumer warpgroups: wgmma -> exp2 -> row sums =====
   const int wg = warp >> 2;
   const int seg = tc_dk_of_kp(kp) / 8;  // 8-element chunks per split term
-  const uint32_t a_addr = smem_u32(sa) + wg * 64 * 16;
-  const int64_t row0 = (int64_t)row_tile * kTcM + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // and row0 + 8
+  const uint32_t a_addr = smem_u32(c.sa) + wg * 64 * 16;
+  const int64_t row0 = (int64_t)c.row_tile * kTcM + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // and row0 + 8
   const int cq = 2 * (lane & 3);  // this thread's first column in every 8-column block
-  float acc[2] = {0.f, 0.f};                 // MODE 0: weighted sums
+  float acc[2] = {0.f, 0.f};                 // MODE 0, 4, 5: weighted sums
   float m[2] = {kNegBig, kNegBig}, srun[2] = {0.f, 0.f};  // MODE 1: running (m, s)
-  mbar_wait(bar_a, 0);
+  mbar_wait(c.bar_a, 0);
   float tb[2] = {0.f, 0.f};  // MODE 4 / 5: coincidence bound of each row
-  if constexpr (MODE >= 4) {
-    clampq = tc_norm_clampq(clampq, coord_absmax);
-    const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    tb[0] = tc_norm_row_bound(sa, kp, lr, clampq);
-    tb[1] = tc_norm_row_bound(sa, kp, lr + 8, clampq);
-  }
-  for (int k = 0; k < nt; ++k) {
+  if constexpr (MODE >= 4) tc_norm_row_bounds(tb, clampq, coord_absmax, c.sa, kp, wg, warp, lane);
+  for (int k = 0; k < c.nt; ++k) {
     const int st = k % NSTAGE;
-    mbar_wait(&full_b[st], (k / NSTAGE) & 1);
+    mbar_wait(&c.full_b[st], (k / NSTAGE) & 1);
     float s[64];
-    tc_exponent_gemm(s, a_addr, smem_u32(sb + st * b_bytes), seg);
+    tc_exponent_gemm(s, a_addr, smem_u32(c.sb + st * c.b_bytes), seg);
     wgmma_wait<0>();
     reg_fence(s);
-    if constexpr (MODE == 0) {
-      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(t0 + k) * kTcBN, cq);
-      const float* wts = reinterpret_cast<const float*>(sb + st * b_bytes + kTcBN * kp * 2);
+    if constexpr (MODE != 1) {
+      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
+      const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
       float ts[2] = {0.f, 0.f};
 #pragma unroll
       for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
         const float2 w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          ts[h] = fmaf(ex2_approx(s[4 * n8 + 2 * h]), w.x, ts[h]);
-          ts[h] = fmaf(ex2_approx(s[4 * n8 + 2 * h + 1]), w.y, ts[h]);
-        }
-      }
-      acc[0] += ts[0];
-      acc[1] += ts[1];
-    } else if constexpr (MODE >= 4) {
-      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(t0 + k) * kTcBN, cq);
-      const float* wts = reinterpret_cast<const float*>(sb + st * b_bytes + kTcBN * kp * 2);
-      float ts[2] = {0.f, 0.f};
-#pragma unroll
-      for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
-        const float2 w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          ts[h] = fmaf(tc_norm_value<MODE>(s[4 * n8 + 2 * h], tb[h], clampq), w.x, ts[h]);
-          ts[h] = fmaf(tc_norm_value<MODE>(s[4 * n8 + 2 * h + 1], tb[h], clampq), w.y, ts[h]);
+          ts[h] = fmaf(tc_pair_value<MODE>(s[4 * n8 + 2 * h], tb[h], clampq), w.x, ts[h]);
+          ts[h] = fmaf(tc_pair_value<MODE>(s[4 * n8 + 2 * h + 1], tb[h], clampq), w.y, ts[h]);
         }
       }
       acc[0] += ts[0];
@@ -457,25 +490,17 @@ __global__ void __launch_bounds__(kTcThreads, 1)
       }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_b[st]);
+    if (lane == 0) mbar_arrive(&c.empty_b[st]);
   }
   const int q = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    int64_t row = row0 + 8 * h;
-    if constexpr (BATCH) {
-      const int64_t local = row - (int64_t)elem * rtpe * kTcM;
-      row = local < n_local ? (int64_t)elem * n_local + local : N;
-    }
-    if constexpr (BLOCKS) {
-      const int g = row_src[row];
-      row = g >= 0 ? g : N;
-    }
+    const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, c.elem, rtpe, n_local, row_src, N);
     if (row < N) {
       if constexpr (MODE != 1) {
-        part[((int64_t)split * kTcParts + q) * N + row] = acc[h];
+        part[((int64_t)c.split * kTcParts + q) * N + row] = acc[h];
       } else {
-        reinterpret_cast<float2*>(part)[((int64_t)split * kTcParts + q) * N + row] = make_float2(m[h], srun[h]);
+        reinterpret_cast<float2*>(part)[((int64_t)c.split * kTcParts + q) * N + row] = make_float2(m[h], srun[h]);
       }
     }
   }
