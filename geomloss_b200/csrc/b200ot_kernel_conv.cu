@@ -297,9 +297,9 @@ static TcBwdTuning tc_bwd_tuning() {
 
 // The plan of a launch group: `ctas` row CTAs, each reading up to `tiles` (>= 1) column tiles.  The split count is
 // chosen for the whole grid and cuts those tiles.  Behind the images: the partials of `rows` rows ((m, s) pairs forward, D+1
-// sums per row backward), then a misc block of misc_bytes.
+// sums per row backward, D+2 for the p = 1 softmin: `head` sums ahead of the D), then a misc block of misc_bytes.
 static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, int64_t ctas, int64_t tiles, int64_t rows,
-                           int64_t misc_bytes) {
+                           int64_t misc_bytes, int head = 1) {
   TcPlan p;
   p.kp = tc_kp(D);
   p.rtpe = p.ctpe = 0;
@@ -323,7 +323,7 @@ static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, in
   p.n_split = (int)ceil_div64(tiles, p.tiles_per_split);
   p.off_b = round_up64(a_tiles * tc_a_img_bytes(p.kp), 256);
   p.off_part = p.off_b + round_up64(b_tiles * b_bytes, 256);
-  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? rows * (D + 1) : kTcParts * rows * 2) * 4, 256);
+  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? rows * (D + head) : kTcParts * rows * 2) * 4, 256);
   p.total = p.off_misc + round_up64(misc_bytes, 256);
   return p;
 }
@@ -331,9 +331,9 @@ static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, in
 // B problems of N rows x M columns side by side (B = 1: one problem), each element padded to whole tiles on its own
 // (tc_pack_kernel).  The splits cut each element's ctpe column tiles, so a CTA never reads another element's columns.
 // Misc block: [0] the energy coordinate maximum, [1 + b] max|w| of element b.
-static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B = 1) {
+static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B = 1, int head = 1) {
   const int rtpe = (int)ceil_div64(N, kTcM), ctpe = (int)ceil_div64(M, kTcBN);
-  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4);
+  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4, head);
   p.rtpe = rtpe;
   p.ctpe = ctpe;
   return p;
@@ -344,10 +344,15 @@ int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
   return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B).total);
 }
 
+// the p = 1 softmin's row gradient keeps D + 2 sums per row
+int64_t tc_l1_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
+  return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B, 2).total);
+}
+
 // What the images of a launch group hold (tc_pack_kernel): the row cloud x and the column cloud y, centred at `center`
 // and multiplied by `scale`; B elements of N rows / M columns, or N / M block-sparse slots gathered through row_src /
 // col_src.  Besides the coordinates: the column weights w, the softmin's column terms h_a + h_scale_b h_b and the
-// softmin row gradient's row term lse2.
+// softmin row gradient's row term lse2.  l1_c = log2e / eps > 0: the p = 1 softmin's layout (tc_pack_kernel's l1).
 struct TcOperands {
   const float *x, *y, *center;
   float scale;
@@ -358,6 +363,7 @@ struct TcOperands {
   float h_scale_b = 0.f;
   const float* lse2 = nullptr;
   const int *row_src = nullptr, *col_src = nullptr;
+  float l1_c = 0.f;
 };
 
 // Packs both images of plan p.  Asked for through a non-null out pointer, it first computes into the misc block:
@@ -392,12 +398,12 @@ static int tc_pack(const TcPlan& p, unsigned char* base, const TcOperands& o, cu
   }
   const int threads = 128;
   tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      o.x, nullptr, nullptr, nullptr, 0.f, 0.f, o.center, o.scale, o.N, o.D, p.kp, kTcM, 0, base, o.lse2, nullptr, cmax,
-      o.B, o.row_src);
+      o.x, nullptr, nullptr, nullptr, 0.f, o.l1_c, o.center, o.scale, o.N, o.D, p.kp, kTcM, 0, base, o.lse2, nullptr, cmax,
+      o.B, o.row_src, o.l1_c > 0.f);
   B200OT_CUDA_TRY(cudaGetLastError());
   tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
       o.y, o.w, o.h_a, o.h_b, o.h_scale_b, kLog2e, o.center, o.scale, o.M, o.D, p.kp, kTcBN, 1, base + p.off_b, nullptr,
-      wmax, cmax, o.B, o.col_src);
+      wmax, cmax, o.B, o.col_src, o.l1_c > 0.f);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
@@ -487,6 +493,63 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
   if (rc) return rc;
   *part_out = reinterpret_cast<float*>(base + p.off_part);
   *n_part_out = p.n_split * kTcParts;
+  return B200OT_OK;
+}
+
+// The p = 1 softmin of B elements of N rows / M columns (B = 1: one problem) on the tensor cores (tcconv.cuh, MODE 6 / 7):
+// packs both clouds on the energy's coordinates and runs the forward reduction (bwd = false: n_part (m, s) sets for
+// b200ot_softmin_finalize) or the row-gradient sums (bwd, lse2 = the forward's: n_part sets of (B N, D+2) sums).
+// *coord_absmax_out: the coordinate maximum the pass derived its scale from.  Arguments already validated.
+int softmin_l1_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                  const float* center, const float* lse2, int64_t B, int64_t N, int64_t M, int D, int p, float eps,
+                  void* scratch, float** part_out, int* n_part_out, const float** coord_absmax_out, cudaStream_t st) {
+  const TcPlan pl = make_tc_plan(N, M, D, bwd, B, bwd ? 2 : 1);
+  if (pl.nstage < 1) return B200OT_EINVAL;
+  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
+  const float* coord_absmax = nullptr;
+  TcOperands o{x, y, center, 1.f, N, M, D, B, nullptr, h_a, h_b, h_scale_b, bwd ? lse2 : nullptr};
+  o.l1_c = kLog2e / eps;
+  int rc = tc_pack(pl, base, o, st, nullptr, &coord_absmax);
+  if (rc) return rc;
+  const TcKernel kern = bwd ? tc_bwd_dk<7, 2, true, true>(D) : tc_reduce_kernel<6, true>;
+  const int self_mode = (x == y && N == M) ? 1 : 0;  // xx / yy: the diagonal takes d = sqrt(clamp) exactly
+  rc = tc_launch(kern, pl, base, B * N, N, D, self_mode, cost_clamp(p), coord_absmax, st);
+  if (rc) return rc;
+  *part_out = reinterpret_cast<float*>(base + pl.off_part);
+  *n_part_out = bwd ? pl.n_split : pl.n_split * kTcParts;
+  *coord_absmax_out = coord_absmax;
+  return B200OT_OK;
+}
+
+// p = 1 on the tensor cores: part (n_split, N, D+2) with [0] = sum P, [1] = sum Q, [2+k] = sum Q Y_k (tcbwd.cuh, MODE 7)
+// -> grad_x = go (X_i sum Q - sum Q Y) / sum P, X = scale (x - center) with the pass's coordinate scale
+__global__ void softmin_l1_bwd_finalize_kernel(const float* __restrict__ part, int n_split,
+                                               const float* __restrict__ x, const float* __restrict__ center,
+                                               const float* __restrict__ grad_out, float* __restrict__ grad_x,
+                                               int64_t N, int D, const float* __restrict__ coord_absmax) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int na = D + 2;
+  const float scale = tc_energy_coord_scale(*coord_absmax);
+  float sp = 0.f, sq = 0.f;
+  for (int s = 0; s < n_split; ++s) {
+    sp += part[((int64_t)s * N + i) * na];
+    sq += part[((int64_t)s * N + i) * na + 1];
+  }
+  const float go = sp > 0.f ? grad_out[i] / sp : 0.f;
+  for (int k = 0; k < D; ++k) {
+    float a = 0.f;
+    for (int s = 0; s < n_split; ++s) a += part[((int64_t)s * N + i) * na + 2 + k];
+    const float X = scale * (x[i * D + k] - (center ? center[k] : 0.f));
+    grad_x[i * D + k] = go * (X * sq - a);
+  }
+}
+
+int softmin_l1_bwd_finalize(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
+                            float* grad_x, int64_t N, int D, const float* coord_absmax, cudaStream_t st) {
+  softmin_l1_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(part, n_part, x, center, grad_out,
+                                                                               grad_x, N, D, coord_absmax);
+  B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
 

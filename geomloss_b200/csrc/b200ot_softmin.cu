@@ -307,6 +307,29 @@ B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const 
   return b200ot_softmin_finalize(tc_part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
 }
 
+// ---- the p = 1 softmin in the tensor-core dimensions (tc_reduce_kernel<6> / tc_bwd_kernel<7>, batched flavour) ----
+B200OT_API int64_t b200ot_softmin_l1_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
+  return tc_l1_args(B, N, M, D, 1) ? tc_l1_scratch_bytes(N, M, D, B) : 0;
+}
+
+B200OT_API int b200ot_softmin_l1_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
+                                     float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                     float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
+                                     int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                     void* stream) {
+  if (!x || !y || !h_a || !scratch || !tc_l1_args(B, N, M, D, p) || !(eps > 0.f) || (!out && !lse2_out))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_softmin_l1_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  const float* coord_absmax = nullptr;
+  const int rc = softmin_l1_tc(false, x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps, scratch, &part,
+                               &n_part, &coord_absmax, (cudaStream_t)stream);
+  if (rc) return rc;
+  return b200ot_softmin_finalize(part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
+}
+
 B200OT_API void b200ot_blocks_shape(int32_t* rows_per_segment, int32_t* col_align) {
   if (rows_per_segment) *rows_per_segment = kTcBlocksTile;
   if (col_align) *col_align = kTcBlocksTile;

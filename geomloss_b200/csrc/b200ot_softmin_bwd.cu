@@ -231,6 +231,24 @@ B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, cons
   return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, p, eps, stream);
 }
 
+B200OT_API int b200ot_softmin_l1_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
+                                       float h_scale_b, const float* center, const float* lse2, const float* grad_out,
+                                       float* grad_x, int64_t B, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
+                                       void* scratch, int64_t scratch_bytes, void* stream) {
+  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_l1_args(B, N, M, D, p) || !(eps > 0.f))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_softmin_l1_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  const float* coord_absmax = nullptr;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = softmin_l1_tc(true, x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps, scratch, &part,
+                               &n_part, &coord_absmax, st);
+  if (rc) return rc;
+  return softmin_l1_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, coord_absmax, st);
+}
+
 B200OT_API int b200ot_softmin_bwd_x_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
                                            float h_scale_b, const float* center, const float* lse2,
                                            const float* grad_out, float* grad_x, int64_t N, const int32_t* row_src,

@@ -59,6 +59,18 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
                        const float* center, int64_t N, int64_t M, int D, float eps, void* scratch,
                        float** part_out, int* n_part_out, cudaStream_t st, int64_t B = 1, bool batched = false);
 
+// The p = 1 softmin on the tensor cores (b200ot_softmin_l1_*): B >= 1 elements, 8 < D <= 64, p = 1 | UNCLAMPED
+inline bool tc_l1_args(int64_t B, int64_t N, int64_t M, int D, int p) {
+  return tc_batched_dims(B, N, M, D) && valid_p(p) && p_exponent(p) == 1;
+}
+int64_t tc_l1_scratch_bytes(int64_t N, int64_t M, int D, int64_t B);
+int softmin_l1_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                  const float* center, const float* lse2, int64_t B, int64_t N, int64_t M, int D, int p, float eps,
+                  void* scratch, float** part_out, int* n_part_out, const float** coord_absmax_out, cudaStream_t st);
+// grad_x of the N rows from softmin_l1_tc's row-gradient sums
+int softmin_l1_bwd_finalize(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
+                            float* grad_x, int64_t N, int D, const float* coord_absmax, cudaStream_t st);
+
 int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
                    void* scratch, float** part_out, int* n_part_out, cudaStream_t st, int64_t B = 1,

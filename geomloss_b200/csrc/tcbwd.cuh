@@ -70,6 +70,9 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t d
 //
 // self_mode: rows and columns are the same cloud (the K_xx term): the exponent of pair (i, i) is exactly 0, as in
 // tc_reduce_kernel — matters when sum_j P_ij is used as the forward VALUE (b200ot_kernel_conv_fwd_bwd_x).
+// MODE 7: p = 1 softmin row gradient (tcconv.cuh, kTcL1QLog2): P = 2^(H_j - c d_ij - lse2_i + k_i), Q = P / d_ij (0 below
+// the row's coincidence bound); GEMM 2 takes Q.  part[(split*N + row)*(D+2) + {0, 1, 2+k}] = {sum P, sum Q, sum Q Y_k}
+// (the coincident pairs weigh in sum P only), finalized as (X_i sum Q - sum Q Y) / sum P.
 // MODE 4 / 5: P of one pair from its exponent s (the rsqrt of a pair below the bound t is discarded by the select)
 template <int MODE>
 __device__ __forceinline__ float tc_norm_p(float s, float t, float w) {
@@ -78,6 +81,15 @@ __device__ __forceinline__ float tc_norm_p(float s, float t, float w) {
   float p = w * r;
   if constexpr (MODE == 4) p *= ex2_approx(-(q * r));
   return q < t ? 0.f : p;
+}
+
+// MODE 7: (P, Q) of one pair from its exponent s, the column's H and the row's rt = (c, k_i - lse2_i)
+__device__ __forceinline__ float2 tc_l1_pq(float s, float t, float clampq, float H, float2 rt) {
+  const float q = -2.f * s;
+  const float d2 = q < t ? clampq : q;
+  const float r = rsqrt_approx(d2);
+  const float p = ex2_approx(fmaf(-rt.x, d2 * r, H) + rt.y);
+  return make_float2(p, q < t ? 0.f : p * r);
 }
 
 // BATCH: B problems side by side, laid out and mapped to rows and column tiles as in tc_reduce_kernel (tcconv.cuh).
@@ -90,10 +102,11 @@ __global__ void __launch_bounds__(kTcThreads, 1)
                   int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe, int64_t n_local,
                   const int4* __restrict__ bseg = nullptr, const int2* __restrict__ bpieces = nullptr,
                   const int* __restrict__ row_src = nullptr) {
-  static_assert(MODE == 2 || MODE == 3 || MODE == 4 || MODE == 5, "row-gradient modes");
+  static_assert(MODE == 2 || MODE == 3 || MODE == 4 || MODE == 5 || MODE == 7, "row-gradient modes");
   static_assert(PT == 1 || PT == 2, "P is fed to GEMM 2 as one or two fp16 terms");
   static_assert(DK % 16 == 0 && DK <= 64, "padded dimension");
   static_assert(!BLOCKS || (MODE == 3 && !BATCH), "the block-sparse layout serves the softmin of one problem");
+  static_assert(MODE != 7 || PT == 2, "the p = 1 row gradient sums P and Q apart: two fp16 terms of Q");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const TcCta c = tc_cta_prologue<BATCH, BLOCKS>(smem, kp, NSTAGE, ntiles_b, tiles_per_split, rtpe, bseg, bpieces);
@@ -110,9 +123,19 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 #pragma unroll
   for (int i = 0; i < DK; ++i) g[i] = 0.f;
   float sum[2] = {0.f, 0.f};
+  float sumq[2] = {0.f, 0.f};  // MODE 7: sum_j Q_ij (sum holds sum_j P_ij)
   mbar_wait(c.bar_a, 0);
-  float tb[2] = {0.f, 0.f};  // MODE 4 / 5: coincidence bound of each row
+  float tb[2] = {0.f, 0.f};  // MODE 4 / 5 / 7: coincidence bound of each row
   if constexpr (MODE >= 4) tc_norm_row_bounds(tb, clampq, coord_absmax, c.sa, kp, wg, warp, lane);
+  float2 rt[2] = {};  // MODE 7: (c, k_i - lse2_i) of each row
+  if constexpr (MODE == 7) {
+    tc_l1_rows(rt, c.sa, kp, wg, warp, lane);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int e = ((__float_as_int(tb[h]) >> 23) & 0xff) - 127;  // 2^e <= T_i < 2^(e+1): T_i is normal
+      rt[h].y = (float)(kTcL1QLog2 + (e >> 1)) - rt[h].y;
+    }
+  }
   for (int k = 0; k < c.nt; ++k) {
     const int st = k % NSTAGE;
     mbar_wait(&c.full_b[st], (k / NSTAGE) & 1);
@@ -125,6 +148,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     if constexpr (MODE != 3) {
       if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
     }
+    float tq[2] = {0.f, 0.f};
     // ---- S -> P, packed as the A fragments of GEMM 2 (ph[2 n8 + h] = the pair of row h in 8-column block n8) ----
     const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
     uint32_t ph[32], pl[PT == 2 ? 32 : 1];
@@ -133,14 +157,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
       float2 w = make_float2(1.f, 1.f);
       if constexpr (MODE != 3) w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
-      if constexpr (MODE >= 4) {
+      if constexpr (MODE == 4 || MODE == 5) {
         w.x *= 1.f / (float)(1 << kTcNormPLog2);
         w.y *= 1.f / (float)(1 << kTcNormPLog2);
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         float p0, p1;
-        if constexpr (MODE >= 4) {
+        if constexpr (MODE == 7) {
+          // w = (H_j, H_j+1); ts sums P, tq and GEMM 2 take Q
+          const float2 pq0 = tc_l1_pq(s[4 * n8 + 2 * h], tb[h], clampq, w.x, rt[h]);
+          const float2 pq1 = tc_l1_pq(s[4 * n8 + 2 * h + 1], tb[h], clampq, w.y, rt[h]);
+          ts[h] += pq0.x + pq1.x;
+          p0 = pq0.y;
+          p1 = pq1.y;
+        } else if constexpr (MODE >= 4) {
           p0 = tc_norm_p<MODE>(s[4 * n8 + 2 * h], tb[h], w.x);
           p1 = tc_norm_p<MODE>(s[4 * n8 + 2 * h + 1], tb[h], w.y);
         } else {
@@ -155,7 +186,11 @@ __global__ void __launch_bounds__(kTcThreads, 1)
         ph[2 * n8 + h] = hh;
         const float2 hf = unpack_f16x2(hh);
         if constexpr (PT == 2) {
-          ts[h] += p0 + p1;
+          if constexpr (MODE == 7) {
+            tq[h] += p0 + p1;
+          } else {
+            ts[h] += p0 + p1;
+          }
           pl[2 * n8 + h] = pack_f16x2(p0 - hf.x, p1 - hf.y);
         } else {
           ts[h] += hf.x + hf.y;  // the sums see exactly what GEMM 2 sees
@@ -164,6 +199,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     }
     sum[0] += ts[0];
     sum[1] += ts[1];
+    if constexpr (MODE == 7) {
+      sumq[0] += tq[0];
+      sumq[1] += tq[1];
+    }
     // ---- GEMM 2: G += P . Y, K = the 128 columns of the tile, 16 per instruction ----
     wgmma_fence();
 #pragma unroll
@@ -190,15 +229,25 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     float tot = sum[h];
     tot += __shfl_xor_sync(0xffffffffu, tot, 1);
     tot += __shfl_xor_sync(0xffffffffu, tot, 2);
+    float totq = 0.f;
+    if constexpr (MODE == 7) {
+      totq = sumq[h];
+      totq += __shfl_xor_sync(0xffffffffu, totq, 1);
+      totq += __shfl_xor_sync(0xffffffffu, totq, 2);
+    }
+    constexpr int kHead = MODE == 7 ? 2 : 1;  // row sums ahead of the D gradient sums
     const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, c.elem, rtpe, n_local, row_src, N);
     if (row < N) {
-      float* dst = part + ((int64_t)c.split * N + row) * (D + 1);
+      float* dst = part + ((int64_t)c.split * N + row) * (D + kHead);
       if (cq == 0) dst[0] = tot;
+      if constexpr (MODE == 7) {
+        if (cq == 0) dst[1] = totq;
+      }
 #pragma unroll
       for (int j = 0; j < DK / 2; ++j) {
         if (((j >> 1) & 1) != h) continue;
         const int c = 8 * (j >> 2) + cq + (j & 1);
-        if (c < D) dst[1 + c] = g[j] + g[j + DK / 2];
+        if (c < D) dst[kHead + c] = g[j] + g[j + DK / 2];
       }
     }
   }

@@ -71,6 +71,20 @@ constexpr float kTcNormFloor = 1.0f / 16384.f;  // 2^-14: floor of T_i (scaled u
 // The finalize undoes both scales.
 constexpr int kTcNormPLog2 = 6;
 
+// p = 1 softmin (MODE 6 forward, MODE 7 row gradient): f_i = -eps ln2 log2 sum_j 2^(H_j - c d_ij), d from the same
+// exponent GEMM as the energy kernel, on the energy's coordinates (x - center times the power of two of
+// tc_energy_coord_scale), so T_i, its floor and the error bound above hold as they stand.  c = log2e / (eps scale) is
+// applied in the epilogue's FFMA; scaling the coordinates by log2e / eps instead would overflow fp16 at small eps and
+// large coordinates.  A pair below T_i (and the diagonal of xx / yy) takes d = sqrt(clamp): 1e-4 (tensorized) or ~0
+// (unclamped), the values the reference gives coincident points.  In real units the floor is d < 2^-7 / scale, at
+// most 2^-16 of the largest centred coordinate.
+// Row gradient: P = 2^(t_ij - lse2_i + k_i) and Q = P / d (0 below T_i) feed the sums {sum P, sum Q, sum Q Y}.  Q goes
+// to an fp16 GEMM: k_i is the largest power of two with 2^k_i <= 2^kTcL1QLog2 sqrt(T_i), so Q <= 2^15 < 65504 for every
+// admitted pair (P <= 2^k_i, d >= sqrt(T_i)); k_i >= 8 since T_i >= 2^-14.  A pair of softmax weight rho has
+// Q = rho 2^k_i / d > rho 2^14 sqrt(T_i) / d, normal (>= 2^-14) whenever rho >= 2^-28 d / sqrt(T_i).  k_i cancels in
+// the gradient (X_i sum Q - sum Q Y) / sum P, and so does the coordinate scale (a sum of unit vectors).
+constexpr int kTcL1QLog2 = 15;
+
 // power of two that maps the largest centred coordinate `amax` into [2^9, 2^10) (1 for an all-zero cloud); the
 // exponent is bounded so that clamp * scale^2 stays finite
 __host__ __device__ inline float tc_energy_coord_scale(float amax) {
@@ -94,6 +108,19 @@ __device__ __forceinline__ uint4 pack8_f16(const __half* src) {
   return v;
 }
 
+// v as three bf16 terms h + m + l (24 significant bits), packed in bits 0..15, 16..31 and 32..47
+__device__ __forceinline__ uint64_t tc_bf16x3_bits(float v) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  const float q = v - __bfloat162float(h);
+  const __nv_bfloat16 m = __float2bfloat16_rn(q);
+  const __nv_bfloat16 l = __float2bfloat16_rn(q - __bfloat162float(m));
+  return (uint64_t)__bfloat16_as_ushort(h) | ((uint64_t)__bfloat16_as_ushort(m) << 16) |
+         ((uint64_t)__bfloat16_as_ushort(l) << 32);
+}
+__device__ __forceinline__ float tc_bf16_at(uint32_t word, int hi) {
+  return __bfloat162float(__ushort_as_bfloat16((unsigned short)(hi ? word >> 16 : word & 0xffffu)));
+}
+
 // Column images carry, besides the split coordinates, the per-column additive exponent term
 //   c_j = h_scale * (h_a[j] + h_scale_b * h_b[j]) - |Y_j|^2 / 2      (h_a null: just the fold)
 // in the rank-one chunk, and the fp32 weight w_j (kernel conv) behind the bf16 data.  Padding columns get
@@ -104,6 +131,10 @@ __device__ __forceinline__ uint4 pack8_f16(const __half* src) {
 // same way, and the weights of element b are normalised by w_absmax[b].
 // Gather (block-sparse problems, n = number of slots, a multiple of the tile): slot p reads point gather[p], or is
 // padding when gather[p] < 0.
+// l1 (the p = 1 softmin, MODE 6 / 7): the rank-one chunk carries -|X|^2/2 alone, as for the kernel norms.  A column's
+// H_j = h_scale (h_a + h_scale_b h_b) goes to the fp32 weight slot instead (-1e38 for padding).  A row carries, in
+// elements 8..13 of the rank-one chunk (zero in every column, so the GEMM never sees them), the exponent factor
+// c = h_scale / (coordinate scale) and the row term row_extra (the forward's lse2), each as three bf16 terms.
 static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float* __restrict__ w,
                                       const float* __restrict__ h_a, const float* __restrict__ h_b,
                                       float h_scale_b, float h_scale, const float* __restrict__ center,
@@ -112,7 +143,7 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
                                       const float* __restrict__ row_extra = nullptr,
                                       const float* __restrict__ w_absmax = nullptr,
                                       const float* __restrict__ coord_absmax = nullptr, int64_t nb = 1,
-                                      const int* __restrict__ gather = nullptr) {
+                                      const int* __restrict__ gather = nullptr, int l1 = 0) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t npad = ((n + tile - 1) / tile) * tile;
   if (p >= npad * nb) return;
@@ -153,8 +184,8 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
   {
     float r = live ? -0.5f * sq : 0.f;
     // softmin backward: exponent - lse2_i + kTcPLog2 (P = 2^14 softmax weight, common.cuh)
-    if (!is_cols && row_extra != nullptr && live) r -= row_extra[src] - (float)kTcPLog2;
-    if (is_cols && h_a != nullptr) {
+    if (!is_cols && row_extra != nullptr && live && !l1) r -= row_extra[src] - (float)kTcPLog2;
+    if (is_cols && h_a != nullptr && !l1) {
       if (live) {
         float h = h_a[src];
         if (h_b != nullptr) h = fmaf(h_scale_b, h_b[src], h);
@@ -182,13 +213,28 @@ static __global__ void tc_pack_kernel(const float* __restrict__ pts, const float
     v.w = 0u;
     const int chunk = kTcTerms * (dk / 8);
     *reinterpret_cast<uint4*>(img + ((int64_t)chunk * tile + pt) * 16) = v;
-    *reinterpret_cast<uint4*>(img + ((int64_t)(chunk + 1) * tile + pt) * 16) = make_uint4(0u, 0u, 0u, 0u);
+    uint4 v2 = make_uint4(0u, 0u, 0u, 0u);
+    if (l1 && !is_cols) {
+      const uint64_t cf = tc_bf16x3_bits(h_scale / scale), le = tc_bf16x3_bits(live && row_extra ? row_extra[src] : 0.f);
+      v2.x = cf & 0xffffffffu;                   // c: elements 8, 9
+      v2.y = (cf >> 32) | ((le & 0xffffu) << 16);  // c: element 10, lse2: element 11
+      v2.z = (uint32_t)(le >> 16);               // lse2: elements 12, 13
+    }
+    *reinterpret_cast<uint4*>(img + ((int64_t)(chunk + 1) * tile + pt) * 16) = v2;
   }
   if (is_cols) {
     // (row-gradient kernels feed P = w e to an fp16 GEMM: weights are normalised to |w| <= kTcPScale = 2^14, which
     // keeps P out of fp16's subnormal range; undone in the finalize)
     float wv = (live && w) ? w[src] : 0.f;
     if (w_absmax != nullptr && w_absmax[b] > 0.f) wv = (wv / w_absmax[b]) * kTcPScale;
+    if (l1) {
+      wv = -1.0e38f;
+      if (live) {
+        float h = h_a[src];
+        if (h_b != nullptr) h = fmaf(h_scale_b, h_b[src], h);
+        wv = h_scale * h;
+      }
+    }
     reinterpret_cast<float*>(img + (int64_t)tile * kp * 2)[pt] = wv;
   }
 }
@@ -259,6 +305,20 @@ __device__ __forceinline__ void tc_norm_row_bounds(float (&tb)[2], float& clampq
   const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   tb[0] = tc_norm_row_bound(sa, kp, lr, clampq);
   tb[1] = tc_norm_row_bound(sa, kp, lr + 8, clampq);
+}
+// MODE 6 / 7: the exponent factor c and the row term lse2 of a row of the row image (tc_pack_kernel's l1 layout), and
+// the same for the thread's two rows
+__device__ __forceinline__ float2 tc_l1_row_terms(const unsigned char* sa, int kp, int local_row) {
+  const int chunk = kTcTerms * (tc_dk_of_kp(kp) / 8) + 1;
+  const uint4 v = *reinterpret_cast<const uint4*>(sa + ((int64_t)chunk * kTcM + local_row) * 16);
+  return make_float2(tc_bf16_at(v.x, 0) + tc_bf16_at(v.x, 1) + tc_bf16_at(v.y, 0),
+                     tc_bf16_at(v.y, 1) + tc_bf16_at(v.z, 0) + tc_bf16_at(v.z, 1));
+}
+__device__ __forceinline__ void tc_l1_rows(float2 (&rt)[2], const unsigned char* sa, int kp, int wg, int warp,
+                                           int lane) {
+  const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  rt[0] = tc_l1_row_terms(sa, kp, lr);
+  rt[1] = tc_l1_row_terms(sa, kp, lr + 8);
 }
 // The weighted value of one pair from its exponent s: 2^s (MODE 0), or k(d) with d^2 = clamp for a pair below the row
 // bound t (and the diagonal), else -2 s (MODE 4 / 5)
@@ -395,6 +455,8 @@ __device__ __forceinline__ int64_t tc_out_row(int64_t row, int elem, int rtpe, i
 //         sum-guarded exactly like softmin.cuh; same partial format as softmin_partial_kernel)
 // MODE 4: laplacian kernel conv  part[...] = sum_j w_j 2^-d_ij       MODE 5: energy  part[...] = sum_j w_j d_ij
 //         (d_ij from the exponent as described above; `clampq` and `coord_absmax` are read by these modes only)
+// MODE 6: p = 1 softmin, MODE 1's (m, s) partials of sum_j 2^(H_j - c d_ij) (d_ij as for MODE 5, H_j from the weight
+//         slot, c from the row image; see kTcL1QLog2)
 // (row gradients — modes 2 and 3 — are a two-GEMM kernel of their own: tcbwd.cuh)
 //
 // A CTA owns one 128-row tile: its row image is loaded once by TMA and stays in shared memory, the column tiles
@@ -419,7 +481,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
                      int D, int self_mode, float clampq, const float* __restrict__ coord_absmax, int rtpe,
                      int64_t n_local, const int4* __restrict__ bseg = nullptr,
                      const int2* __restrict__ bpieces = nullptr, const int* __restrict__ row_src = nullptr) {
-  static_assert(MODE == 0 || MODE == 1 || MODE == 4 || MODE == 5, "row gradients live in tcbwd.cuh");
+  static_assert(MODE == 0 || MODE == 1 || MODE == 4 || MODE == 5 || MODE == 6, "row gradients live in tcbwd.cuh");
   static_assert(!BLOCKS || (MODE == 1 && !BATCH), "the block-sparse layout serves the softmin of one problem");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -437,8 +499,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   float acc[2] = {0.f, 0.f};                 // MODE 0, 4, 5: weighted sums
   float m[2] = {kNegBig, kNegBig}, srun[2] = {0.f, 0.f};  // MODE 1: running (m, s)
   mbar_wait(c.bar_a, 0);
-  float tb[2] = {0.f, 0.f};  // MODE 4 / 5: coincidence bound of each row
+  float tb[2] = {0.f, 0.f};  // MODE 4 / 5 / 6: coincidence bound of each row
   if constexpr (MODE >= 4) tc_norm_row_bounds(tb, clampq, coord_absmax, c.sa, kp, wg, warp, lane);
+  float2 rt[2] = {};  // MODE 6: (c, -) of each row
+  if constexpr (MODE == 6) tc_l1_rows(rt, c.sa, kp, wg, warp, lane);
   for (int k = 0; k < c.nt; ++k) {
     const int st = k % NSTAGE;
     mbar_wait(&c.full_b[st], (k / NSTAGE) & 1);
@@ -446,7 +510,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     tc_exponent_gemm(s, a_addr, smem_u32(c.sb + st * c.b_bytes), seg);
     wgmma_wait<0>();
     reg_fence(s);
-    if constexpr (MODE != 1) {
+    if constexpr (MODE == 6) {
+      // the p = 1 exponent t = H_j - c d_ij in place of s, then the softmin's log-sum-exp below
+      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
+      const float* hs = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
+#pragma unroll
+      for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+        const float2 hj = *reinterpret_cast<const float2*>(hs + 8 * n8 + cq);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          s[4 * n8 + 2 * h] = fmaf(-rt[h].x, tc_pair_value<5>(s[4 * n8 + 2 * h], tb[h], clampq), hj.x);
+          s[4 * n8 + 2 * h + 1] = fmaf(-rt[h].x, tc_pair_value<5>(s[4 * n8 + 2 * h + 1], tb[h], clampq), hj.y);
+        }
+      }
+    }
+    if constexpr (MODE != 1 && MODE != 6) {
       if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
       const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
       float ts[2] = {0.f, 0.f};
@@ -497,7 +575,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   for (int h = 0; h < 2; ++h) {
     const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, c.elem, rtpe, n_local, row_src, N);
     if (row < N) {
-      if constexpr (MODE != 1) {
+      if constexpr (MODE != 1 && MODE != 6) {
         part[((int64_t)c.split * kTcParts + q) * N + row] = acc[h];
       } else {
         reinterpret_cast<float2*>(part)[((int64_t)c.split * kTcParts + q) * N + row] = make_float2(m[h], srun[h]);

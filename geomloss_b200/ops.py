@@ -73,7 +73,8 @@ def _f32c(t, name):
     return t.contiguous()
 
 
-MAX_D_TC = 64  # softmin (p = 2) and the three kernel convolutions, forward + row gradients: tensor-core path, 8 < D <= 64
+MAX_D_TC = 64  # softmin (p = 2, and p = 1 through softmin_l1) and the three kernel convolutions, forward + row
+# gradients: tensor-core path, 8 < D <= 64
 
 
 def _check_clouds(x, y, max_d=None):
@@ -86,7 +87,8 @@ def _check_clouds(x, y, max_d=None):
         raise NotImplementedError(f"D = {x.shape[1]} > {max_d}: not instantiated in this build (CUDA-core kernels "
                                   f"serve every operator for D <= {MAX_D}; the tensor-core kernels serve the p = 2 "
                                   f"softmin and the gaussian, laplacian and energy kernel convolutions, forward and row "
-                                  f"gradients, up to D = {MAX_D_TC}; the p = 1 softmin stops at D = {MAX_D})")
+                                  f"gradients, up to D = {MAX_D_TC}; the p = 1 softmin above D = {MAX_D} is "
+                                  f"ops.softmin_l1 / softmin_l1_raw)")
     if x.device != y.device:
         raise ValueError("x and y must be on the same device")
 
@@ -555,3 +557,91 @@ def kernel_conv_batched(kind, x, y, w, blur, *, center=None):
     """out (B,N) = K(x[b], y[b]) @ w[b] for every b, differentiable w.r.t. x, y and w."""
     fused = (FUSED_CONV_GRAD and torch.is_grad_enabled() and x.requires_grad and (kind_id(kind) & 0xFF) == 0)
     return _KernelConvBatched.apply(x, y, w, kind, blur, center, bool(fused))
+
+
+# ------------------------------------------------------------------------------------------------
+# the p = 1 softmin in the tensor-core dimensions (8 < D <= 64): f_i = -eps log sum_j exp(h_j - |x_i - y_j| / eps), one
+# problem (N,D) / (M,D) or a batch (B,N,D) / (B,M,D) in one launch group per call (b200ot_softmin_l1_*).
+# ------------------------------------------------------------------------------------------------
+def _l1_args(x, y, p):
+    if (p & 0xFF) != 1 or (p & ~(0xFF | P_UNCLAMPED)) != 0:
+        raise ValueError(f"softmin_l1 computes the p = 1 softmin (p = 1 or 1 | P_UNCLAMPED), got p = {p}")
+    if x.dim() == 2 and y.dim() == 2:
+        return False, _check_batch(x.unsqueeze(0), y.unsqueeze(0))
+    return True, _check_batch(x, y)
+
+
+def softmin_l1_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, out_old=None, alpha_old=0.0,
+                   beta=1.0, out=None, want_lse2=False):
+    """``softmin_batched_raw`` for the cost |x - y|: out <- alpha_old*out_old + beta*softmin(eps, (x, y), h), (N,) for
+    (N,D) clouds, (B,N) for (B,N,D) ones.  No autograd.  Returns ``(out, lse2 | None)``."""
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
+    batched, (B, N, M, D) = _l1_args(x, y, p)
+    _per_point(h_a, B * M, "h_a")
+    _per_point(h_b, B * M, "h_b")
+    _per_point(out_old, B * N, "out_old")
+    shape = (B, N) if batched else (N,)
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev), nvtx_range(f"b200ot.softmin_l1 B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=dev)
+        lse2 = torch.empty(shape, dtype=torch.float32, device=dev) if want_lse2 else None
+        scratch = _scratch(L.b200ot_softmin_l1_scratch_bytes(B, N, M, D), dev, "softmin_l1")
+        rc = L.b200ot_softmin_l1_fwd(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
+                                     _ptr(out_old), float(alpha_old), float(beta), _ptr(out), _ptr(lse2), B, N, M, D,
+                                     int(p), float(eps), _ptr(scratch), scratch.numel(), _stream(dev))
+    _lib.check(rc, "b200ot_softmin_l1_fwd")
+    count_launches(5)  # coordinate maximum, two packs, reduction, finalize
+    return out, lse2
+
+
+def softmin_l1_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=1, center=None):
+    """grad_x, shaped like x, of <grad_out, softmin_l1(eps, x, y, h)> with y, h constant (b200ot_softmin_l1_bwd_x)."""
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
+    _, (B, N, M, D) = _l1_args(x, y, p)
+    _per_point(grad_out, B * N, "grad_out")
+    _per_point(lse2, B * N, "lse2")
+    dev = x.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        scratch = _scratch(L.b200ot_softmin_l1_scratch_bytes(B, N, M, D), dev, "softmin_l1")
+        rc = L.b200ot_softmin_l1_bwd_x(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
+                                       _ptr(lse2), _ptr(grad_out), _ptr(gx), B, N, M, D, int(p), float(eps),
+                                       _ptr(scratch), scratch.numel(), _stream(dev))
+    _lib.check(rc, "b200ot_softmin_l1_bwd_x")
+    count_launches(5)  # coordinate maximum, two packs, reduction, finalize
+    return gx
+
+
+class _SoftminL1(torch.autograd.Function):
+    """softmin_l1 with _Softmin's autograd contract: the gradient flows to the row cloud x only."""
+
+    @staticmethod
+    def forward(ctx, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out):
+        need_grad = ctx.needs_input_grad[0]
+        out, lse2 = softmin_l1_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out,
+                                   want_lse2=need_grad)
+        if need_grad:
+            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
+                                  lse2)
+            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), h_b is not None, center is not None)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
+        h_scale_b, eps, p, scale_out, has_hb, has_center = ctx.meta
+        go = (grad_out * scale_out).contiguous()
+        gx = softmin_l1_grad_rows(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, lse2, go, p=p,
+                                  center=center if has_center else None)
+        return gx, None, None, None, None, None, None, None, None
+
+
+def softmin_l1(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, scale_out=1.0):
+    """Differentiable (w.r.t. x) ``scale_out * softmin_l1_raw(...)``, for (N,D) or (B,N,D) clouds."""
+    return _SoftminL1.apply(x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps, p,
+                            center, scale_out)

@@ -19,10 +19,11 @@ explicit labels for both clouds (the 6-tensor call form) the two-scale Sinkhorn 
 reference, whose ``clusterize`` takes labels in any dimension: the CUDA-core ranges kernels up to D = 8, the
 tensor-core block-sparse softmins above (p = 2; p = 1 above D = 8 raises NotImplementedError).  Column-sharded
 multi-GPU engines keep the single-scale route for such calls.
+The Sinkhorn loss with p = 1 above D = 8 runs on the tensor-core p = 1 softmin (ops.softmin_l1), batched or not, in
+both cost conventions; column-sharded multi-GPU engines have no such operator and raise NotImplementedError there.
 Batched inputs (B, N, D) run as ONE launch group per reduction for the whole batch: a block-diagonal ranges problem
-for D <= 8 (ranges.py), the batched tensor-core operators for 8 < D <= 64 (ops.softmin_batched / kernel_conv_batched;
-Sinkhorn with p = 2 only: p = 1 above D = 8 raises NotImplementedError, batched or not).  Column-sharded multi-GPU
-engines solve the batch element by element.
+for D <= 8 (ranges.py), the batched tensor-core operators for 8 < D <= 64 (ops.softmin_batched, ops.softmin_l1,
+kernel_conv_batched).  Column-sharded multi-GPU engines solve the batch element by element.
 Inputs must be float32 CUDA tensors: there is no CPU path.
 """
 from __future__ import annotations
@@ -180,9 +181,7 @@ class SamplesLoss(Module):
             from .sinkhorn import max_diameter
 
             kw["diameter"] = max_diameter(x.reshape(-1, D), y.reshape(-1, D))
-        # (a p = 1 Sinkhorn above D = 8 has no batched operator: the loop below raises NotImplementedError)
-        one_group = D <= MAX_D or (D <= MAX_D_TC and (self.loss != "sinkhorn" or self.p == 2)
-                                   and N * M <= BATCHED_TC_MAX_PAIRS)
+        one_group = D <= MAX_D or (D <= MAX_D_TC and N * M <= BATCHED_TC_MAX_PAIRS)
         if B > 1 and one_group and not self._engine and self.loss != "hausdorff":
             # the whole batch in one launch group per reduction (D <= 8: block-diagonal ranges problem; above: the
             # batched tensor-core operators)

@@ -224,7 +224,8 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
  * sinkhorn_samples.py:229-290; kernel_loss on (B, N, D) inputs).  x (B,N,D), y (B,M,D); h_a, h_b, w (B,M); out,
  * lse2, grad_out (B,N); grad_x (B,N,D); center (D) shared by the whole batch.  Row i of element b is reduced over
  * the columns of element b only.  Arguments and results are those of the one-problem entries above, element by
- * element; p = 2 only (p = 1 has no tensor-core softmin); D <= 8 batches go through the ranges entry points.
+ * element; p = 2 only (the p = 1 softmin has entries of its own, b200ot_softmin_l1_*); D <= 8 batches go through the
+ * ranges entry points.
  * EINVAL for B < 1, D <= 8 or D > 64; scratch: b200ot_batched_scratch_bytes(B, N, M, D) bytes, 16-byte aligned.
  * The batched row gradients run the default variant of the row-gradient kernel ($B200OT_TC_BWD is not read).
  * ------------------------------------------------------------------------------------------- */
@@ -251,6 +252,28 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float*
                                                     const float* center, float* out, float* grad_unit, int64_t B,
                                                     int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
                                                     void* scratch, int64_t scratch_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * The p = 1 softmin in the tensor-core dimensions (8 < D <= 64): f_i = -eps log sum_j exp(h_j - |x_i - y_j| / eps),
+ * the reference's cost |x - y| (`distances`, utils.py:56-61) in its tensorized (p = 1) or pykeops
+ * (p = 1 | B200OT_P_UNCLAMPED) convention.  Batched layout, arguments and results as the batched entries above
+ * (B = 1: one problem); lse2_out / lse2 in the same log2 units, so b200ot_softmin_finalize's epilogue applies.
+ * EINVAL (before any launch) for null pointers, B < 1, N or M <= 0, D <= 8 or D > 64, p other than 1 or
+ * 1 | B200OT_P_UNCLAMPED, eps <= 0; EALIGN for a misaligned scratch; ESCRATCH below
+ * b200ot_softmin_l1_scratch_bytes(B, N, M, D) (0 for a shape these entries refuse).
+ * ------------------------------------------------------------------------------------------- */
+B200OT_API int64_t b200ot_softmin_l1_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D);
+B200OT_API int b200ot_softmin_l1_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
+                                     float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                     float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
+                                     int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                     void* stream);
+/* grad_x (B,N,D) of <grad_out, f> with y and h constant: go_i sum_j w_ij (x_i - y_j) / |x_i - y_j| (zero for
+ * coincident pairs, which keep their weight) */
+B200OT_API int b200ot_softmin_l1_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
+                                       float h_scale_b, const float* center, const float* lse2, const float* grad_out,
+                                       float* grad_x, int64_t B, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
+                                       void* scratch, int64_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Block-sparse softmins in the tensor-core dimensions (8 < D <= 64, p = 2 or 2 | B200OT_P_UNCLAMPED): the fine phase

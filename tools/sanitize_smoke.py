@@ -30,7 +30,7 @@ def check(name, got, ref, tol=2e-5):
     assert err < tol, name
 
 
-which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "blocks", "grid", "loss", "small"}
+which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "blocks", "grid", "loss", "small"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -154,6 +154,21 @@ if "batched" in which:
         val, gu = ops.kernel_conv_batched_value_and_grad_rows(0, xd, yd, wd, 2.0, center=center)
         check(f"batched_conv_value_d{d}", val, ((-d2 / 8.0).exp() @ w.double()[:, :, None])[..., 0], 1e-4)
         assert torch.isfinite(gu).all()
+if "l1" in which:
+    # the p = 1 softmin (tc_reduce_kernel<6, BATCH>, tc_bwd_kernel<7, 2, MERGE, dk, BATCH> at every dk)
+    B, n = 2, 300
+    for d in (16, 32, 48, 64):
+        x, y, h = torch.rand(B, n, d, generator=g), torch.rand(B, n, d, generator=g), torch.randn(B, n, generator=g)
+        xd, yd, hd, ones = x.to(DEV), y.to(DEV), h.to(DEV), torch.ones(B, n, device=DEV)
+        center = ops.default_center(xd.view(-1, d), yd.view(-1, d))
+        dist = ((x[:, :, None, :].double() - y[:, None, :, :].double()) ** 2).sum(-1).clamp_min(1e-8).sqrt()
+        out, lse2 = ops.softmin_l1_raw(0.5, xd, yd, hd, p=1, center=center, want_lse2=True)
+        check(f"l1_softmin_d{d}", out, (-0.5 * torch.logsumexp(h.double()[:, None, :] - dist / 0.5, dim=2)).float(),
+              1e-4)
+        gx = ops.softmin_l1_grad_rows(0.5, xd, yd, hd, None, 0.0, lse2, ones, p=1, center=center)
+        prob = torch.softmax(h.double()[:, None, :] - dist / 0.5, dim=2)
+        unit = (x.double()[:, :, None, :] - y.double()[:, None, :, :]) / dist[..., None]
+        check(f"l1_softmin_grad_d{d}", gx, (prob[..., None] * unit).sum(2), 1e-4)
 if "blocks" in which:
     # the block-sparse tensor-core softmins (tc_reduce_kernel<1, false, BLOCKS>, tc_bwd_kernel<3, 2, true, dk, false,
     # BLOCKS>): clusters of 1, 127, 128, 129 and 300 points, a row cluster that keeps nothing, a self problem
