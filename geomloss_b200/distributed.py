@@ -23,6 +23,8 @@ default is the CUDA implementation and it refuses non-CUDA tensors.
 """
 from __future__ import annotations
 
+from functools import partial
+
 import torch
 import torch.distributed as dist
 
@@ -50,20 +52,14 @@ class CudaStages:
             # log-sum-exp, which IS a merged partial (m = lse2, s = 1)
             lse2 = ops.softmin_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, want_lse2=True)[1]
             return torch.stack([lse2, torch.ones_like(lse2)], dim=1).contiguous()
-        with torch.cuda.device(dev):
-            merged = torch.empty(N, 2, dtype=torch.float32, device=dev)
-            nsplit = L.b200ot_softmin_num_splits(N, M, D)
-            cols = ops._scratch(L.b200ot_packed_cols_floats(M, D, 1) * 4, dev, "shard_cols")
-            part = ops._scratch(nsplit * N * 8, dev, "shard_part")
-            st = ops._stream(dev)
-            _lib.check(L.b200ot_softmin_pack(ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b), float(h_scale_b),
-                                             ops._ptr(center), M, D, int(p), float(eps), ops._ptr(cols), st),
-                       "b200ot_softmin_pack")
-            _lib.check(L.b200ot_softmin_partial(ops._ptr(x), ops._ptr(center), ops._ptr(cols), ops._ptr(part),
-                                                nsplit, N, M, D, int(p), float(eps), st), "b200ot_softmin_partial")
-            _lib.check(L.b200ot_softmin_merge(ops._ptr(part), nsplit, ops._ptr(merged), N, st),
-                       "b200ot_softmin_merge")
-        ops.count_launches(3)
+        merged = torch.empty(N, 2, dtype=torch.float32, device=dev)
+        nsplit = ops._query(dev, "b200ot_softmin_num_splits", N, M, D)
+        cols = ops._scratch(L.b200ot_packed_cols_floats(M, D, 1) * 4, dev, "shard_cols")
+        part = ops._scratch(nsplit * N * 8, dev, "shard_part")
+        ops._call(dev, "b200ot_softmin_pack", y, h_a, h_b, float(h_scale_b), center, M, D, int(p), float(eps), cols,
+                  launches=1)
+        ops._call(dev, "b200ot_softmin_partial", x, center, cols, part, nsplit, N, M, D, int(p), float(eps), launches=1)
+        ops._call(dev, "b200ot_softmin_merge", part, nsplit, merged, N, launches=1)
         return merged
 
     def empty_shard(self, N, dev):
@@ -73,17 +69,7 @@ class CudaStages:
         return out
 
     def softmin_finalize(self, parts, eps, out_old, alpha_old, beta, want_lse2):
-        W, N, _ = parts.shape
-        dev = parts.device
-        L = _lib.lib()
-        with torch.cuda.device(dev):
-            out = torch.empty(N, dtype=torch.float32, device=dev)
-            lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
-            _lib.check(L.b200ot_softmin_finalize(ops._ptr(parts), W, ops._ptr(ops._f32c(out_old, "out_old")),
-                                                 float(alpha_old), float(beta), ops._ptr(out), ops._ptr(lse2), N,
-                                                 float(eps), ops._stream(dev)), "b200ot_softmin_finalize")
-        ops.count_launches(1)
-        return out, lse2
+        return ranges.softmin_finalize(parts, parts.shape[0], eps, out_old, alpha_old, beta, want_lse2)
 
     def softmin_bwd_shard(self, eps, x, y, h_a, h_b, h_scale_b, p, center, lse2):
         """(N, D+1) partial sums of the backward pass over the column shard (any supported D)."""
@@ -92,29 +78,14 @@ class CudaStages:
         N, D = x.shape
         M = y.shape[0]
         dev = x.device
-        L = _lib.lib()
-        with torch.cuda.device(dev):
-            sums = torch.empty(N, D + 1, dtype=torch.float32, device=dev)
-            scratch = ops._scratch(L.b200ot_softmin_scratch_bytes(N, M, D), dev, "softmin")
-            _lib.check(L.b200ot_softmin_bwd_sums(ops._ptr(x), ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b),
-                                                 float(h_scale_b), ops._ptr(center), ops._ptr(lse2), ops._ptr(sums), N,
-                                                 M, D, int(p), float(eps), ops._ptr(scratch), scratch.numel(),
-                                                 ops._stream(dev)), "b200ot_softmin_bwd_sums")
-        ops.count_launches(3)
+        sums = torch.empty(N, D + 1, dtype=torch.float32, device=dev)
+        scratch = ops._scratch(ops._query(dev, "b200ot_softmin_scratch_bytes", N, M, D), dev, "softmin")
+        ops._call(dev, "b200ot_softmin_bwd_sums", x, y, h_a, h_b, float(h_scale_b), center, lse2, sums, N, M, D, int(p),
+                  float(eps), scratch, scratch.numel(), launches=3)
         return sums
 
     def softmin_bwd_finalize(self, sums, eps, x, center, grad_out, p):
-        x, center, grad_out = ops._f32c(x, "x"), ops._f32c(center, "center"), ops._f32c(grad_out, "grad_out")
-        N, D = x.shape
-        dev = x.device
-        L = _lib.lib()
-        with torch.cuda.device(dev):
-            gx = torch.empty_like(x)
-            _lib.check(L.b200ot_softmin_bwd_finalize(ops._ptr(sums), 1, ops._ptr(x), ops._ptr(center),
-                                                     ops._ptr(grad_out), ops._ptr(gx), N, D, int(p), float(eps),
-                                                     ops._stream(dev)), "b200ot_softmin_bwd_finalize")
-        ops.count_launches(1)
-        return gx
+        return ranges.softmin_bwd_finalize(sums, eps, x, center, grad_out, p)
 
     # -- ranges mode (multiscale fine phase): ALL columns are packed, the pieces select this rank's clusters --
     def softmin_sparse_shard(self, eps, x, y, h_a, h_b, h_scale_b, p, center, prob):
@@ -197,8 +168,26 @@ class ColumnShardedEngine:
 
     # -- forward + backward (the final, gradient-carrying Sinkhorn step) --------------------------
     def softmin(self, eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0, local=False):
-        return _ShardedSoftmin.apply(self, x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(),
-                                     h_scale_b, eps, p, center, scale_out, local, None)
+        return ops._softmin_apply(partial(self.softmin_raw, local=local), partial(self.softmin_grad_rows, local=local),
+                                  eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)
+
+    def softmin_grad_rows(self, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None, local=False,
+                          prob=None):
+        """grad_x of <grad_out, softmin_raw(...)> (``prob`` None) or of <grad_out, sparse_raw(..., prob)>, with y, h
+        constant: the shards' partial sums, added over the ranks unless ``local``, then finalized."""
+        M = y.shape[0]
+        lo, hi = (0, M) if local else shard_bounds(M, self.rank, self.world)
+        if prob is not None:
+            sums = self.stages.softmin_bwd_sparse_shard(eps, x, y, h_a, h_b, h_scale_b, p, center, lse2, prob)
+        elif hi > lo:
+            sums = self.stages.softmin_bwd_shard(eps, x, y[lo:hi], h_a[lo:hi], None if h_b is None else h_b[lo:hi],
+                                                 h_scale_b, p, center, lse2)
+        else:
+            sums = torch.zeros(x.shape[0], x.shape[1] + 1, dtype=x.dtype, device=x.device)
+        if not local:
+            dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=self.group)
+            self.collectives += 1
+        return self.stages.softmin_bwd_finalize(sums, eps, x, center, grad_out, p)
 
     # -- the operator set of multiscale.sinkhorn_multiscale (same names as multiscale.LocalEngine) ----
     def build(self, keep, row_counts, layout, variant=None):
@@ -230,8 +219,8 @@ class ColumnShardedEngine:
         return self.stages.softmin_finalize(parts, eps, out_old, alpha_old, beta, want_lse2)
 
     def sparse(self, eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None, scale_out=1.0):
-        return _ShardedSoftmin.apply(self, x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(),
-                                     h_scale_b, eps, p, center, scale_out, False, prob)
+        return ops._softmin_apply(partial(self.sparse_raw, prob=prob), partial(self.softmin_grad_rows, prob=prob), eps,
+                                  x, y, h_a, h_b, h_scale_b, p, center, scale_out)
 
     # -- kernel MMD matvec: out = K(x, y) @ w with the columns sharded, one all_reduce(SUM) --------
     def kernel_conv(self, kind, x, y, w, blur, *, center=None):
@@ -243,46 +232,6 @@ class ColumnShardedEngine:
         loss_module._engine = dict(softmin_raw=self.softmin_raw, softmin_grad=self.softmin, conv=self.kernel_conv)
         loss_module._multiscale_engine = self
         return loss_module
-
-
-class _ShardedSoftmin(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, eng, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out, local, prob):
-        need = ctx.needs_input_grad[1]
-        if prob is not None:
-            out, lse2 = eng.sparse_raw(eps, x, y, h_a, h_b, h_scale_b, prob, p=p, center=center, beta=scale_out,
-                                       want_lse2=need)
-        else:
-            out, lse2 = eng.softmin_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out,
-                                        want_lse2=need, local=local)
-        if need:
-            ctx.eng, ctx.local, ctx.prob = eng, local, prob
-            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
-                                  lse2)
-            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), h_b is not None, center is not None)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        eng = ctx.eng
-        x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
-        h_scale_b, eps, p, scale_out, has_hb, has_center = ctx.meta
-        h_b = h_b if has_hb else None
-        center = center if has_center else None
-        M = y.shape[0]
-        lo, hi = (0, M) if ctx.local else shard_bounds(M, eng.rank, eng.world)
-        if ctx.prob is not None:
-            sums = eng.stages.softmin_bwd_sparse_shard(eps, x, y, h_a, h_b, h_scale_b, p, center, lse2, ctx.prob)
-        elif hi > lo:
-            sums = eng.stages.softmin_bwd_shard(eps, x, y[lo:hi], h_a[lo:hi], None if h_b is None else h_b[lo:hi],
-                                                h_scale_b, p, center, lse2)
-        else:
-            sums = torch.zeros(x.shape[0], x.shape[1] + 1, dtype=x.dtype, device=x.device)
-        if not ctx.local:
-            dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=eng.group)
-            eng.collectives += 1
-        gx = eng.stages.softmin_bwd_finalize(sums, eps, x, center, (grad_out * scale_out).contiguous(), p)
-        return None, gx, None, None, None, None, None, None, None, None, None, None
 
 
 class _ShardedConv(torch.autograd.Function):

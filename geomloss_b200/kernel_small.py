@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib, ops
+from . import ops
 from .sinkhorn_small import SMALL_MAX  # noqa: F401  (one threshold for both small paths)
 
 
@@ -16,13 +16,8 @@ def _forward(kid, a, x, b, y, blur, want_ay):
     dev = x.device
     a_x, b_y, b_x = torch.empty(B, N, device=dev), torch.empty(B, M, device=dev), torch.empty(B, N, device=dev)
     a_y = torch.empty(B, M, device=dev) if want_ay else None
-    L = _lib.lib()
-    P = ops._ptr
-    with torch.cuda.device(dev):
-        rc = L.b200ot_kernel_mmd_small(P(x), P(y), P(a), P(b), P(a_x), P(b_y), P(b_x), P(a_y), B, N, M, D, int(kid),
-                                       float(blur), ops._stream(dev))
-    _lib.check(rc, "b200ot_kernel_mmd_small")
-    ops.count_launches(1)
+    ops._call(dev, "b200ot_kernel_mmd_small", x, y, a, b, a_x, b_y, b_x, a_y, B, N, M, D, int(kid), float(blur),
+              launches=1)
     return a_x, b_y, b_x, a_y
 
 
@@ -33,12 +28,7 @@ class _MMDValue(torch.autograd.Function):
         a_x, b_y, b_x, a_y = _forward(kid, a, x, b, y, blur, want_ay=need_b)
         B, N, _ = x.shape
         val = torch.empty(B, dtype=torch.float32, device=x.device)
-        with torch.cuda.device(x.device):
-            rc = _lib.lib().b200ot_kernel_mmd_value_small(ops._ptr(a), ops._ptr(b), ops._ptr(a_x), ops._ptr(b_y),
-                                                          ops._ptr(b_x), B, N, y.shape[1], ops._ptr(val),
-                                                          ops._stream(x.device))
-        _lib.check(rc, "b200ot_kernel_mmd_value_small")
-        ops.count_launches(1)
+        ops._call(x.device, "b200ot_kernel_mmd_value_small", a, b, a_x, b_y, b_x, B, N, y.shape[1], val, launches=1)
         ctx.save_for_backward(a, x, b, y, a_x, b_y, b_x, a_y if need_b else a_x)
         ctx.meta = (int(kid), float(blur), need_b)
         return val
@@ -57,13 +47,8 @@ class _MMDValue(torch.autograd.Function):
             B, N, D = x.shape
             M = y.shape[1]
             gx, gy = torch.empty_like(x), torch.empty_like(y)
-            L = _lib.lib()
-            P = ops._ptr
-            with torch.cuda.device(x.device):
-                rc = L.b200ot_kernel_mmd_bwd_small(P(x), P(y), P(a), P(b), P(go), P(gx), P(gy), B, N, M, D, kid, blur,
-                                                   ops._stream(x.device))
-            _lib.check(rc, "b200ot_kernel_mmd_bwd_small")
-            ops.count_launches(1)
+            ops._call(x.device, "b200ot_kernel_mmd_bwd_small", x, y, a, b, go, gx, gy, B, N, M, D, kid, blur,
+                      launches=1)
         return ga, gx, gb, gy, None, None
 
 

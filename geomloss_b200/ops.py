@@ -8,6 +8,7 @@ PyTorch is used for memory, streams and autograd bookkeeping only.
 from __future__ import annotations
 
 import ctypes
+from typing import Callable, NamedTuple, Optional
 
 import torch
 
@@ -61,6 +62,25 @@ def _ptr(t):
 
 def _stream(dev):
     return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _call(dev, name, *args, launches):
+    """Enqueue the C entry ``name`` on the current stream of ``dev``: tensors travel as device pointers, every other
+    argument (None, numbers, ctypes objects) as it is, the stream last.  A failure raises ``B200OTError``; the entry's
+    ``launches`` kernels are counted."""
+    fn = getattr(_lib.lib(), name)
+    ptrs = [_ptr(a) if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(dev):
+        rc = fn(*ptrs, _stream(dev))
+    _lib.check(rc, name)
+    count_launches(launches)
+
+
+def _query(dev, name, *args):
+    """The answer of the size query ``name`` for ``dev``: split counts, and so scratch sizes, follow the SM count of
+    the current device, so the query runs with ``dev`` current."""
+    with torch.cuda.device(dev):
+        return getattr(_lib.lib(), name)(*args)
 
 
 def _f32c(t, name):
@@ -121,18 +141,14 @@ def cloud_extent(x, y=None):
     x = x.detach().contiguous()
     y = None if y is None or y.shape[0] == 0 else y.detach().contiguous()
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        key = (dev, torch.cuda.current_stream(dev).cuda_stream)
-        scratch = _extent_scratch.get(key)
-        if scratch is None:  # zero once: the kernel's ticket counter returns to zero after every launch
-            scratch = _extent_scratch[key] = torch.zeros(L.b200ot_cloud_extent_scratch_bytes(), dtype=torch.uint8,
-                                                         device=dev)
-        out = torch.empty(2, x.shape[1], dtype=torch.float32, device=dev)
-        rc = L.b200ot_cloud_extent(_ptr(x), x.shape[0], _ptr(y), 0 if y is None else y.shape[0], x.shape[1], _ptr(out),
-                                   _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_cloud_extent")
-    count_launches(1)
+    key = (dev, torch.cuda.current_stream(dev).cuda_stream)
+    scratch = _extent_scratch.get(key)
+    if scratch is None:  # zero once: the kernel's ticket counter returns to zero after every launch
+        scratch = _extent_scratch[key] = torch.zeros(_lib.lib().b200ot_cloud_extent_scratch_bytes(), dtype=torch.uint8,
+                                                     device=dev)
+    out = torch.empty(2, x.shape[1], dtype=torch.float32, device=dev)
+    _call(dev, "b200ot_cloud_extent", x, x.shape[0], y, 0 if y is None else y.shape[0], x.shape[1], out, scratch,
+          scratch.numel(), launches=1)
     return out
 
 
@@ -165,18 +181,13 @@ def softmin_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, ou
     if h_a.numel() != M or (h_b is not None and h_b.numel() != M):
         raise ValueError("h must have one entry per column")
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.softmin N={N} M={M} D={D} eps={float(eps):.3g}"):
+    with nvtx_range(f"b200ot.softmin N={N} M={M} D={D} eps={float(eps):.3g}"):
         if out is None:
             out = torch.empty(N, dtype=torch.float32, device=dev)
         lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
-        nbytes = L.b200ot_softmin_scratch_bytes(N, M, D)
-        scratch = _scratch(nbytes, dev, "softmin")
-        rc = L.b200ot_softmin_fwd(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
-                                  _ptr(out_old), float(alpha_old), float(beta), _ptr(out), _ptr(lse2), N, M, D,
-                                  int(p), float(eps), _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_softmin_fwd")
-    count_launches(3)
+        scratch = _scratch(_query(dev, "b200ot_softmin_scratch_bytes", N, M, D), dev, "softmin")
+        _call(dev, "b200ot_softmin_fwd", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
+              float(beta), out, lse2, N, M, D, int(p), float(eps), scratch, scratch.numel(), launches=3)
     return out, lse2
 
 
@@ -188,49 +199,50 @@ def softmin_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, ce
     N, D = x.shape
     M = y.shape[0]
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        nbytes = L.b200ot_softmin_scratch_bytes(N, M, D)
-        scratch = _scratch(nbytes, dev, "softmin")
-        rc = L.b200ot_softmin_bwd_x(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
-                                    _ptr(lse2), _ptr(grad_out), _ptr(gx), N, M, D, int(p), float(eps),
-                                    _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_softmin_bwd_x")
-    count_launches(3)
+    gx = torch.empty_like(x)
+    scratch = _scratch(_query(dev, "b200ot_softmin_scratch_bytes", N, M, D), dev, "softmin")
+    _call(dev, "b200ot_softmin_bwd_x", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, N, M, D, int(p),
+          float(eps), scratch, scratch.numel(), launches=3)
     return gx
 
 
 class _Softmin(torch.autograd.Function):
-    """softmin(eps, (x, y), h) with the reference's autograd contract: the gradient flows to the row
-    cloud x only; y and h are treated as constants (they are ``.detach()``-ed at every call site of the
-    reference: sinkhorn_samples.py:392-393, sinkhorn_divergence.py:616-623)."""
+    """``scale_out * softmin(eps, (x, y), h_a + h_scale_b*h_b)`` with the reference's autograd contract: the gradient
+    flows to the row cloud x only; y and h are treated as constants (they are ``.detach()``-ed at every call site of
+    the reference: sinkhorn_samples.py:392-393, sinkhorn_divergence.py:616-623).
+
+    ``fwd`` and ``bwd`` are the forward and row-gradient operators of one kind of problem (one problem, a batch, the
+    p = 1 cost, ranges, column shards):
+        fwd(eps, x, y, h_a, h_b, h_scale_b, *, p, center, beta, want_lse2) -> (out, lse2)
+        bwd(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p, center) -> grad_x"""
 
     @staticmethod
-    def forward(ctx, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out):
-        need_grad = ctx.needs_input_grad[0]
-        out, lse2 = softmin_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out,
-                                want_lse2=need_grad)
+    def forward(ctx, fwd, bwd, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out):
+        need_grad = ctx.needs_input_grad[2]
+        out, lse2 = fwd(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out, want_lse2=need_grad)
         if need_grad:
-            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
-                                  lse2)
-            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), h_b is not None, center is not None)
+            ctx.bwd = bwd
+            ctx.save_for_backward(x, y, h_a, h_b, center, lse2)
+            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out))
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
-        h_scale_b, eps, p, scale_out, has_hb, has_center = ctx.meta
-        go = (grad_out * scale_out).contiguous()
-        gx = softmin_grad_rows(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, lse2, go, p=p,
-                               center=center if has_center else None)
-        return gx, None, None, None, None, None, None, None, None
+        h_scale_b, eps, p, scale_out = ctx.meta
+        gx = ctx.bwd(eps, x, y, h_a, h_b, h_scale_b, lse2, (grad_out * scale_out).contiguous(), p=p, center=center)
+        return (None, None, gx) + (None,) * 8
+
+
+def _softmin_apply(fwd, bwd, eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out):
+    """``_Softmin`` on the row cloud x, the columns and their potentials detached."""
+    return _Softmin.apply(fwd, bwd, x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps,
+                          p, center, scale_out)
 
 
 def softmin(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
     """Differentiable (w.r.t. x) ``scale_out * softmin(eps, (x, y.detach()), (h_a + h_scale_b*h_b).detach())``."""
-    return _Softmin.apply(x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps, p,
-                          center, scale_out)
+    return _softmin_apply(softmin_raw, softmin_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -252,15 +264,11 @@ def kernel_conv_raw(kind, x, y, w, blur, *, center=None):
     if w.numel() != M:
         raise ValueError("w must have one entry per column")
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.kernel_conv kind={kind} N={N} M={M} D={D}"):
+    with nvtx_range(f"b200ot.kernel_conv kind={kind} N={N} M={M} D={D}"):
         out = torch.empty(N, dtype=torch.float32, device=dev)
-        nbytes = L.b200ot_kernel_conv_scratch_bytes(N, M, D)
-        scratch = _scratch(nbytes, dev, "conv")
-        rc = L.b200ot_kernel_conv_fwd(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(out), N, M, D,
-                                      kind_id(kind), float(blur), _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_kernel_conv_fwd")
-    count_launches(3)
+        scratch = _scratch(_query(dev, "b200ot_kernel_conv_scratch_bytes", N, M, D), dev, "conv")
+        _call(dev, "b200ot_kernel_conv_fwd", x, y, w, center, out, N, M, D, kind_id(kind), float(blur), scratch,
+              scratch.numel(), launches=3)
     return out
 
 
@@ -271,16 +279,10 @@ def kernel_conv_grad_rows(kind, x, y, w, blur, grad_out, *, center=None):
     N, D = x.shape
     M = y.shape[0]
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        nbytes = L.b200ot_kernel_conv_scratch_bytes(N, M, D)
-        scratch = _scratch(nbytes, dev, "conv")
-        rc = L.b200ot_kernel_conv_bwd_x(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(grad_out), _ptr(gx), N, M, D,
-                                        kind_id(kind), float(blur), _ptr(scratch), scratch.numel(),
-                                        _stream(dev))
-    _lib.check(rc, "b200ot_kernel_conv_bwd_x")
-    count_launches(3)
+    gx = torch.empty_like(x)
+    scratch = _scratch(_query(dev, "b200ot_kernel_conv_scratch_bytes", N, M, D), dev, "conv")
+    _call(dev, "b200ot_kernel_conv_bwd_x", x, y, w, center, grad_out, gx, N, M, D, kind_id(kind), float(blur), scratch,
+          scratch.numel(), launches=3)
     return gx
 
 
@@ -296,16 +298,12 @@ def kernel_conv_value_and_grad_rows(kind, x, y, w, blur, *, center=None):
     if w.numel() != M:
         raise ValueError("w must have one entry per column")
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.kernel_conv value+grad kind={kind} N={N} M={M} D={D}"):
+    with nvtx_range(f"b200ot.kernel_conv value+grad kind={kind} N={N} M={M} D={D}"):
         out = torch.empty(N, dtype=torch.float32, device=dev)
         gunit = torch.empty_like(x)
-        nbytes = L.b200ot_kernel_conv_scratch_bytes(N, M, D)
-        scratch = _scratch(nbytes, dev, "conv")
-        rc = L.b200ot_kernel_conv_fwd_bwd_x(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(out), _ptr(gunit), N, M, D,
-                                            kind_id(kind), float(blur), _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_kernel_conv_fwd_bwd_x")
-    count_launches(3)
+        scratch = _scratch(_query(dev, "b200ot_kernel_conv_scratch_bytes", N, M, D), dev, "conv")
+        _call(dev, "b200ot_kernel_conv_fwd_bwd_x", x, y, w, center, out, gunit, N, M, D, kind_id(kind), float(blur),
+              scratch, scratch.numel(), launches=3)
     return out, gunit
 
 
@@ -318,43 +316,62 @@ def kernel_conv_value_and_grad_rows(kind, x, y, w, blur, *, center=None):
 FUSED_CONV_GRAD = _os.environ.get("B200OT_FUSED_CONV_GRAD", "1") == "1"
 
 
+class _ConvOps(NamedTuple):
+    """The operators of one kind of kernel matvec problem:
+        raw(kind, x, y, w, blur, *, center) -> out
+        grad_rows(kind, x, y, w, blur, grad_out, *, center) -> grad_x
+        value_and_grad_rows(kind, x, y, w, blur, *, center) -> (out, grad_unit), or None"""
+    raw: Callable
+    grad_rows: Callable
+    value_and_grad_rows: Optional[Callable] = None
+
+
 class _KernelConv(torch.autograd.Function):
-    """out = K(x, y) @ w, differentiable w.r.t. x, y and w (kernels are symmetric, so the y- and
-    w-gradients are the same reduction with the roles of the clouds swapped)."""
+    """out = K(x, y) @ w, differentiable w.r.t. x, y and w.  ``rows`` holds the operators of the problem (x against
+    y), ``cols`` those of its transpose (y against x): kernels are symmetric, so the y- and w-gradients are the same
+    reductions with the roles of the clouds swapped.  ``cols`` is None when the transpose is not available (ranges
+    problems built without it); ``fused``: value and unit row gradient from one pass (``rows.value_and_grad_rows``)."""
 
     @staticmethod
-    def forward(ctx, x, y, w, kind, blur, center, fused):
+    def forward(ctx, rows, cols, x, y, w, kind, blur, center, fused):
         if fused:
-            out, gunit = kernel_conv_value_and_grad_rows(kind, x, y, w, blur, center=center)
+            out, gunit = rows.value_and_grad_rows(kind, x, y, w, blur, center=center)
         else:
-            out, gunit = kernel_conv_raw(kind, x, y, w, blur, center=center), None
-        ctx.save_for_backward(x, y, w, center if center is not None else w, gunit if fused else w)
-        ctx.meta = (kind, float(blur), center is not None, fused)
+            out, gunit = rows.raw(kind, x, y, w, blur, center=center), None
+        ctx.ops = (rows, cols)
+        ctx.save_for_backward(x, y, w, center, gunit)
+        ctx.meta = (kind, float(blur))
         return out
 
     @staticmethod
     def backward(ctx, go):
         x, y, w, center, gunit = ctx.saved_tensors
-        kind, blur, has_center, fused = ctx.meta
-        center = center if has_center else None
+        rows, cols = ctx.ops
+        kind, blur = ctx.meta
         go = go.contiguous()
         gx = gy = gw = None
-        if ctx.needs_input_grad[0]:
-            if fused:
-                gx = go.unsqueeze(1) * gunit
-            else:
-                gx = kernel_conv_grad_rows(kind, x, y, w, blur, go, center=center)
-        if ctx.needs_input_grad[1]:
-            # d/dy_j sum_i go_i k(x_i, y_j) w_j = w_j * sum_i go_i dk(y_j, x_i)/dy_j
-            gy = kernel_conv_grad_rows(kind, y, x, go, blur, w, center=center)
         if ctx.needs_input_grad[2]:
-            gw = kernel_conv_raw(kind, y, x, go, blur, center=center)
-        return gx, gy, gw, None, None, None, None
+            if gunit is not None:
+                gx = go.unsqueeze(-1) * gunit
+            else:
+                gx = rows.grad_rows(kind, x, y, w, blur, go, center=center)
+        if (ctx.needs_input_grad[3] or ctx.needs_input_grad[4]) and cols is None:
+            raise RuntimeError("the transposed ranges problem is needed for gradients w.r.t. y / w")
+        if ctx.needs_input_grad[3]:
+            # d/dy_j sum_i go_i k(x_i, y_j) w_j = w_j * sum_i go_i dk(y_j, x_i)/dy_j
+            gy = cols.grad_rows(kind, y, x, go, blur, w, center=center)
+        if ctx.needs_input_grad[4]:
+            gw = cols.raw(kind, y, x, go, blur, center=center).view_as(w)
+        return None, None, gx, gy, gw, None, None, None, None
+
+
+def _fused(kind, x):
+    return bool(FUSED_CONV_GRAD and torch.is_grad_enabled() and x.requires_grad and (kind_id(kind) & 0xFF) == 0)
 
 
 def kernel_conv(kind, x, y, w, blur, *, center=None):
-    fused = (FUSED_CONV_GRAD and torch.is_grad_enabled() and x.requires_grad and (kind_id(kind) & 0xFF) == 0)
-    return _KernelConv.apply(x, y, w, kind, blur, center, bool(fused))
+    dense = _ConvOps(kernel_conv_raw, kernel_conv_grad_rows, kernel_conv_value_and_grad_rows)
+    return _KernelConv.apply(dense, dense, x, y, w, kind, blur, center, _fused(kind, x))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -382,8 +399,8 @@ def _per_point(t, n, name):
         raise ValueError(f"{name} must have one entry per point of its cloud ({n}), got {tuple(t.shape)}")
 
 
-def _batched_scratch(L, B, N, M, D, dev):
-    return _scratch(L.b200ot_batched_scratch_bytes(B, N, M, D), dev, "batched")
+def _batched_scratch(B, N, M, D, dev):
+    return _scratch(_query(dev, "b200ot_batched_scratch_bytes", B, N, M, D), dev, "batched")
 
 
 def softmin_batched_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, out_old=None, alpha_old=0.0,
@@ -399,17 +416,13 @@ def softmin_batched_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=
     _per_point(h_b, B * M, "h_b")
     _per_point(out_old, B * N, "out_old")
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.softmin_batched B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
+    with nvtx_range(f"b200ot.softmin_batched B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
         if out is None:
             out = torch.empty(B, N, dtype=torch.float32, device=dev)
         lse2 = torch.empty(B, N, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = _batched_scratch(L, B, N, M, D, dev)
-        rc = L.b200ot_softmin_fwd_batched(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
-                                          _ptr(out_old), float(alpha_old), float(beta), _ptr(out), _ptr(lse2), B, N,
-                                          M, D, int(p), float(eps), _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_softmin_fwd_batched")
-    count_launches(3)
+        scratch = _batched_scratch(B, N, M, D, dev)
+        _call(dev, "b200ot_softmin_fwd_batched", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
+              float(beta), out, lse2, B, N, M, D, int(p), float(eps), scratch, scratch.numel(), launches=3)
     return out, lse2
 
 
@@ -419,46 +432,17 @@ def softmin_batched_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *,
     center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
     B, N, M, D = _check_batch(x, y)
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        scratch = _batched_scratch(L, B, N, M, D, dev)
-        rc = L.b200ot_softmin_bwd_x_batched(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
-                                            _ptr(lse2), _ptr(grad_out), _ptr(gx), B, N, M, D, int(p), float(eps),
-                                            _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_softmin_bwd_x_batched")
-    count_launches(3)
+    gx = torch.empty_like(x)
+    scratch = _batched_scratch(B, N, M, D, dev)
+    _call(dev, "b200ot_softmin_bwd_x_batched", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, B, N, M,
+          D, int(p), float(eps), scratch, scratch.numel(), launches=3)
     return gx
-
-
-class _SoftminBatched(torch.autograd.Function):
-    """softmin_batched with _Softmin's autograd contract: the gradient flows to the row clouds x only."""
-
-    @staticmethod
-    def forward(ctx, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out):
-        need_grad = ctx.needs_input_grad[0]
-        out, lse2 = softmin_batched_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out,
-                                        want_lse2=need_grad)
-        if need_grad:
-            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
-                                  lse2)
-            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), h_b is not None, center is not None)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
-        h_scale_b, eps, p, scale_out, has_hb, has_center = ctx.meta
-        go = (grad_out * scale_out).contiguous()
-        gx = softmin_batched_grad_rows(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, lse2, go, p=p,
-                                       center=center if has_center else None)
-        return gx, None, None, None, None, None, None, None, None
 
 
 def softmin_batched(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
     """Differentiable (w.r.t. x) batched softmin, (B,N): ``softmin`` element by element."""
-    return _SoftminBatched.apply(x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps,
-                                 p, center, scale_out)
+    return _softmin_apply(softmin_batched_raw, softmin_batched_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center,
+                          scale_out)
 
 
 def _conv_batched_args(x, y, w, center):
@@ -472,15 +456,11 @@ def kernel_conv_batched_raw(kind, x, y, w, blur, *, center=None):
     """out (B,N), out[b, i] = sum_j k(x[b, i], y[b, j]) w[b, j], no autograd."""
     x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.kernel_conv_batched kind={kind} B={B} N={N} M={M} D={D}"):
+    with nvtx_range(f"b200ot.kernel_conv_batched kind={kind} B={B} N={N} M={M} D={D}"):
         out = torch.empty(B, N, dtype=torch.float32, device=dev)
-        scratch = _batched_scratch(L, B, N, M, D, dev)
-        rc = L.b200ot_kernel_conv_fwd_batched(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(out), B, N, M, D,
-                                              kind_id(kind), float(blur), _ptr(scratch), scratch.numel(),
-                                              _stream(dev))
-    _lib.check(rc, "b200ot_kernel_conv_fwd_batched")
-    count_launches(3)
+        scratch = _batched_scratch(B, N, M, D, dev)
+        _call(dev, "b200ot_kernel_conv_fwd_batched", x, y, w, center, out, B, N, M, D, kind_id(kind), float(blur),
+              scratch, scratch.numel(), launches=3)
     return out
 
 
@@ -489,15 +469,10 @@ def kernel_conv_batched_grad_rows(kind, x, y, w, blur, grad_out, *, center=None)
     grad_out = _f32c(grad_out, "grad_out")
     _per_point(grad_out, B * N, "grad_out")
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        scratch = _batched_scratch(L, B, N, M, D, dev)
-        rc = L.b200ot_kernel_conv_bwd_x_batched(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(grad_out), _ptr(gx), B,
-                                                N, M, D, kind_id(kind), float(blur), _ptr(scratch), scratch.numel(),
-                                                _stream(dev))
-    _lib.check(rc, "b200ot_kernel_conv_bwd_x_batched")
-    count_launches(3)
+    gx = torch.empty_like(x)
+    scratch = _batched_scratch(B, N, M, D, dev)
+    _call(dev, "b200ot_kernel_conv_bwd_x_batched", x, y, w, center, grad_out, gx, B, N, M, D, kind_id(kind),
+          float(blur), scratch, scratch.numel(), launches=3)
     return gx
 
 
@@ -507,56 +482,19 @@ def kernel_conv_batched_value_and_grad_rows(kind, x, y, w, blur, *, center=None)
         raise ValueError("the one-pass value + row gradient exists for the gaussian kernel only")
     x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.kernel_conv_batched value+grad B={B} N={N} M={M} D={D}"):
+    with nvtx_range(f"b200ot.kernel_conv_batched value+grad B={B} N={N} M={M} D={D}"):
         out = torch.empty(B, N, dtype=torch.float32, device=dev)
         gunit = torch.empty_like(x)
-        scratch = _batched_scratch(L, B, N, M, D, dev)
-        rc = L.b200ot_kernel_conv_fwd_bwd_x_batched(_ptr(x), _ptr(y), _ptr(w), _ptr(center), _ptr(out), _ptr(gunit),
-                                                    B, N, M, D, kind_id(kind), float(blur), _ptr(scratch),
-                                                    scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_kernel_conv_fwd_bwd_x_batched")
-    count_launches(3)
+        scratch = _batched_scratch(B, N, M, D, dev)
+        _call(dev, "b200ot_kernel_conv_fwd_bwd_x_batched", x, y, w, center, out, gunit, B, N, M, D, kind_id(kind),
+              float(blur), scratch, scratch.numel(), launches=3)
     return out, gunit
-
-
-class _KernelConvBatched(torch.autograd.Function):
-    """kernel_conv_batched with _KernelConv's contract: gradients to x, y and w; `fused`: the gaussian value and unit
-    row gradient from one pass."""
-
-    @staticmethod
-    def forward(ctx, x, y, w, kind, blur, center, fused):
-        if fused:
-            out, gunit = kernel_conv_batched_value_and_grad_rows(kind, x, y, w, blur, center=center)
-        else:
-            out, gunit = kernel_conv_batched_raw(kind, x, y, w, blur, center=center), None
-        ctx.save_for_backward(x, y, w, center if center is not None else w, gunit if fused else w)
-        ctx.meta = (kind, float(blur), center is not None, fused)
-        return out
-
-    @staticmethod
-    def backward(ctx, go):
-        x, y, w, center, gunit = ctx.saved_tensors
-        kind, blur, has_center, fused = ctx.meta
-        center = center if has_center else None
-        go = go.contiguous()
-        gx = gy = gw = None
-        if ctx.needs_input_grad[0]:
-            if fused:
-                gx = go.unsqueeze(-1) * gunit
-            else:
-                gx = kernel_conv_batched_grad_rows(kind, x, y, w, blur, go, center=center)
-        if ctx.needs_input_grad[1]:
-            gy = kernel_conv_batched_grad_rows(kind, y, x, go, blur, w, center=center)
-        if ctx.needs_input_grad[2]:
-            gw = kernel_conv_batched_raw(kind, y, x, go, blur, center=center).view_as(w)
-        return gx, gy, gw, None, None, None, None
 
 
 def kernel_conv_batched(kind, x, y, w, blur, *, center=None):
     """out (B,N) = K(x[b], y[b]) @ w[b] for every b, differentiable w.r.t. x, y and w."""
-    fused = (FUSED_CONV_GRAD and torch.is_grad_enabled() and x.requires_grad and (kind_id(kind) & 0xFF) == 0)
-    return _KernelConvBatched.apply(x, y, w, kind, blur, center, bool(fused))
+    batched = _ConvOps(kernel_conv_batched_raw, kernel_conv_batched_grad_rows, kernel_conv_batched_value_and_grad_rows)
+    return _KernelConv.apply(batched, batched, x, y, w, kind, blur, center, _fused(kind, x))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -583,17 +521,14 @@ def softmin_l1_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None,
     _per_point(out_old, B * N, "out_old")
     shape = (B, N) if batched else (N,)
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev), nvtx_range(f"b200ot.softmin_l1 B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
+    with nvtx_range(f"b200ot.softmin_l1 B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
         if out is None:
             out = torch.empty(shape, dtype=torch.float32, device=dev)
         lse2 = torch.empty(shape, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = _scratch(L.b200ot_softmin_l1_scratch_bytes(B, N, M, D), dev, "softmin_l1")
-        rc = L.b200ot_softmin_l1_fwd(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
-                                     _ptr(out_old), float(alpha_old), float(beta), _ptr(out), _ptr(lse2), B, N, M, D,
-                                     int(p), float(eps), _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_softmin_l1_fwd")
-    count_launches(5)  # coordinate maximum, two packs, reduction, finalize
+        scratch = _scratch(_query(dev, "b200ot_softmin_l1_scratch_bytes", B, N, M, D), dev, "softmin_l1")
+        # coordinate maximum, two packs, reduction, finalize
+        _call(dev, "b200ot_softmin_l1_fwd", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
+              float(beta), out, lse2, B, N, M, D, int(p), float(eps), scratch, scratch.numel(), launches=5)
     return out, lse2
 
 
@@ -605,43 +540,14 @@ def softmin_l1_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=1,
     _per_point(grad_out, B * N, "grad_out")
     _per_point(lse2, B * N, "lse2")
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        scratch = _scratch(L.b200ot_softmin_l1_scratch_bytes(B, N, M, D), dev, "softmin_l1")
-        rc = L.b200ot_softmin_l1_bwd_x(_ptr(x), _ptr(y), _ptr(h_a), _ptr(h_b), float(h_scale_b), _ptr(center),
-                                       _ptr(lse2), _ptr(grad_out), _ptr(gx), B, N, M, D, int(p), float(eps),
-                                       _ptr(scratch), scratch.numel(), _stream(dev))
-    _lib.check(rc, "b200ot_softmin_l1_bwd_x")
-    count_launches(5)  # coordinate maximum, two packs, reduction, finalize
+    gx = torch.empty_like(x)
+    scratch = _scratch(_query(dev, "b200ot_softmin_l1_scratch_bytes", B, N, M, D), dev, "softmin_l1")
+    # coordinate maximum, two packs, reduction, finalize
+    _call(dev, "b200ot_softmin_l1_bwd_x", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, B, N, M, D,
+          int(p), float(eps), scratch, scratch.numel(), launches=5)
     return gx
-
-
-class _SoftminL1(torch.autograd.Function):
-    """softmin_l1 with _Softmin's autograd contract: the gradient flows to the row cloud x only."""
-
-    @staticmethod
-    def forward(ctx, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out):
-        need_grad = ctx.needs_input_grad[0]
-        out, lse2 = softmin_l1_raw(eps, x, y, h_a, h_b, h_scale_b, p=p, center=center, beta=scale_out,
-                                   want_lse2=need_grad)
-        if need_grad:
-            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
-                                  lse2)
-            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), h_b is not None, center is not None)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
-        h_scale_b, eps, p, scale_out, has_hb, has_center = ctx.meta
-        go = (grad_out * scale_out).contiguous()
-        gx = softmin_l1_grad_rows(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, lse2, go, p=p,
-                                  center=center if has_center else None)
-        return gx, None, None, None, None, None, None, None, None
 
 
 def softmin_l1(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, scale_out=1.0):
     """Differentiable (w.r.t. x) ``scale_out * softmin_l1_raw(...)``, for (N,D) or (B,N,D) clouds."""
-    return _SoftminL1.apply(x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps, p,
-                            center, scale_out)
+    return _softmin_apply(softmin_l1_raw, softmin_l1_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)

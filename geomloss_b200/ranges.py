@@ -24,6 +24,7 @@ padding rows write nothing.
 from __future__ import annotations
 
 import ctypes
+from functools import partial
 
 import torch
 
@@ -208,35 +209,26 @@ def softmin_shard_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=No
     if N != prob.n_rows or y.shape[0] != prob.layout.n_cols:
         raise ValueError("point clouds do not match the ranges problem they are reduced with")
     dev = x.device
-    L = _lib.lib()
     lay = prob.layout
-    with torch.cuda.device(dev):
-        if part is None:
-            part = torch.empty(N, 2, dtype=torch.float32, device=dev)
-        cols = ops._scratch(L.b200ot_packed_cols_floats(lay.n_slots, D, 1) * 4, dev, "ranges_cols")
-        st = ops._stream(dev)
-        _lib.check(L.b200ot_softmin_pack_gather(ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b), float(h_scale_b),
-                                                ops._ptr(center), ops._ptr(lay.src), lay.n_slots, D, int(p),
-                                                float(eps), ops._ptr(cols), st), "b200ot_softmin_pack_gather")
-        _lib.check(L.b200ot_softmin_partial_ranges(ops._ptr(x), ops._ptr(center), ops._ptr(cols), ops._ptr(prob.seg),
-                                                   prob.n_seg, ops._ptr(prob.pieces), ops._ptr(part), N, D, int(p),
-                                                   float(eps), prob.variant, st), "b200ot_softmin_partial_ranges")
-    ops.count_launches(2)
+    if part is None:
+        part = torch.empty(N, 2, dtype=torch.float32, device=dev)
+    cols = ops._scratch(_lib.lib().b200ot_packed_cols_floats(lay.n_slots, D, 1) * 4, dev, "ranges_cols")
+    ops._call(dev, "b200ot_softmin_pack_gather", y, h_a, h_b, float(h_scale_b), center, lay.src, lay.n_slots, D,
+              int(p), float(eps), cols, launches=1)
+    ops._call(dev, "b200ot_softmin_partial_ranges", x, center, cols, prob.seg, prob.n_seg, prob.pieces, part, N, D,
+              int(p), float(eps), prob.variant, launches=1)
     return part
 
 
 def softmin_finalize(parts, n_part, eps, out_old, alpha_old, beta, want_lse2, out=None):
+    """Merge the ``n_part`` (m, s) partials ``parts`` (n_part, N, 2) per row, with the fused Sinkhorn epilogue."""
     N = parts.shape[-2]
     dev = parts.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        if out is None:
-            out = torch.empty(N, dtype=torch.float32, device=dev)
-        lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
-        _lib.check(L.b200ot_softmin_finalize(ops._ptr(parts), int(n_part), ops._ptr(ops._f32c(out_old, "out_old")),
-                                             float(alpha_old), float(beta), ops._ptr(out), ops._ptr(lse2), N,
-                                             float(eps), ops._stream(dev)), "b200ot_softmin_finalize")
-    ops.count_launches(1)
+    if out is None:
+        out = torch.empty(N, dtype=torch.float32, device=dev)
+    lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
+    ops._call(dev, "b200ot_softmin_finalize", parts, int(n_part), ops._f32c(out_old, "out_old"), float(alpha_old),
+              float(beta), out, lse2, N, float(eps), launches=1)
     return out, lse2
 
 
@@ -248,13 +240,12 @@ def _blocks_args(prob, x, y):
     rl, cl = prob.row_layout, prob.layout
     nbytes = prob._scratch_bytes.get(D)
     if nbytes is None:
-        nbytes = _lib.lib().b200ot_blocks_scratch_bytes(N, rl.n_slots, cl.n_slots, ops._ptr(prob.seg), prob.n_seg,
-                                                        ops._ptr(prob.pieces), D)
+        nbytes = ops._query(x.device, "b200ot_blocks_scratch_bytes", N, rl.n_slots, cl.n_slots, ops._ptr(prob.seg),
+                            prob.n_seg, ops._ptr(prob.pieces), D)
         if nbytes <= 0:
             raise ValueError("invalid tensor-core block problem")
         prob._scratch_bytes[D] = nbytes
-    return (N, ops._ptr(rl.src), rl.n_slots, ops._ptr(cl.src), cl.n_slots, ops._ptr(prob.seg), prob.n_seg,
-            ops._ptr(prob.pieces), D), nbytes
+    return (N, rl.src, rl.n_slots, cl.src, cl.n_slots, prob.seg, prob.n_seg, prob.pieces, D), nbytes
 
 
 def softmin_blocks_raw(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None, out_old=None, alpha_old=0.0,
@@ -264,19 +255,13 @@ def softmin_blocks_raw(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None
                                                                     (center, "center"), (out_old, "out_old")))
     _check_path(prob, x.shape[1])
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        (N, *rest), nbytes = _blocks_args(prob, x, y)
-        if out is None:
-            out = torch.empty(N, dtype=torch.float32, device=dev)
-        lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = ops._scratch(nbytes, dev, "blocks")
-        _lib.check(L.b200ot_softmin_fwd_blocks(ops._ptr(x), ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b),
-                                               float(h_scale_b), ops._ptr(center), ops._ptr(out_old),
-                                               float(alpha_old), float(beta), ops._ptr(out), ops._ptr(lse2), N, *rest,
-                                               int(p), float(eps), ops._ptr(scratch), nbytes, ops._stream(dev)),
-                   "b200ot_softmin_fwd_blocks")
-    ops.count_launches(4)
+    (N, *rest), nbytes = _blocks_args(prob, x, y)
+    if out is None:
+        out = torch.empty(N, dtype=torch.float32, device=dev)
+    lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
+    scratch = ops._scratch(nbytes, dev, "blocks")
+    ops._call(dev, "b200ot_softmin_fwd_blocks", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
+              float(beta), out, lse2, N, *rest, int(p), float(eps), scratch, nbytes, launches=4)
     return out, lse2
 
 
@@ -286,17 +271,11 @@ def softmin_blocks_bwd_x(eps, x, y, h_a, h_b, h_scale_b, prob, lse2, grad_out, *
                                      (lse2, "lse2"), (grad_out, "grad_out")))
     _check_path(prob, x.shape[1])
     dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        (N, *rest), nbytes = _blocks_args(prob, x, y)
-        gx = torch.empty_like(x)
-        scratch = ops._scratch(nbytes, dev, "blocks")
-        _lib.check(L.b200ot_softmin_bwd_x_blocks(ops._ptr(x), ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b),
-                                                 float(h_scale_b), ops._ptr(center), ops._ptr(lse2),
-                                                 ops._ptr(grad_out), ops._ptr(gx), N, *rest, int(p), float(eps),
-                                                 ops._ptr(scratch), nbytes, ops._stream(dev)),
-                   "b200ot_softmin_bwd_x_blocks")
-    ops.count_launches(4)
+    (N, *rest), nbytes = _blocks_args(prob, x, y)
+    gx = torch.empty_like(x)
+    scratch = ops._scratch(nbytes, dev, "blocks")
+    ops._call(dev, "b200ot_softmin_bwd_x_blocks", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, N,
+              *rest, int(p), float(eps), scratch, nbytes, launches=4)
     return gx
 
 
@@ -318,70 +297,38 @@ def softmin_bwd_shard_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, lse2, *, p=2,
     if prob.variant == TC:
         raise ValueError("tensor-core block problems run as one call (softmin_blocks_bwd_x), without exposed sums")
     dev = x.device
-    L = _lib.lib()
     lay = prob.layout
-    with torch.cuda.device(dev):
-        sums = torch.zeros(N, D + 1, dtype=torch.float32, device=dev)
-        cols = ops._scratch(L.b200ot_packed_cols_floats(lay.n_slots, D, 1) * 4, dev, "ranges_cols")
-        st = ops._stream(dev)
-        _lib.check(L.b200ot_softmin_pack_gather(ops._ptr(y), ops._ptr(h_a), ops._ptr(h_b), float(h_scale_b),
-                                                ops._ptr(center), ops._ptr(lay.src), lay.n_slots, D, int(p),
-                                                float(eps), ops._ptr(cols), st), "b200ot_softmin_pack_gather")
-        _lib.check(L.b200ot_softmin_bwd_partial_ranges(ops._ptr(x), ops._ptr(center), ops._ptr(cols), ops._ptr(lse2),
-                                                       ops._ptr(prob.seg), prob.n_seg, ops._ptr(prob.pieces),
-                                                       ops._ptr(sums), N, D, int(p), float(eps), prob.variant, st),
-                   "b200ot_softmin_bwd_partial_ranges")
-    ops.count_launches(2)
+    sums = torch.zeros(N, D + 1, dtype=torch.float32, device=dev)
+    cols = ops._scratch(_lib.lib().b200ot_packed_cols_floats(lay.n_slots, D, 1) * 4, dev, "ranges_cols")
+    ops._call(dev, "b200ot_softmin_pack_gather", y, h_a, h_b, float(h_scale_b), center, lay.src, lay.n_slots, D,
+              int(p), float(eps), cols, launches=1)
+    ops._call(dev, "b200ot_softmin_bwd_partial_ranges", x, center, cols, lse2, prob.seg, prob.n_seg, prob.pieces, sums,
+              N, D, int(p), float(eps), prob.variant, launches=1)
     return sums
 
 
 def softmin_bwd_finalize(sums, eps, x, center, grad_out, p):
+    """grad_x from the (N, D+1) row-gradient sums of all the column pieces (summed over shards)."""
     x, center, grad_out = ops._f32c(x, "x"), ops._f32c(center, "center"), ops._f32c(grad_out, "grad_out")
     N, D = x.shape
-    dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        _lib.check(L.b200ot_softmin_bwd_finalize(ops._ptr(sums), 1, ops._ptr(x), ops._ptr(center),
-                                                 ops._ptr(grad_out), ops._ptr(gx), N, D, int(p), float(eps),
-                                                 ops._stream(dev)), "b200ot_softmin_bwd_finalize")
-    ops.count_launches(1)
+    gx = torch.empty_like(x)
+    ops._call(x.device, "b200ot_softmin_bwd_finalize", sums, 1, x, center, grad_out, gx, N, D, int(p), float(eps),
+              launches=1)
     return gx
 
 
-class _RangesSoftmin(torch.autograd.Function):
-    """Ranges-mode softmin with the reference's autograd contract (gradient to the row cloud only)."""
-
-    @staticmethod
-    def forward(ctx, x, y, h_a, h_b, h_scale_b, eps, p, center, scale_out, prob):
-        need = ctx.needs_input_grad[0]
-        out, lse2 = softmin_ranges_raw(eps, x, y, h_a, h_b, h_scale_b, prob, p=p, center=center, beta=scale_out,
-                                       want_lse2=need)
-        if need:
-            ctx.save_for_backward(x, y, h_a, h_b if h_b is not None else h_a, center if center is not None else h_a,
-                                  lse2)
-            ctx.meta = (float(h_scale_b), float(eps), int(p), float(scale_out), prob, h_b is not None,
-                        center is not None)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        x, y, h_a, h_b, center, lse2 = ctx.saved_tensors
-        h_scale_b, eps, p, scale_out, prob, has_hb, has_center = ctx.meta
-        center = center if has_center else None
-        if prob.variant == TC:
-            gx = softmin_blocks_bwd_x(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, prob, lse2,
-                                      (grad_out * scale_out).contiguous(), p=p, center=center)
-            return gx, None, None, None, None, None, None, None, None, None
-        sums = softmin_bwd_shard_ranges(eps, x, y, h_a, h_b if has_hb else None, h_scale_b, prob, lse2, p=p,
-                                        center=center)
-        gx = softmin_bwd_finalize(sums, eps, x, center, (grad_out * scale_out).contiguous(), p)
-        return gx, None, None, None, None, None, None, None, None, None
+def softmin_ranges_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None, prob):
+    """grad_x of <grad_out, softmin_ranges_raw(eps, x, y, h, prob)> with y, h constant (the row-gradient operator of
+    ``ops._Softmin``, ``prob`` bound by keyword)."""
+    if prob.variant == TC:
+        return softmin_blocks_bwd_x(eps, x, y, h_a, h_b, h_scale_b, prob, lse2, grad_out, p=p, center=center)
+    sums = softmin_bwd_shard_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, lse2, p=p, center=center)
+    return softmin_bwd_finalize(sums, eps, x, center, grad_out, p)
 
 
 def softmin_ranges(eps, x, y, h_a, h_b, h_scale_b, prob, *, p=2, center=None, scale_out=1.0):
-    return _RangesSoftmin.apply(x, y.detach(), h_a.detach(), None if h_b is None else h_b.detach(), h_scale_b, eps, p,
-                                center, scale_out, prob)
+    return ops._softmin_apply(partial(softmin_ranges_raw, prob=prob), partial(softmin_ranges_grad_rows, prob=prob),
+                              eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -400,82 +347,48 @@ def conv_shard_ranges(kind_id, x, y, w, blur, prob, *, center=None, backward=Fal
     if N != prob.n_rows or y.shape[0] != prob.layout.n_cols:
         raise ValueError("point clouds do not match the ranges problem they are reduced with")
     dev = x.device
-    L = _lib.lib()
     lay = prob.layout
-    width = _conv_width(kind_id, D, backward)
-    with torch.cuda.device(dev):
-        part = torch.zeros(N, width, dtype=torch.float32, device=dev)
-        cols = ops._scratch(L.b200ot_packed_cols_floats(lay.n_slots, D, 2) * 4, dev, "ranges_cols")
-        st = ops._stream(dev)
-        _lib.check(L.b200ot_kernel_conv_pack_gather(ops._ptr(y), ops._ptr(w), ops._ptr(center), ops._ptr(lay.src),
-                                                    lay.n_slots, D, int(kind_id), float(blur), ops._ptr(cols), st),
-                   "b200ot_kernel_conv_pack_gather")
-        _lib.check(L.b200ot_kernel_conv_partial_ranges(ops._ptr(x), ops._ptr(center), ops._ptr(cols),
-                                                       ops._ptr(prob.seg), prob.n_seg, ops._ptr(prob.pieces),
-                                                       ops._ptr(part), N, D, int(kind_id), float(blur),
-                                                       1 if backward else 0, prob.variant, st),
-                   "b200ot_kernel_conv_partial_ranges")
-    ops.count_launches(2)
+    part = torch.zeros(N, _conv_width(kind_id, D, backward), dtype=torch.float32, device=dev)
+    cols = ops._scratch(_lib.lib().b200ot_packed_cols_floats(lay.n_slots, D, 2) * 4, dev, "ranges_cols")
+    ops._call(dev, "b200ot_kernel_conv_pack_gather", y, w, center, lay.src, lay.n_slots, D, int(kind_id), float(blur),
+              cols, launches=1)
+    ops._call(dev, "b200ot_kernel_conv_partial_ranges", x, center, cols, prob.seg, prob.n_seg, prob.pieces, part, N, D,
+              int(kind_id), float(blur), 1 if backward else 0, prob.variant, launches=1)
     return part
 
 
 def conv_finalize(kind_id, part):
     N = part.shape[0]
-    dev = part.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        out = torch.empty(N, dtype=torch.float32, device=dev)
-        _lib.check(L.b200ot_kernel_conv_finalize(ops._ptr(part), 1, ops._ptr(out), N, int(kind_id), ops._stream(dev)),
-                   "b200ot_kernel_conv_finalize")
-    ops.count_launches(1)
+    out = torch.empty(N, dtype=torch.float32, device=part.device)
+    ops._call(part.device, "b200ot_kernel_conv_finalize", part, 1, out, N, int(kind_id), launches=1)
     return out
 
 
 def conv_bwd_finalize(kind_id, part, x, center, grad_out, blur):
     x, center, grad_out = ops._f32c(x, "x"), ops._f32c(center, "center"), ops._f32c(grad_out, "grad_out")
     N, D = x.shape
-    dev = x.device
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        gx = torch.empty_like(x)
-        _lib.check(L.b200ot_kernel_conv_bwd_finalize(ops._ptr(part), 1, ops._ptr(x), ops._ptr(center),
-                                                     ops._ptr(grad_out), ops._ptr(gx), N, D, int(kind_id),
-                                                     float(blur), ops._stream(dev)), "b200ot_kernel_conv_bwd_finalize")
-    ops.count_launches(1)
+    gx = torch.empty_like(x)
+    ops._call(x.device, "b200ot_kernel_conv_bwd_finalize", part, 1, x, center, grad_out, gx, N, D, int(kind_id),
+              float(blur), launches=1)
     return gx
 
 
-class _RangesConv(torch.autograd.Function):
-    """out = (K(x, y) restricted to prob) @ w, differentiable w.r.t. x, y and w; ``prob_t`` is the transposed problem
-    (rows y, columns x) that serves the y- and w-gradients (kernels are symmetric)."""
+def _conv_ops(prob):
+    """``ops._ConvOps`` of the ranges problem ``prob`` (None: no operators)."""
+    if prob is None:
+        return None
 
-    @staticmethod
-    def forward(ctx, x, y, w, kind_id, blur, center, prob, prob_t):
-        out = conv_finalize(kind_id, conv_shard_ranges(kind_id, x, y, w, blur, prob, center=center))
-        ctx.save_for_backward(x, y, w, center if center is not None else w)
-        ctx.meta = (kind_id, float(blur), center is not None, prob, prob_t)
-        return out
+    def raw(kind_id, x, y, w, blur, *, center=None):
+        return conv_finalize(kind_id, conv_shard_ranges(kind_id, x, y, w, blur, prob, center=center))
 
-    @staticmethod
-    def backward(ctx, go):
-        x, y, w, center = ctx.saved_tensors
-        kind_id, blur, has_center, prob, prob_t = ctx.meta
-        center = center if has_center else None
-        go = go.contiguous()
-        gx = gy = gw = None
-        if ctx.needs_input_grad[0]:
-            part = conv_shard_ranges(kind_id, x, y, w, blur, prob, center=center, backward=True)
-            gx = conv_bwd_finalize(kind_id, part, x, center, go, blur)
-        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            if prob_t is None:
-                raise RuntimeError("the transposed ranges problem is needed for gradients w.r.t. y / w")
-        if ctx.needs_input_grad[1]:
-            part = conv_shard_ranges(kind_id, y, x, go, blur, prob_t, center=center, backward=True)
-            gy = conv_bwd_finalize(kind_id, part, y, center, w, blur)
-        if ctx.needs_input_grad[2]:
-            gw = conv_finalize(kind_id, conv_shard_ranges(kind_id, y, x, go, blur, prob_t, center=center))
-        return gx, gy, gw, None, None, None, None, None
+    def grad_rows(kind_id, x, y, w, blur, grad_out, *, center=None):
+        part = conv_shard_ranges(kind_id, x, y, w, blur, prob, center=center, backward=True)
+        return conv_bwd_finalize(kind_id, part, x, center, grad_out, blur)
+
+    return ops._ConvOps(raw, grad_rows)
 
 
 def kernel_conv_ranges(kind_id, x, y, w, blur, prob, prob_t=None, *, center=None):
-    return _RangesConv.apply(x, y, w, kind_id, blur, center, prob, prob_t)
+    """out = (K(x, y) restricted to prob) @ w, differentiable w.r.t. x, y and w; ``prob_t`` is the transposed problem
+    (rows y, columns x) that serves the y- and w-gradients (kernels are symmetric)."""
+    return ops._KernelConv.apply(_conv_ops(prob), _conv_ops(prob_t), x, y, w, kind_id, blur, center, False)

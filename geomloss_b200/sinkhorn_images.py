@@ -18,7 +18,7 @@ import numpy as np
 import torch
 from torch.nn.functional import avg_pool2d, avg_pool3d, interpolate
 
-from . import _lib, ops
+from . import ops
 from .sinkhorn import damping, epsilon_schedule
 
 
@@ -62,13 +62,8 @@ def softmin_grid(eps, p, h_a, h_b=None, h_scale_b=0.0, *, out_old=None, alpha_ol
         raise ValueError("grid sides must be equal")
     dev = h_a.device
     out = torch.empty_like(h_a)
-    L = _lib.lib()
-    with torch.cuda.device(dev):
-        rc = L.b200ot_softmin_grid(ops._ptr(h_a), ops._ptr(h_b), float(h_scale_b), ops._ptr(out_old), float(alpha_old),
-                                   float(beta), ops._ptr(out), h_a.shape[0] * h_a.shape[1], N, d, int(p), float(eps),
-                                   ops._stream(dev))
-    _lib.check(rc, "b200ot_softmin_grid")
-    ops.count_launches(d)
+    ops._call(dev, "b200ot_softmin_grid", h_a, h_b, float(h_scale_b), out_old, float(alpha_old), float(beta), out,
+              h_a.shape[0] * h_a.shape[1], N, d, int(p), float(eps), launches=d)
     return out
 
 

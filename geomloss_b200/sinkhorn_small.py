@@ -14,7 +14,7 @@ import ctypes
 
 import torch
 
-from . import _lib, ops
+from . import ops
 from .sinkhorn import damping, extent_diameter, scaling_parameters, sinkhorn_cost_batched
 
 # largest cloud served by the one-launch-per-iteration kernels; beyond, the tiled TMA kernels win
@@ -42,14 +42,9 @@ def _descent(x, y, a, b, eps_list, rho, p, debias, lh):
     bufs = torch.empty(2, B * (2 * N + 2 * M), dtype=torch.float32, device=dev)
     eps_arr = (ctypes.c_double * len(eps_list))(*[float(e) for e in eps_list])
     which = ctypes.c_int32(0)
-    L = _lib.lib()
-    P = ops._ptr
-    with torch.cuda.device(dev):
-        rc = L.b200ot_sinkhorn_loop_small(P(x), P(y), P(a), P(b), 1, eps_arr, len(eps_list),
-                                          -1.0 if rho is None else float(rho), 1 if debias else 0, P(bufs[0]),
-                                          P(bufs[1]), ctypes.byref(which), B, N, M, D, int(p), P(lh), ops._stream(dev))
-    _lib.check(rc, "b200ot_sinkhorn_loop_small")
-    ops.count_launches(len(eps_list) + 1)
+    ops._call(dev, "b200ot_sinkhorn_loop_small", x, y, a, b, 1, eps_arr, len(eps_list),
+              -1.0 if rho is None else float(rho), 1 if debias else 0, bufs[0], bufs[1], ctypes.byref(which), B, N, M,
+              D, int(p), lh, launches=len(eps_list) + 1)
     return _views(bufs[0] if which.value else bufs[1], B, N, M, debias)
 
 
@@ -65,14 +60,8 @@ class _FinalStep(torch.autograd.Function):
         n_f_ba, n_g_ab, n_f_aa, n_g_bb = _views(new, B, N, M, debias)
         need = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         lse2 = torch.empty(B * (2 * N + 2 * M), device=dev) if need else None
-        L = _lib.lib()
-        P = ops._ptr
-        with torch.cuda.device(dev):
-            rc = L.b200ot_sinkhorn_iteration_small(P(x), P(y), P(a), P(b), P(f_ba), P(g_ab), P(f_aa), P(g_bb),
-                                                   P(n_f_ba), P(n_g_ab), P(n_f_aa), P(n_g_bb), P(lse2), B, N, M, D,
-                                                   int(p), float(eps), 0.0, float(lam), 1, P(lh), ops._stream(dev))
-        _lib.check(rc, "b200ot_sinkhorn_iteration_small")
-        ops.count_launches(1)
+        ops._call(dev, "b200ot_sinkhorn_iteration_small", x, y, a, b, f_ba, g_ab, f_aa, g_bb, n_f_ba, n_g_ab, n_f_aa,
+                  n_g_bb, lse2, B, N, M, D, int(p), float(eps), 0.0, float(lam), 1, lh, launches=1)
         if need:
             ctx.save_for_backward(x, y, a, b, f_ba, g_ab, f_aa if debias else f_ba, g_bb if debias else g_ab, lse2, lh)
             ctx.meta = (float(eps), float(lam), int(p), bool(debias))
@@ -88,15 +77,8 @@ class _FinalStep(torch.autograd.Function):
         M = y.shape[1]
         gos = [None if g is None else g.contiguous() for g in gos] + [None] * (4 - len(gos))
         gx, gy = torch.empty_like(x), torch.empty_like(y)
-        L = _lib.lib()
-        P = ops._ptr
-        with torch.cuda.device(x.device):
-            rc = L.b200ot_sinkhorn_final_bwd_small(P(x), P(y), P(a), P(b), P(f_ba), P(g_ab),
-                                                   P(f_aa) if debias else None, P(g_bb) if debias else None, P(lse2),
-                                                   P(gos[0]), P(gos[1]), P(gos[2]), P(gos[3]), P(gx), P(gy), B, N, M,
-                                                   D, p, eps, lam, None, 1, P(lh), ops._stream(x.device))
-        _lib.check(rc, "b200ot_sinkhorn_final_bwd_small")
-        ops.count_launches(1)
+        ops._call(x.device, "b200ot_sinkhorn_final_bwd_small", x, y, a, b, f_ba, g_ab, f_aa if debias else None,
+                  g_bb if debias else None, lse2, *gos, gx, gy, B, N, M, D, p, eps, lam, None, 1, lh, launches=1)
         return (gx, gy) + (None,) * 11
 
 
@@ -120,24 +102,14 @@ class _FinalValue(torch.autograd.Function):
         n_f_ba, n_g_ab, n_f_aa, n_g_bb = _views(new, B, N, M, debias)
         go_f_ba, go_g_ab, go_f_aa, go_g_bb = _views(gos, B, N, M, debias)
         ad, bd = a.detach(), b.detach()
-        L = _lib.lib()
-        P = ops._ptr
-        with torch.cuda.device(dev):
-            st = ops._stream(dev)
-            rc = L.b200ot_sinkhorn_iteration_small(P(x), P(y), P(ad), P(bd), P(f_ba), P(g_ab), P(f_aa), P(g_bb),
-                                                   P(n_f_ba), P(n_g_ab), P(n_f_aa), P(n_g_bb),
-                                                   P(lse2) if need_xy else None, B, N, M, D, int(p), float(eps), 0.0,
-                                                   float(lam), 1, P(lh), st)
-            _lib.check(rc, "b200ot_sinkhorn_iteration_small")
-            rc = L.b200ot_sinkhorn_cost_small(P(ad), P(bd), P(n_f_ba), P(n_g_ab), P(n_f_aa), P(n_g_bb), B, N, M,
-                                              -1.0 if rho is None else float(rho), float(eps_final), P(value),
-                                              P(go_f_ba) if need_xy else None, P(go_g_ab) if need_xy else None,
-                                              P(go_f_aa) if need_xy and debias else None,
-                                              P(go_g_bb) if need_xy and debias else None,
-                                              P(terms[: B * N]) if need_w else None,
-                                              P(terms[B * N:]) if need_w else None, st)
-            _lib.check(rc, "b200ot_sinkhorn_cost_small")
-        ops.count_launches(2)
+        ops._call(dev, "b200ot_sinkhorn_iteration_small", x, y, ad, bd, f_ba, g_ab, f_aa, g_bb, n_f_ba, n_g_ab, n_f_aa,
+                  n_g_bb, lse2 if need_xy else None, B, N, M, D, int(p), float(eps), 0.0, float(lam), 1, lh,
+                  launches=1)
+        ops._call(dev, "b200ot_sinkhorn_cost_small", ad, bd, n_f_ba, n_g_ab, n_f_aa, n_g_bb, B, N, M,
+                  -1.0 if rho is None else float(rho), float(eps_final), value, go_f_ba if need_xy else None,
+                  go_g_ab if need_xy else None, go_f_aa if need_xy and debias else None,
+                  go_g_bb if need_xy and debias else None, terms[: B * N] if need_w else None,
+                  terms[B * N:] if need_w else None, launches=1)
         if need_xy or need_w:
             ctx.save_for_backward(x, y, ad, bd, f_ba, g_ab, f_aa if debias else f_ba, g_bb if debias else g_ab, work,
                                   lh)
@@ -157,16 +129,9 @@ class _FinalValue(torch.autograd.Function):
             lse2, gos = work[tot: 2 * tot], work[2 * tot: 3 * tot]
             go_f_ba, go_g_ab, go_f_aa, go_g_bb = _views(gos, B, N, M, debias)
             gx, gy = torch.empty_like(x), torch.empty_like(y)
-            L = _lib.lib()
-            P = ops._ptr
-            with torch.cuda.device(x.device):
-                rc = L.b200ot_sinkhorn_final_bwd_small(P(x), P(y), P(a), P(b), P(f_ba), P(g_ab),
-                                                       P(f_aa) if debias else None, P(g_bb) if debias else None,
-                                                       P(lse2), P(go_f_ba), P(go_g_ab), P(go_f_aa), P(go_g_bb), P(gx),
-                                                       P(gy), B, N, M, D, p, eps, lam, P(gv), 1, P(lh),
-                                                       ops._stream(x.device))
-            _lib.check(rc, "b200ot_sinkhorn_final_bwd_small")
-            ops.count_launches(1)
+            ops._call(x.device, "b200ot_sinkhorn_final_bwd_small", x, y, a, b, f_ba, g_ab, f_aa if debias else None,
+                      g_bb if debias else None, lse2, go_f_ba, go_g_ab, go_f_aa, go_g_bb, gx, gy, B, N, M, D, p, eps,
+                      lam, gv, 1, lh, launches=1)
         if need_w:
             terms = work[3 * tot:]
             if ctx.needs_input_grad[2]:
