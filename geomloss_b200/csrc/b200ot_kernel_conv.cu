@@ -12,6 +12,7 @@
 #include "rowsum_launch.cuh"
 #include "tcbwd.cuh"
 #include "tcconv.cuh"
+#include "tcwide.cuh"
 
 #include <stdio.h>
 #include <stdlib.h>
@@ -298,8 +299,10 @@ static TcBwdTuning tc_bwd_tuning() {
 // The plan of a launch group: `ctas` row CTAs, each reading up to `tiles` (>= 1) column tiles.  The split count is
 // chosen for the whole grid and cuts those tiles.  Behind the images: the partials of `rows` rows ((m, s) pairs forward, D+1
 // sums per row backward, D+2 for the p = 1 softmin: `head` sums ahead of the D), then a misc block of misc_bytes.
+// `slices` > 0: the K-slab ring of the kernels above D = 64 (tcwide.cuh), whose row gradients run `slices` CTAs per
+// row tile and split.
 static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, int64_t ctas, int64_t tiles, int64_t rows,
-                           int64_t misc_bytes, int head = 1) {
+                           int64_t misc_bytes, int head = 1, int slices = 0) {
   TcPlan p;
   p.kp = tc_kp(D);
   p.rtpe = p.ctpe = 0;
@@ -307,13 +310,21 @@ static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, in
   p.b_tiles = b_tiles;
   p.ctas = ctas;
   const int64_t b_bytes = tc_b_img_bytes(p.kp, kTcBN);
-  const int64_t bar_bytes = 256;  // mbarriers behind the column ring
-  // the CTA's row image stays in shared memory; the rest of the 227 KB a block may use holds the column ring
-  const int64_t avail = 227 * 1024 - bar_bytes - tc_a_span(p.kp);
-  int64_t ns = avail / b_bytes;
-  p.nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
-  p.smem = tc_a_span(p.kp) + p.nstage * b_bytes + bar_bytes;
-  int64_t want = ceil_div64((int64_t)num_sms() * 4, ctas);
+  if (slices > 0) {
+    // row tail, column tails and slab ring (tcwide.cuh): as many stages as fit, whatever D
+    int ns = kTcMaxStage;
+    while (ns > 0 && tc_wide_smem(ns) > 227 * 1024) --ns;
+    p.nstage = ns;
+    p.smem = tc_wide_smem(ns);
+  } else {
+    const int64_t bar_bytes = 256;  // mbarriers behind the column ring
+    // the CTA's row image stays in shared memory; the rest of the 227 KB a block may use holds the column ring
+    const int64_t avail = 227 * 1024 - bar_bytes - tc_a_span(p.kp);
+    int64_t ns = avail / b_bytes;
+    p.nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
+    p.smem = tc_a_span(p.kp) + p.nstage * b_bytes + bar_bytes;
+  }
+  int64_t want = ceil_div64((int64_t)num_sms() * 4, ctas * std::max(slices, 1));
   const int forced = forced_splits();  // test hook (plan.cuh)
   if (forced > 0) want = forced;
   if (want < 1) want = 1;
@@ -407,10 +418,6 @@ static int tc_pack(const TcPlan& p, unsigned char* base, const TcOperands& o, cu
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
-
-// The parameter list of tc_reduce_kernel and tc_bwd_kernel
-using TcKernel = void (*)(const unsigned char*, const unsigned char*, float*, int64_t, int, int, int, int, int, int,
-                          float, const float*, int, int64_t, const int4*, const int2*, const int*);
 
 // One launch of a reduction or row-gradient kernel over plan p, into the plan's partials: `rows` rows (n_local per
 // batch element; block-sparse problems: seg / pieces / row_src)
@@ -549,6 +556,99 @@ int softmin_l1_bwd_finalize(const float* part, int n_part, const float* x, const
                             float* grad_x, int64_t N, int D, const float* coord_absmax, cudaStream_t st) {
   softmin_l1_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(part, n_part, x, center, grad_out,
                                                                                grad_x, N, D, coord_absmax);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Above D = 64 (tcwide.cuh): the same images, plans and finalize kernels, the K-slab kernels of b200ot_wide.cu.
+// B elements of N rows / M columns (B = 1: one problem).
+// ---------------------------------------------------------------------------------------------------
+static TcPlan make_tc_wide_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B, int head) {
+  const int rtpe = (int)ceil_div64(N, kTcM), ctpe = (int)ceil_div64(M, kTcBN);
+  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4, head,
+                          bwd ? tc_wide_slabs(D) : 1);
+  p.rtpe = rtpe;
+  p.ctpe = ctpe;
+  return p;
+}
+
+int64_t tc_wide_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
+  // the forward and the row gradient (D + 2 sums per row for the p = 1 softmin) split the columns differently
+  return std::max(make_tc_wide_plan(N, M, D, false, B, 1).total, make_tc_wide_plan(N, M, D, true, B, 2).total);
+}
+
+// Pack (with the weight and coordinate maxima asked for) and one wide kernel of MODE over the plan; leaves n_part sets
+// of partials (forward: (m, s) pairs or sums per row; bwd: (B N, D + head) sums) in *part_out.
+static int tc_wide_pass(int mode, bool bwd, const TcOperands& o, int head, int self_mode, float clampq, bool want_wmax,
+                        bool want_cmax, void* scratch, cudaStream_t st, float** part_out, int* n_part_out,
+                        const float** w_absmax_out, const float** coord_absmax_out) {
+  const TcPlan p = make_tc_wide_plan(o.N, o.M, o.D, bwd, o.B, head);
+  if (p.nstage < 1) return B200OT_EINVAL;
+  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
+  const float *w_absmax = nullptr, *coord_absmax = nullptr;
+  int rc = tc_pack(p, base, o, st, want_wmax ? &w_absmax : nullptr, want_cmax ? &coord_absmax : nullptr);
+  if (rc) return rc;
+  const TcKernel kern = tc_wide_kernel(mode, bwd);
+  if (kern == nullptr) return B200OT_EINVAL;
+  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+  const dim3 grid((unsigned)p.ctas, (unsigned)p.n_split, bwd ? (unsigned)tc_wide_slabs(o.D) : 1u);
+  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(base, base + p.off_b, reinterpret_cast<float*>(base + p.off_part),
+                                                 o.B * o.N, p.kp, p.ctpe, p.tiles_per_split, p.nstage, o.D, self_mode,
+                                                 clampq, coord_absmax, p.rtpe, o.N, nullptr, nullptr, nullptr);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  *part_out = reinterpret_cast<float*>(base + p.off_part);
+  *n_part_out = bwd ? p.n_split : p.n_split * kTcParts;
+  if (w_absmax_out) *w_absmax_out = w_absmax;
+  if (coord_absmax_out) *coord_absmax_out = coord_absmax;
+  return B200OT_OK;
+}
+
+// The softmin above D = 64, p = 2 (MODE 1 / 3) or p = 1 (MODE 6 / 7, the energy's coordinates as in softmin_l1_tc).
+// Forward: n_part (m, s) sets for b200ot_softmin_finalize.  bwd (lse2 = the forward's): n_part sets of (B N, D + 1)
+// sums for softmin_bwd_finalize_tc (p = 2), or (B N, D + 2) for softmin_l1_bwd_finalize (p = 1, *coord_absmax_out).
+int softmin_wide_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                    const float* center, const float* lse2, int64_t B, int64_t N, int64_t M, int D, int p, float eps,
+                    void* scratch, float** part_out, int* n_part_out, const float** coord_absmax_out,
+                    cudaStream_t st) {
+  if (p_exponent(p) == 2) {
+    TcOperands o{x, y, center, softmin_coord_scale(2, eps), N, M, D, B, nullptr, h_a, h_b, h_scale_b,
+                 bwd ? lse2 : nullptr};
+    return tc_wide_pass(bwd ? 3 : 1, bwd, o, 1, 0, 0.f, false, false, scratch, st, part_out, n_part_out, nullptr,
+                        nullptr);
+  }
+  TcOperands o{x, y, center, 1.f, N, M, D, B, nullptr, h_a, h_b, h_scale_b, bwd ? lse2 : nullptr};
+  o.l1_c = kLog2e / eps;
+  const int self_mode = (x == y && N == M) ? 1 : 0;  // xx / yy: the diagonal takes d = sqrt(clamp) exactly
+  return tc_wide_pass(bwd ? 7 : 6, bwd, o, bwd ? 2 : 1, self_mode, cost_clamp(p), false, true, scratch, st, part_out,
+                      n_part_out, nullptr, coord_absmax_out);
+}
+
+// The kernel convolutions above D = 64: out (forward) or grad_x (bwd, grad_out given), as conv_fwd_tc / conv_bwd_tc
+static int conv_wide_tc(bool bwd, int kind, const float* x, const float* y, const float* w, const float* center,
+                        const float* grad_out, float* res, int64_t B, int64_t N, int64_t M, int D, float blur,
+                        void* scratch, cudaStream_t st) {
+  const int kb = kind_base(kind);
+  const ConvScales cs = conv_scales(kind, blur);
+  const int mode = kb == B200OT_KERNEL_GAUSSIAN ? (bwd ? 2 : 0) : (kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5);
+  const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
+  float* part = nullptr;
+  int n_part = 0;
+  const float *w_absmax = nullptr, *coord_absmax = nullptr;
+  const int rc = tc_wide_pass(mode, bwd, {x, y, center, cs.scale, N, M, D, B, w}, 1, self_mode, cs.clampq, bwd,
+                              kb == B200OT_KERNEL_ENERGY, scratch, st, &part, &n_part, &w_absmax, &coord_absmax);
+  if (rc) return rc;
+  if (!bwd) {
+    conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
+        part, n_part, kb == B200OT_KERNEL_ENERGY ? -1.f : 1.f, res, B * N, coord_absmax);
+  } else {
+    const float coef = kb == B200OT_KERNEL_GAUSSIAN
+                           ? 1.0f / (cs.scale * blur * blur)
+                           : (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
+    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
+        part, n_part, x, center, grad_out, res, B * N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax, nullptr,
+        coord_absmax, N);
+  }
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
@@ -879,6 +979,74 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float*
   if (!out) return B200OT_EINVAL;
   return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, B, N, M, D, kind, blur, scratch, scratch_bytes,
                          stream, true);
+}
+
+// ---- above D = 64: the K-slab tensor-core kernels (tcwide.cuh), B >= 1 elements ----
+B200OT_API int64_t b200ot_wide_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
+  return tc_wide_dims(B, N, M, D) ? tc_wide_scratch_bytes(N, M, D, B) : 0;
+}
+
+B200OT_API int b200ot_wide_softmin_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
+                                       float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                       float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
+                                       int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                       void* stream) {
+  if (!x || !y || !h_a || !scratch || !tc_wide_dims(B, N, M, D) || !valid_p(p) || !(eps > 0.f) || (!out && !lse2_out))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  const float* coord_absmax = nullptr;
+  const int rc = softmin_wide_tc(false, x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps, scratch, &part,
+                                 &n_part, &coord_absmax, (cudaStream_t)stream);
+  if (rc) return rc;
+  return b200ot_softmin_finalize(part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
+}
+
+B200OT_API int b200ot_wide_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
+                                         float h_scale_b, const float* center, const float* lse2,
+                                         const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                         int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                         void* stream) {
+  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_wide_dims(B, N, M, D) || !valid_p(p) ||
+      !(eps > 0.f))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  float* part = nullptr;
+  int n_part = 0;
+  const float* coord_absmax = nullptr;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = softmin_wide_tc(true, x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps, scratch, &part,
+                                 &n_part, &coord_absmax, st);
+  if (rc) return rc;
+  // P carries kTcPScale (p = 2) or 2^k_i (p = 1), which cancel: both finalizes divide by each row's sum of P
+  if (p_exponent(p) == 1)
+    return softmin_l1_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, coord_absmax, st);
+  return softmin_bwd_finalize_tc(part, n_part, x, center, grad_out, grad_x, B * N, D, eps, st);
+}
+
+B200OT_API int b200ot_wide_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
+                                           float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
+                                           float blur, void* scratch, int64_t scratch_bytes, void* stream) {
+  if (!x || !y || !w || !out || !scratch || !tc_wide_dims(B, N, M, D) || !valid_kind(kind) || !blur_ok(kind, blur))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  return conv_wide_tc(false, kind, x, y, w, center, nullptr, out, B, N, M, D, blur, scratch, (cudaStream_t)stream);
+}
+
+B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, const float* w, const float* center,
+                                             const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                             int32_t D, int32_t kind, float blur, void* scratch,
+                                             int64_t scratch_bytes, void* stream) {
+  if (!x || !y || !w || !grad_out || !grad_x || !scratch || !tc_wide_dims(B, N, M, D) || !valid_kind(kind) ||
+      !blur_ok(kind, blur))
+    return B200OT_EINVAL;
+  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
+  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
+  return conv_wide_tc(true, kind, x, y, w, center, grad_out, grad_x, B, N, M, D, blur, scratch, (cudaStream_t)stream);
 }
 
 }  // extern "C"

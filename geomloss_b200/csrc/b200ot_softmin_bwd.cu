@@ -60,6 +60,14 @@ static int rowsum_merge(const float* part, int n_part, int width, float* merged,
   return B200OT_OK;
 }
 
+int softmin_bwd_finalize_tc(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
+                            float* grad_x, int64_t N, int D, float eps, cudaStream_t st) {
+  softmin_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
+      part, n_part, x, center, grad_out, grad_x, N, D, 2, 1.0f / softmin_coord_scale(2, eps));
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
 template <int MODE, int D>
 static int launch_rowsum(const ReducePlan& pl, cudaStream_t st, const float* x, const float* center, float scale,
                          float clampq, const float* cols, const float* lse2, float* part, int64_t N,

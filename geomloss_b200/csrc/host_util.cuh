@@ -71,6 +71,24 @@ int softmin_l1_tc(bool bwd, const float* x, const float* y, const float* h_a, co
 int softmin_l1_bwd_finalize(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
                             float* grad_x, int64_t N, int D, const float* coord_absmax, cudaStream_t st);
 
+// Above D = 64 (b200ot_wide_*, tcwide.cuh): B >= 1 elements, 64 < D <= B200OT_MAX_D_WIDE
+inline bool tc_wide_dims(int64_t B, int64_t N, int64_t M, int D) {
+  return B >= 1 && N > 0 && M > 0 && D > 64 && D <= B200OT_MAX_D_WIDE;
+}
+int64_t tc_wide_scratch_bytes(int64_t N, int64_t M, int D, int64_t B);
+// The parameter list of tc_reduce_kernel / tc_bwd_kernel and of the wide kernels
+using TcKernel = void (*)(const unsigned char*, const unsigned char*, float*, int64_t, int, int, int, int, int, int,
+                          float, const float*, int, int64_t, const int4*, const int2*, const int*);
+// the wide kernel of a tc_reduce_kernel (bwd = false) or tc_bwd_kernel MODE, null for a mode it does not serve
+// (b200ot_wide.cu)
+TcKernel tc_wide_kernel(int mode, bool bwd);
+int softmin_wide_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                    const float* center, const float* lse2, int64_t B, int64_t N, int64_t M, int D, int p, float eps,
+                    void* scratch, float** part_out, int* n_part_out, const float** coord_absmax_out, cudaStream_t st);
+// grad_x of the N rows from the p = 2 softmin's tensor-core row-gradient sums, (n_part, N, D + 1), any D
+int softmin_bwd_finalize_tc(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
+                            float* grad_x, int64_t N, int D, float eps, cudaStream_t st);
+
 int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
                    float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
                    void* scratch, float** part_out, int* n_part_out, cudaStream_t st, int64_t B = 1,

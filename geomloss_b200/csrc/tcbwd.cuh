@@ -92,6 +92,108 @@ __device__ __forceinline__ float2 tc_l1_pq(float s, float t, float clampq, float
   return make_float2(p, q < t ? 0.f : p * r);
 }
 
+// S -> P of one column tile, packed as the A fragments of GEMM 2 (ph[2 n8 + h] = the pair of row h in 8-column block
+// n8; pl the lo terms when PT = 2), and the tile's contribution to the row sums (sum: P, sumq: Q for MODE 7).  The
+// column slot, tile and rows as for tc_reduce_tile (tcconv.cuh).
+template <int MODE, int PT>
+__device__ __forceinline__ void tc_bwd_tile(float (&s)[64], const TcCta& c, int st, int kp, int k, int64_t row0,
+                                            const float (&tb)[2], const float2 (&rt)[2], float clampq, int self_mode,
+                                            int cq, uint32_t (&ph)[32], uint32_t (&pl)[PT == 2 ? 32 : 1],
+                                            float (&sum)[2], float (&sumq)[2]) {
+  if constexpr (MODE != 3) {
+    if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
+  }
+  float tq[2] = {0.f, 0.f};
+  const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
+  float ts[2] = {0.f, 0.f};
+#pragma unroll
+  for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+    float2 w = make_float2(1.f, 1.f);
+    if constexpr (MODE != 3) w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
+    if constexpr (MODE == 4 || MODE == 5) {
+      w.x *= 1.f / (float)(1 << kTcNormPLog2);
+      w.y *= 1.f / (float)(1 << kTcNormPLog2);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float p0, p1;
+      if constexpr (MODE == 7) {
+        // w = (H_j, H_j+1); ts sums P, tq and GEMM 2 take Q
+        const float2 pq0 = tc_l1_pq(s[4 * n8 + 2 * h], tb[h], clampq, w.x, rt[h]);
+        const float2 pq1 = tc_l1_pq(s[4 * n8 + 2 * h + 1], tb[h], clampq, w.y, rt[h]);
+        ts[h] += pq0.x + pq1.x;
+        p0 = pq0.y;
+        p1 = pq1.y;
+      } else if constexpr (MODE >= 4) {
+        p0 = tc_norm_p<MODE>(s[4 * n8 + 2 * h], tb[h], w.x);
+        p1 = tc_norm_p<MODE>(s[4 * n8 + 2 * h + 1], tb[h], w.y);
+      } else {
+        p0 = ex2_approx(s[4 * n8 + 2 * h]);
+        p1 = ex2_approx(s[4 * n8 + 2 * h + 1]);
+      }
+      if constexpr (MODE == 2) {
+        p0 *= w.x;
+        p1 *= w.y;
+      }
+      const uint32_t hh = pack_f16x2(p0, p1);
+      ph[2 * n8 + h] = hh;
+      const float2 hf = unpack_f16x2(hh);
+      if constexpr (PT == 2) {
+        if constexpr (MODE == 7) {
+          tq[h] += p0 + p1;
+        } else {
+          ts[h] += p0 + p1;
+        }
+        pl[2 * n8 + h] = pack_f16x2(p0 - hf.x, p1 - hf.y);
+      } else {
+        ts[h] += hf.x + hf.y;  // the sums see exactly what GEMM 2 sees
+      }
+    }
+  }
+  sum[0] += ts[0];
+  sum[1] += ts[1];
+  if constexpr (MODE == 7) {
+    sumq[0] += tq[0];
+    sumq[1] += tq[1];
+  }
+}
+
+// Row sums over the quad and gradient sums out: the thread's two rows of [G_a | G_b] (g, DK columns each) are the
+// gradient sums of dimensions d0 .. d0 + DK - 1 (those below D are written); `heads`: also the row sums ahead of them.
+template <int MODE, int DK, bool BATCH, bool BLOCKS>
+__device__ __forceinline__ void tc_bwd_store(float* __restrict__ part, const float (&g)[DK], const float (&sum)[2],
+                                             const float (&sumq)[2], int64_t row0, int split, int elem, int rtpe,
+                                             int64_t n_local, const int* __restrict__ row_src, int64_t N, int D,
+                                             int d0, bool heads, int cq) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float tot = sum[h];
+    tot += __shfl_xor_sync(0xffffffffu, tot, 1);
+    tot += __shfl_xor_sync(0xffffffffu, tot, 2);
+    float totq = 0.f;
+    if constexpr (MODE == 7) {
+      totq = sumq[h];
+      totq += __shfl_xor_sync(0xffffffffu, totq, 1);
+      totq += __shfl_xor_sync(0xffffffffu, totq, 2);
+    }
+    constexpr int kHead = MODE == 7 ? 2 : 1;  // row sums ahead of the D gradient sums
+    const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, elem, rtpe, n_local, row_src, N);
+    if (row < N) {
+      float* dst = part + ((int64_t)split * N + row) * (D + kHead);
+      if (cq == 0 && heads) dst[0] = tot;
+      if constexpr (MODE == 7) {
+        if (cq == 0 && heads) dst[1] = totq;
+      }
+#pragma unroll
+      for (int j = 0; j < DK / 2; ++j) {
+        if (((j >> 1) & 1) != h) continue;
+        const int c = d0 + 8 * (j >> 2) + cq + (j & 1);
+        if (c < D) dst[kHead + c] = g[j] + g[j + DK / 2];
+      }
+    }
+  }
+}
+
 // BATCH: B problems side by side, laid out and mapped to rows and column tiles as in tc_reduce_kernel (tcconv.cuh).
 // BLOCKS: block-sparse softmin (MODE 3), segments, pieces and row_src as in tc_reduce_kernel; a split without a tile
 // writes zero sums.
@@ -145,64 +247,8 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     tc_exponent_gemm(s, a_addr, b_addr, DK / 8);
     wgmma_wait<0>();
     reg_fence(s);
-    if constexpr (MODE != 3) {
-      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
-    }
-    float tq[2] = {0.f, 0.f};
-    // ---- S -> P, packed as the A fragments of GEMM 2 (ph[2 n8 + h] = the pair of row h in 8-column block n8) ----
-    const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
     uint32_t ph[32], pl[PT == 2 ? 32 : 1];
-    float ts[2] = {0.f, 0.f};
-#pragma unroll
-    for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
-      float2 w = make_float2(1.f, 1.f);
-      if constexpr (MODE != 3) w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
-      if constexpr (MODE == 4 || MODE == 5) {
-        w.x *= 1.f / (float)(1 << kTcNormPLog2);
-        w.y *= 1.f / (float)(1 << kTcNormPLog2);
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float p0, p1;
-        if constexpr (MODE == 7) {
-          // w = (H_j, H_j+1); ts sums P, tq and GEMM 2 take Q
-          const float2 pq0 = tc_l1_pq(s[4 * n8 + 2 * h], tb[h], clampq, w.x, rt[h]);
-          const float2 pq1 = tc_l1_pq(s[4 * n8 + 2 * h + 1], tb[h], clampq, w.y, rt[h]);
-          ts[h] += pq0.x + pq1.x;
-          p0 = pq0.y;
-          p1 = pq1.y;
-        } else if constexpr (MODE >= 4) {
-          p0 = tc_norm_p<MODE>(s[4 * n8 + 2 * h], tb[h], w.x);
-          p1 = tc_norm_p<MODE>(s[4 * n8 + 2 * h + 1], tb[h], w.y);
-        } else {
-          p0 = ex2_approx(s[4 * n8 + 2 * h]);
-          p1 = ex2_approx(s[4 * n8 + 2 * h + 1]);
-        }
-        if constexpr (MODE == 2) {
-          p0 *= w.x;
-          p1 *= w.y;
-        }
-        const uint32_t hh = pack_f16x2(p0, p1);
-        ph[2 * n8 + h] = hh;
-        const float2 hf = unpack_f16x2(hh);
-        if constexpr (PT == 2) {
-          if constexpr (MODE == 7) {
-            tq[h] += p0 + p1;
-          } else {
-            ts[h] += p0 + p1;
-          }
-          pl[2 * n8 + h] = pack_f16x2(p0 - hf.x, p1 - hf.y);
-        } else {
-          ts[h] += hf.x + hf.y;  // the sums see exactly what GEMM 2 sees
-        }
-      }
-    }
-    sum[0] += ts[0];
-    sum[1] += ts[1];
-    if constexpr (MODE == 7) {
-      sumq[0] += tq[0];
-      sumq[1] += tq[1];
-    }
+    tc_bwd_tile<MODE, PT>(s, c, st, kp, k, row0, tb, rt, clampq, self_mode, cq, ph, pl, sum, sumq);
     // ---- GEMM 2: G += P . Y, K = the 128 columns of the tile, 16 per instruction ----
     wgmma_fence();
 #pragma unroll
@@ -223,34 +269,8 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     __syncwarp();
     if (lane == 0) mbar_arrive(&c.empty_b[st]);  // the column tile may be overwritten
   }
-  // ---- row sums over the quad, gradient sums out ----
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float tot = sum[h];
-    tot += __shfl_xor_sync(0xffffffffu, tot, 1);
-    tot += __shfl_xor_sync(0xffffffffu, tot, 2);
-    float totq = 0.f;
-    if constexpr (MODE == 7) {
-      totq = sumq[h];
-      totq += __shfl_xor_sync(0xffffffffu, totq, 1);
-      totq += __shfl_xor_sync(0xffffffffu, totq, 2);
-    }
-    constexpr int kHead = MODE == 7 ? 2 : 1;  // row sums ahead of the D gradient sums
-    const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, c.elem, rtpe, n_local, row_src, N);
-    if (row < N) {
-      float* dst = part + ((int64_t)c.split * N + row) * (D + kHead);
-      if (cq == 0) dst[0] = tot;
-      if constexpr (MODE == 7) {
-        if (cq == 0) dst[1] = totq;
-      }
-#pragma unroll
-      for (int j = 0; j < DK / 2; ++j) {
-        if (((j >> 1) & 1) != h) continue;
-        const int c = 8 * (j >> 2) + cq + (j & 1);
-        if (c < D) dst[kHead + c] = g[j] + g[j + DK / 2];
-      }
-    }
-  }
+  tc_bwd_store<MODE, DK, BATCH, BLOCKS>(part, g, sum, sumq, row0, c.split, c.elem, rtpe, n_local, row_src, N, D, 0,
+                                        true, cq);
 }
 
 }  // namespace b200ot

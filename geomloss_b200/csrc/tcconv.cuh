@@ -450,6 +450,94 @@ __device__ __forceinline__ int64_t tc_out_row(int64_t row, int elem, int rtpe, i
   return row;
 }
 
+// The epilogue of tc_reduce_kernel on one column tile: the exponents s of the thread's two rows (row0 and row0 + 8)
+// against the tile, turned into MODE's row sums (acc: MODE 0 / 4 / 5; the running (m, srun): MODE 1 / 6).  `wts` is
+// the fp32 column slot of ring stage `st` (weights, or H_j for MODE 6) behind a column image of K extent kp; k is the
+// CTA's column tile, row0 the thread's first row.
+template <int MODE>
+__device__ __forceinline__ void tc_reduce_tile(float (&s)[64], const TcCta& c, int st, int kp, int k, int64_t row0,
+                                               const float (&tb)[2], const float2 (&rt)[2], float clampq,
+                                               int self_mode, int cq, float (&acc)[2], float (&m)[2],
+                                               float (&srun)[2]) {
+  if constexpr (MODE == 6) {
+    // the p = 1 exponent t = H_j - c d_ij in place of s, then the softmin's log-sum-exp below
+    if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
+    const float* hs = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
+#pragma unroll
+    for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+      const float2 hj = *reinterpret_cast<const float2*>(hs + 8 * n8 + cq);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        s[4 * n8 + 2 * h] = fmaf(-rt[h].x, tc_pair_value<5>(s[4 * n8 + 2 * h], tb[h], clampq), hj.x);
+        s[4 * n8 + 2 * h + 1] = fmaf(-rt[h].x, tc_pair_value<5>(s[4 * n8 + 2 * h + 1], tb[h], clampq), hj.y);
+      }
+    }
+  }
+  if constexpr (MODE != 1 && MODE != 6) {
+    if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
+    const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
+    float ts[2] = {0.f, 0.f};
+#pragma unroll
+    for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+      const float2 w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        ts[h] = fmaf(tc_pair_value<MODE>(s[4 * n8 + 2 * h], tb[h], clampq), w.x, ts[h]);
+        ts[h] = fmaf(tc_pair_value<MODE>(s[4 * n8 + 2 * h + 1], tb[h], clampq), w.y, ts[h]);
+      }
+    }
+    acc[0] += ts[0];
+    acc[1] += ts[1];
+  } else {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // the 32 exponents of row h in this tile: s[4 n8 + 2 h + e]
+      float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+      for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+        cs0 += ex2_approx(s[4 * n8 + 2 * h] - m[h]);
+        cs1 += ex2_approx(s[4 * n8 + 2 * h + 1] - m[h]);
+      }
+      if (!(cs0 + cs1 <= 1.8446744e19f)) {
+        // outdated max (a term above 2^64 or an overflow): rebase on this chunk's max and redo it
+        float cm = s[2 * h];
+#pragma unroll
+        for (int n8 = 0; n8 < kTcBN / 8; ++n8) cm = fmax3(cm, s[4 * n8 + 2 * h], s[4 * n8 + 2 * h + 1]);
+        srun[h] *= ex2_approx(m[h] - cm);
+        m[h] = cm;
+        cs0 = 0.f;
+        cs1 = 0.f;
+#pragma unroll
+        for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
+          cs0 += ex2_approx(s[4 * n8 + 2 * h] - m[h]);
+          cs1 += ex2_approx(s[4 * n8 + 2 * h + 1] - m[h]);
+        }
+      }
+      srun[h] += cs0 + cs1;
+    }
+  }
+}
+
+// The partials of tc_reduce_kernel's two rows of the thread (layout below)
+template <int MODE, bool BATCH, bool BLOCKS>
+__device__ __forceinline__ void tc_reduce_store(float* __restrict__ part, const float (&acc)[2], const float (&m)[2],
+                                                const float (&srun)[2], int64_t row0, int split, int elem, int rtpe,
+                                                int64_t n_local, const int* __restrict__ row_src, int64_t N,
+                                                int lane) {
+  const int q = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, elem, rtpe, n_local, row_src, N);
+    if (row < N) {
+      if constexpr (MODE != 1 && MODE != 6) {
+        part[((int64_t)split * kTcParts + q) * N + row] = acc[h];
+      } else {
+        reinterpret_cast<float2*>(part)[((int64_t)split * kTcParts + q) * N + row] = make_float2(m[h], srun[h]);
+      }
+    }
+  }
+}
+
 // MODE 0: gaussian kernel conv  part[(split*kTcParts + q)*N + row]   = sum_j w_j 2^S_ij
 // MODE 1: softmin               part2[(split*kTcParts + q)*N + row]  = (m, s) with sum_j 2^S_ij = s 2^m  (lazy max,
 //         sum-guarded exactly like softmin.cuh; same partial format as softmin_partial_kernel)
@@ -510,78 +598,11 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     tc_exponent_gemm(s, a_addr, smem_u32(c.sb + st * c.b_bytes), seg);
     wgmma_wait<0>();
     reg_fence(s);
-    if constexpr (MODE == 6) {
-      // the p = 1 exponent t = H_j - c d_ij in place of s, then the softmin's log-sum-exp below
-      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
-      const float* hs = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
-#pragma unroll
-      for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
-        const float2 hj = *reinterpret_cast<const float2*>(hs + 8 * n8 + cq);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          s[4 * n8 + 2 * h] = fmaf(-rt[h].x, tc_pair_value<5>(s[4 * n8 + 2 * h], tb[h], clampq), hj.x);
-          s[4 * n8 + 2 * h + 1] = fmaf(-rt[h].x, tc_pair_value<5>(s[4 * n8 + 2 * h + 1], tb[h], clampq), hj.y);
-        }
-      }
-    }
-    if constexpr (MODE != 1 && MODE != 6) {
-      if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
-      const float* wts = reinterpret_cast<const float*>(c.sb + st * c.b_bytes + kTcBN * kp * 2);
-      float ts[2] = {0.f, 0.f};
-#pragma unroll
-      for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
-        const float2 w = *reinterpret_cast<const float2*>(wts + 8 * n8 + cq);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          ts[h] = fmaf(tc_pair_value<MODE>(s[4 * n8 + 2 * h], tb[h], clampq), w.x, ts[h]);
-          ts[h] = fmaf(tc_pair_value<MODE>(s[4 * n8 + 2 * h + 1], tb[h], clampq), w.y, ts[h]);
-        }
-      }
-      acc[0] += ts[0];
-      acc[1] += ts[1];
-    } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        // the 32 exponents of row h in this tile: s[4 n8 + 2 h + e]
-        float cs0 = 0.f, cs1 = 0.f;
-#pragma unroll
-        for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
-          cs0 += ex2_approx(s[4 * n8 + 2 * h] - m[h]);
-          cs1 += ex2_approx(s[4 * n8 + 2 * h + 1] - m[h]);
-        }
-        if (!(cs0 + cs1 <= 1.8446744e19f)) {
-          // outdated max (a term above 2^64 or an overflow): rebase on this chunk's max and redo it
-          float cm = s[2 * h];
-#pragma unroll
-          for (int n8 = 0; n8 < kTcBN / 8; ++n8) cm = fmax3(cm, s[4 * n8 + 2 * h], s[4 * n8 + 2 * h + 1]);
-          srun[h] *= ex2_approx(m[h] - cm);
-          m[h] = cm;
-          cs0 = 0.f;
-          cs1 = 0.f;
-#pragma unroll
-          for (int n8 = 0; n8 < kTcBN / 8; ++n8) {
-            cs0 += ex2_approx(s[4 * n8 + 2 * h] - m[h]);
-            cs1 += ex2_approx(s[4 * n8 + 2 * h + 1] - m[h]);
-          }
-        }
-        srun[h] += cs0 + cs1;
-      }
-    }
+    tc_reduce_tile<MODE>(s, c, st, kp, k, row0, tb, rt, clampq, self_mode, cq, acc, m, srun);
     __syncwarp();
     if (lane == 0) mbar_arrive(&c.empty_b[st]);
   }
-  const int q = lane & 3;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int64_t row = tc_out_row<BATCH, BLOCKS>(row0 + 8 * h, c.elem, rtpe, n_local, row_src, N);
-    if (row < N) {
-      if constexpr (MODE != 1 && MODE != 6) {
-        part[((int64_t)c.split * kTcParts + q) * N + row] = acc[h];
-      } else {
-        reinterpret_cast<float2*>(part)[((int64_t)c.split * kTcParts + q) * N + row] = make_float2(m[h], srun[h]);
-      }
-    }
-  }
+  tc_reduce_store<MODE, BATCH, BLOCKS>(part, acc, m, srun, row0, c.split, c.elem, rtpe, n_local, row_src, N, lane);
 }
 
 }  // namespace b200ot

@@ -25,16 +25,16 @@ def kernel_points(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=Non
     """1/2 |a - b|_k^2 for unbatched a:(N,) x:(N,D) b:(M,) y:(M,D).        kernel_samples.py:92-146
 
     ``conv(kind, x, y, w, blur, center=)`` defaults to the single-GPU kernel; distributed.py injects the
-    column-sharded one.  ``keops``: the reference's use_keops=True convention (backend "online" / "multiscale"):
-    laplacian and energy take sqrt(|x-y|^2) without the 1e-8 clamp of the tensorized `distances`
-    (utils.py:56-61 vs kernel_samples.py:71-82)."""
+    column-sharded one; above D = 64 the default is the wide tensor-core kernel (ops.kernel_conv_wide).  ``keops``:
+    the reference's use_keops=True convention (backend "online" / "multiscale"): laplacian and energy take
+    sqrt(|x-y|^2) without the 1e-8 clamp of the tensorized `distances` (utils.py:56-61 vs kernel_samples.py:71-82)."""
     if kernel is not None:
         raise NotImplementedError("user-supplied kernel callables are outside the CUDA hot path")
     if name not in ops.KERNEL_KINDS:
         # the reference maps loss="hausdorff" to kernel_loss(name=None) and dies with KeyError(None)
         # (samples_loss.py:22-26, kernel_samples.py:107-108): keep the error type, say why.
         raise KeyError(name)
-    conv = conv or ops.kernel_conv
+    conv = conv or (ops.kernel_conv_wide if x.shape[-1] > ops.MAX_D_TC else ops.kernel_conv)
     if keops:
         name = ops.KERNEL_KINDS[name] | ops.KERNEL_UNCLAMPED
     dg = _TwiceGrad.apply
@@ -51,7 +51,8 @@ def kernel_points(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=Non
 def kernel_points_batched(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=None, keops=False, **_ignored):
     """Batched kernel norms a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D): the three (four) matvecs take one launch group each
     for the whole batch — for D <= 8 ranges-mode reductions over the block-diagonal stacked problem, for 8 < D <= 64
-    the batched tensor-core operators (ops.kernel_conv_batched).
+    the batched tensor-core operators (ops.kernel_conv_batched), for 64 < D <= 1024 the wide ones
+    (ops.kernel_conv_wide).
     Reference: kernel_loss on (B, ...) inputs (kernel_samples.py:92-146)."""
     from . import ranges
 
@@ -67,7 +68,7 @@ def kernel_points_batched(a, x, b, y, name=None, blur=0.05, potentials=False, ke
     center = ops.default_center(xf.detach(), yf.detach())
     dg = _TwiceGrad.apply
     if D > ops.MAX_D:
-        cv = ops.kernel_conv_batched
+        cv = ops.kernel_conv_wide if D > ops.MAX_D_TC else ops.kernel_conv_batched
         a_x = cv(kid, dg(x), x.detach(), a.detach(), blur, center=center)
         b_y = cv(kid, dg(y), y.detach(), b.detach(), blur, center=center)
         b_x = cv(kid, x, y, b, blur, center=center)

@@ -551,3 +551,123 @@ def softmin_l1_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=1,
 def softmin_l1(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, scale_out=1.0):
     """Differentiable (w.r.t. x) ``scale_out * softmin_l1_raw(...)``, for (N,D) or (B,N,D) clouds."""
     return _softmin_apply(softmin_l1_raw, softmin_l1_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)
+
+
+# ------------------------------------------------------------------------------------------------
+# above D = 64 (64 < D <= MAX_D_WIDE): the p = 2 and p = 1 softmins and the three kernel convolutions on the K-slab
+# tensor-core kernels (csrc/tcwide.cuh, b200ot_wide_*), one problem (N,D) / (M,D) or a batch (B,N,D) / (B,M,D) in one
+# launch group per call.  Same contracts as the one-problem and batched operators above.
+# ------------------------------------------------------------------------------------------------
+MAX_D_WIDE = 1024  # B200OT_MAX_D_WIDE
+
+
+def _wide_args(x, y):
+    """(batched, (B, N, M, D)) of (N,D) / (M,D) or (B,N,D) / (B,M,D) clouds in the wide dimensions."""
+    batched = not (x.dim() == 2 and y.dim() == 2)
+    xb, yb = (x, y) if batched else (x.unsqueeze(0), y.unsqueeze(0))
+    if xb.dim() != 3 or yb.dim() != 3 or xb.shape[0] != yb.shape[0] or xb.shape[2] != yb.shape[2]:
+        raise ValueError(f"expected x:(N,D), y:(M,D) or x:(B,N,D), y:(B,M,D); got {tuple(x.shape)}, {tuple(y.shape)}")
+    B, N, D = xb.shape
+    M = yb.shape[1]
+    if B == 0 or N == 0 or M == 0:
+        raise ValueError("empty batch or point cloud")
+    if not MAX_D_TC < D <= MAX_D_WIDE:
+        raise NotImplementedError(f"the wide tensor-core operators serve {MAX_D_TC} < D <= {MAX_D_WIDE}, got D = {D} "
+                                  f"(no kernel of this build reduces clouds above D = {MAX_D_WIDE})")
+    if x.device != y.device:
+        raise ValueError("x and y must be on the same device")
+    return batched, (B, N, M, D)
+
+
+def _wide_scratch(B, N, M, D, dev):
+    return _scratch(_query(dev, "b200ot_wide_scratch_bytes", B, N, M, D), dev, "wide")
+
+
+def softmin_wide_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, out_old=None, alpha_old=0.0,
+                     beta=1.0, out=None, want_lse2=False):
+    """``softmin_raw`` above D = 64 for p = 1 or 2 (| P_UNCLAMPED): out <- alpha_old*out_old + beta*softmin(eps, (x, y),
+    h), (N,) for (N,D) clouds, (B,N) for (B,N,D) ones.  No autograd.  Returns ``(out, lse2 | None)``."""
+    batched, (B, N, M, D) = _wide_args(x, y)
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
+    _per_point(h_a, B * M, "h_a")
+    _per_point(h_b, B * M, "h_b")
+    _per_point(out_old, B * N, "out_old")
+    shape = (B, N) if batched else (N,)
+    dev = x.device
+    with nvtx_range(f"b200ot.softmin_wide B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=dev)
+        lse2 = torch.empty(shape, dtype=torch.float32, device=dev) if want_lse2 else None
+        scratch = _wide_scratch(B, N, M, D, dev)
+        # two packs, reduction, finalize (p = 1: and the coordinate maximum)
+        _call(dev, "b200ot_wide_softmin_fwd", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
+              float(beta), out, lse2, B, N, M, D, int(p), float(eps), scratch, scratch.numel(),
+              launches=5 if (p & 0xFF) == 1 else 4)
+    return out, lse2
+
+
+def softmin_wide_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None):
+    """grad_x, shaped like x, of <grad_out, softmin_wide(eps, x, y, h)> with y, h constant
+    (b200ot_wide_softmin_bwd_x)."""
+    _, (B, N, M, D) = _wide_args(x, y)
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
+    _per_point(grad_out, B * N, "grad_out")
+    _per_point(lse2, B * N, "lse2")
+    dev = x.device
+    gx = torch.empty_like(x)
+    scratch = _wide_scratch(B, N, M, D, dev)
+    _call(dev, "b200ot_wide_softmin_bwd_x", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, B, N, M, D,
+          int(p), float(eps), scratch, scratch.numel(), launches=5 if (p & 0xFF) == 1 else 4)
+    return gx
+
+
+def softmin_wide(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
+    """Differentiable (w.r.t. x) ``scale_out * softmin_wide_raw(...)``, for (N,D) or (B,N,D) clouds."""
+    return _softmin_apply(softmin_wide_raw, softmin_wide_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center,
+                          scale_out)
+
+
+def _conv_wide_args(x, y, w, center):
+    batched, (B, N, M, D) = _wide_args(x, y)  # the shape check first: D > MAX_D_WIDE is refused on any device
+    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
+    _per_point(w, B * M, "w")
+    return x, y, w, center, batched, B, N, M, D
+
+
+def kernel_conv_wide_raw(kind, x, y, w, blur, *, center=None):
+    """out_i = sum_j k(x_i, y_j) w_j above D = 64, (N,) or (B,N); no autograd."""
+    x, y, w, center, batched, B, N, M, D = _conv_wide_args(x, y, w, center)
+    dev = x.device
+    energy = (kind_id(kind) & 0xFF) == KERNEL_KINDS["energy"]
+    with nvtx_range(f"b200ot.kernel_conv_wide kind={kind} B={B} N={N} M={M} D={D}"):
+        out = torch.empty((B, N) if batched else (N,), dtype=torch.float32, device=dev)
+        scratch = _wide_scratch(B, N, M, D, dev)
+        # two packs, reduction, finalize (energy: and the coordinate maximum)
+        _call(dev, "b200ot_wide_kernel_conv_fwd", x, y, w, center, out, B, N, M, D, kind_id(kind), float(blur), scratch,
+              scratch.numel(), launches=5 if energy else 4)
+    return out
+
+
+def kernel_conv_wide_grad_rows(kind, x, y, w, blur, grad_out, *, center=None):
+    """grad_x, shaped like x, of <grad_out, kernel_conv_wide_raw(kind, x, y, w, blur)>
+    (b200ot_wide_kernel_conv_bwd_x)."""
+    x, y, w, center, _, B, N, M, D = _conv_wide_args(x, y, w, center)
+    grad_out = _f32c(grad_out, "grad_out")
+    _per_point(grad_out, B * N, "grad_out")
+    dev = x.device
+    energy = (kind_id(kind) & 0xFF) == KERNEL_KINDS["energy"]
+    gx = torch.empty_like(x)
+    scratch = _wide_scratch(B, N, M, D, dev)
+    # weight maximum, two packs, reduction, finalize (energy: and the coordinate maximum)
+    _call(dev, "b200ot_wide_kernel_conv_bwd_x", x, y, w, center, grad_out, gx, B, N, M, D, kind_id(kind), float(blur),
+          scratch, scratch.numel(), launches=6 if energy else 5)
+    return gx
+
+
+def kernel_conv_wide(kind, x, y, w, blur, *, center=None):
+    """out = K(x, y) @ w above D = 64, (N,) or (B,N), differentiable w.r.t. x, y and w (no one-pass value + gradient:
+    the forward and the row gradient are separate launches)."""
+    wide = _ConvOps(kernel_conv_wide_raw, kernel_conv_wide_grad_rows, None)
+    return _KernelConv.apply(wide, wide, x, y, w, kind, blur, center, False)

@@ -23,7 +23,10 @@ The Sinkhorn loss with p = 1 above D = 8 runs on the tensor-core p = 1 softmin (
 both cost conventions; column-sharded multi-GPU engines have no such operator and raise NotImplementedError there.
 Batched inputs (B, N, D) run as ONE launch group per reduction for the whole batch: a block-diagonal ranges problem
 for D <= 8 (ranges.py), the batched tensor-core operators for 8 < D <= 64 (ops.softmin_batched, ops.softmin_l1,
-kernel_conv_batched).  Column-sharded multi-GPU engines solve the batch element by element.
+kernel_conv_batched) and the wide ones for 64 < D <= 1024 (ops.softmin_wide, kernel_conv_wide).  Column-sharded
+multi-GPU engines solve the batch element by element.
+Above D = 64 every loss runs on the wide tensor-core operators (K-slab kernels, DESIGN.md section 3.5d), up to
+D = 1024; above that, and for labelled two-scale calls or column-sharded engines above D = 64, NotImplementedError.
 Inputs must be float32 CUDA tensors: there is no CPU path.
 """
 from __future__ import annotations
@@ -35,7 +38,7 @@ import warnings
 
 from .kernel_loss import kernel_points, kernel_points_batched
 from .multiscale import kernel_multiscale, sinkhorn_multiscale
-from .ops import MAX_D, MAX_D_TC
+from .ops import MAX_D, MAX_D_TC, MAX_D_WIDE
 from . import kernel_small, sinkhorn_small
 from .sinkhorn import sinkhorn_points, sinkhorn_points_batched
 
@@ -138,6 +141,13 @@ class SamplesLoss(Module):
         # user labels above D = 3 (the voxel grid stops there): the two-scale Sinkhorn on one GPU, up to D = 64
         labelled = (l_x is not None and l_y is not None and D <= MAX_D_TC and not self._engine
                     and self._multiscale_engine is None)
+        if backend == "multiscale" and self.loss == "sinkhorn" and l_x is not None and l_y is not None and D > MAX_D_TC:
+            # no block-sparse kernel above D = 64: refuse rather than return the single-scale value
+            raise NotImplementedError(f"the labelled two-scale Sinkhorn serves D <= {MAX_D_TC}, got D = {D} (the "
+                                      f"single-scale backends 'tensorized' / 'online' serve D <= {MAX_D_WIDE})")
+        if self._engine and D > MAX_D_TC:
+            raise NotImplementedError(f"column-sharded engines serve D <= {MAX_D_TC}, got D = {D} (one GPU serves "
+                                      f"D <= {MAX_D_WIDE})")
         if backend == "multiscale" and self.loss == "sinkhorn" and (D <= 3 or labelled):
             # single problem (B == 0, or B == 1 squeezed like the reference does, samples_loss.py:249-251)
             sq = (lambda t: t[0]) if B == 1 else (lambda t: t)
@@ -181,7 +191,7 @@ class SamplesLoss(Module):
             from .sinkhorn import max_diameter
 
             kw["diameter"] = max_diameter(x.reshape(-1, D), y.reshape(-1, D))
-        one_group = D <= MAX_D or (D <= MAX_D_TC and N * M <= BATCHED_TC_MAX_PAIRS)
+        one_group = D <= MAX_D or (D <= MAX_D_WIDE and N * M <= BATCHED_TC_MAX_PAIRS)
         if B > 1 and one_group and not self._engine and self.loss != "hausdorff":
             # the whole batch in one launch group per reduction (D <= 8: block-diagonal ranges problem; above: the
             # batched tensor-core operators)

@@ -276,6 +276,36 @@ B200OT_API int b200ot_softmin_l1_bwd_x(const float* x, const float* y, const flo
                                        void* scratch, int64_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Above D = 64 (64 < D <= B200OT_MAX_D_WIDE): the p = 2 and p = 1 softmins and the three kernel convolutions,
+ * forward and row gradient, on tensor-core kernels that stream the coordinates in 64-dimension slabs.  Batched layout,
+ * arguments and results as the batched entries above (B = 1: one problem): the softmin entries take those of
+ * b200ot_softmin_l1_* with p = 1 or 2 (| B200OT_P_UNCLAMPED), the convolutions those of b200ot_kernel_conv_*_batched
+ * (kind | B200OT_KERNEL_UNCLAMPED).  EINVAL (before any launch) for null pointers, B < 1, N or M <= 0, D <= 64 or
+ * D > B200OT_MAX_D_WIDE, a bad p or kind, eps <= 0, blur <= 0 (gaussian, laplacian); EALIGN for a misaligned
+ * scratch; ESCRATCH below b200ot_wide_scratch_bytes(B, N, M, D) (0 for a shape these entries refuse), one size for
+ * every entry of the family.
+ * ------------------------------------------------------------------------------------------- */
+#define B200OT_MAX_D_WIDE 1024
+B200OT_API int64_t b200ot_wide_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D);
+B200OT_API int b200ot_wide_softmin_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
+                                       float h_scale_b, const float* center, const float* out_old, float alpha_old,
+                                       float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
+                                       int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                       void* stream);
+B200OT_API int b200ot_wide_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
+                                         float h_scale_b, const float* center, const float* lse2,
+                                         const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                         int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                         void* stream);
+B200OT_API int b200ot_wide_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
+                                           float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
+                                           float blur, void* scratch, int64_t scratch_bytes, void* stream);
+B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, const float* w, const float* center,
+                                             const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
+                                             int32_t D, int32_t kind, float blur, void* scratch,
+                                             int64_t scratch_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Block-sparse softmins in the tensor-core dimensions (8 < D <= 64, p = 2 or 2 | B200OT_P_UNCLAMPED): the fine phase
  * of the two-scale Sinkhorn with user cluster labels (sinkhorn_multiscale, sinkhorn_samples.py:547-681), the
  * counterpart of the ranges entries above, which serve D <= B200OT_MAX_D.  A separate family with its own layout:

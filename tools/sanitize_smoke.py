@@ -30,7 +30,8 @@ def check(name, got, ref, tol=2e-5):
     assert err < tol, name
 
 
-which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "blocks", "grid", "loss", "small"}
+which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "wide", "blocks", "grid", "loss",
+                              "small"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -169,6 +170,29 @@ if "l1" in which:
         prob = torch.softmax(h.double()[:, None, :] - dist / 0.5, dim=2)
         unit = (x.double()[:, :, None, :] - y.double()[:, None, :, :]) / dist[..., None]
         check(f"l1_softmin_grad_d{d}", gx, (prob[..., None] * unit).sum(2), 1e-4)
+if "wide" in which:
+    # above D = 64 (tc_wide_reduce_kernel / tc_wide_bwd_kernel, csrc/tcwide.cuh): one launch of every b200ot_wide_*
+    # entry, a batch of 2 at a partial last slab (D = 72) and at two slabs (D = 128)
+    B, n = 2, 300
+    for d in (72, 128):
+        x, y, h = torch.rand(B, n, d, generator=g), torch.rand(B, n, d, generator=g), torch.randn(B, n, generator=g)
+        w = torch.rand(B, n, generator=g)
+        xd, yd, hd, wd, ones = x.to(DEV), y.to(DEV), h.to(DEV), w.to(DEV), torch.ones(B, n, device=DEV)
+        center = ops.default_center(xd.view(-1, d), yd.view(-1, d))
+        d2 = ((x[:, :, None, :].double() - y[:, None, :, :].double()) ** 2).sum(-1)
+        for p in (1, 2):
+            C = d2 / 2 if p == 2 else d2.clamp_min(1e-8).sqrt()
+            out, lse2 = ops.softmin_wide_raw(0.5, xd, yd, hd, p=p, center=center, want_lse2=True)
+            ref = -0.5 * torch.logsumexp(h.double()[:, None, :] - C / 0.5, dim=2)
+            check(f"wide_softmin_p{p}_d{d}", out, ref.float(), 1e-4)
+            gx = ops.softmin_wide_grad_rows(0.5, xd, yd, hd, None, 0.0, lse2, ones, p=p, center=center)
+            assert torch.isfinite(gx).all()
+        for kind in ("gaussian", "energy"):
+            val = ops.kernel_conv_wide_raw(kind, xd, yd, wd, 2.0, center=center)
+            K = (-d2 / 8.0).exp() if kind == "gaussian" else -d2.clamp_min(1e-8).sqrt()
+            check(f"wide_conv_{kind}_d{d}", val, (K @ w.double()[:, :, None])[..., 0], 1e-4)
+            gx = ops.kernel_conv_wide_grad_rows(kind, xd, yd, wd, 2.0, ones, center=center)
+            assert torch.isfinite(gx).all()
 if "blocks" in which:
     # the block-sparse tensor-core softmins (tc_reduce_kernel<1, false, BLOCKS>, tc_bwd_kernel<3, 2, true, dk, false,
     # BLOCKS>): clusters of 1, 127, 128, 129 and 300 points, a row cluster that keeps nothing, a self problem
