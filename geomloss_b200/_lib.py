@@ -30,6 +30,9 @@ _SIGNATURES = {
                                      c_int32, c_int32, c_float, _P, c_int64, _P]),
     "b200ot_softmin_bwd_x": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32,
                                        c_float, _P, c_int64, _P]),
+    "b200ot_plan_apply_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32, c_int64]),
+    "b200ot_plan_apply": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, _P, _P, _P, c_int64, c_int64, c_int32, c_int64,
+                                    c_int32, c_float, _P, c_int64, _P]),
     "b200ot_packed_cols_floats": (c_int64, [c_int64, c_int32, c_int32]),
     "b200ot_softmin_pack": (c_int32, [_P, _P, _P, c_float, _P, c_int64, c_int32, c_int32, c_float, _P, _P]),
     "b200ot_softmin_num_splits": (c_int32, [c_int64, c_int64, c_int32]),

@@ -10,6 +10,7 @@
 #include "plan.cuh"
 #include "rowsum.cuh"
 #include "rowsum_launch.cuh"
+#include "tcapply.cuh"
 #include "tcbwd.cuh"
 #include "tcconv.cuh"
 #include "tcwide.cuh"
@@ -500,6 +501,79 @@ int softmin_partial_tc(const float* x, const float* y, const float* h_a, const f
   if (rc) return rc;
   *part_out = reinterpret_cast<float*>(base + p.off_part);
   *n_part_out = p.n_split * kTcParts;
+  return B200OT_OK;
+}
+
+// The plan applied to a value matrix (tcapply.cuh): the images and splits of the softmin row gradient's plan, and
+// behind the images the partials (n_split, N, 1 + min(K, 64)), one slab's value image and the K column maxima of V.
+// V wider than 64 columns runs in slabs of 64 (the last one padded to a multiple of 16), each a pass of its own over
+// the pairs through the same partials and value image.  A ring stage holds a column tile and the slab's value image:
+// at dk = 64 and 64 value columns 36.5 + 32 KB, two stages next to the 36 KB row image.
+struct TcApplyPlan {
+  TcPlan p;
+  int64_t off_v, off_vmax, total;
+};
+static int tc_apply_dkv(int K, int k0) { return tc_dk(std::min(64, K - k0)); }
+static void tc_apply_stages(int kp, int dkv, int* nstage, int64_t* smem) {
+  const int64_t bar_bytes = 256, b_bytes = tc_b_img_bytes(kp, kTcBN);
+  const int64_t ns = (227 * 1024 - bar_bytes - tc_a_span(kp)) / (b_bytes + tc_value_img_bytes(dkv));
+  *nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
+  *smem = tc_a_span(kp) + *nstage * (b_bytes + tc_value_img_bytes(dkv)) + bar_bytes;
+}
+static TcApplyPlan make_tc_apply_plan(int64_t N, int64_t M, int D, int K) {
+  TcApplyPlan a;
+  a.p = make_tc_plan(N, M, D, true);
+  a.off_v = a.p.off_part + round_up64((int64_t)a.p.n_split * N * (1 + std::min(K, 64)) * 4, 256);
+  a.off_vmax = a.off_v + round_up64(a.p.b_tiles * tc_value_img_bytes(tc_apply_dkv(K, 0)), 256);
+  a.total = a.off_vmax + round_up64((int64_t)K * 4, 256);
+  return a;
+}
+
+int64_t plan_apply_tc_scratch_bytes(int64_t N, int64_t M, int D, int K) { return make_tc_apply_plan(N, M, D, K).total; }
+
+template <int DKV>
+static int tc_apply_launch(const TcApplyPlan& a, unsigned char* base, int64_t N, int kv, cudaStream_t st) {
+  int nstage;
+  int64_t smem;
+  tc_apply_stages(a.p.kp, DKV, &nstage, &smem);
+  if (nstage < 2) return B200OT_EINVAL;
+  B200OT_CUDA_TRY(cudaFuncSetAttribute(tc_apply_kernel<DKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const dim3 grid((unsigned)a.p.ctas, (unsigned)a.p.n_split);
+  tc_apply_kernel<DKV><<<grid, kTcThreads, (size_t)smem, st>>>(base, base + a.p.off_b, base + a.off_v,
+                                                              reinterpret_cast<float*>(base + a.p.off_part), N,
+                                                              a.p.kp, a.p.ctpe, a.p.tiles_per_split, nstage, kv);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// out (N, K) = row_factor_i sum_j softmax_j(...) V_jk on the tensor-core path.  Arguments already validated.
+int plan_apply_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                  const float* center, const float* lse2, const float* v, const float* row_factor, float* out,
+                  int64_t N, int64_t M, int D, int K, float eps, void* scratch, cudaStream_t st) {
+  const TcApplyPlan a = make_tc_apply_plan(N, M, D, K);
+  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
+  int rc = tc_pack(a.p, base, {x, y, center, softmin_coord_scale(2, eps), N, M, D, 1, nullptr, h_a, h_b, h_scale_b, lse2},
+                   st);
+  if (rc) return rc;
+  float* vmax = reinterpret_cast<float*>(base + a.off_vmax);
+  B200OT_CUDA_TRY(cudaMemsetAsync(vmax, 0, (size_t)K * sizeof(float), st));
+  col_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(M, 8), 1024), dim3(32, 8), 0, st>>>(v, M, K, vmax);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  float* part = reinterpret_cast<float*>(base + a.p.off_part);
+  for (int k0 = 0; k0 < K; k0 += 64) {
+    const int kv = std::min(64, K - k0), dkv = tc_apply_dkv(K, k0);
+    const int64_t ncols = a.p.b_tiles * kTcBN;
+    tc_pack_values_kernel<<<(unsigned)ceil_div64(ncols, 128), 128, 0, st>>>(v, vmax, M, K, k0, dkv, ncols,
+                                                                           base + a.off_v);
+    B200OT_CUDA_TRY(cudaGetLastError());
+    rc = dkv == 16   ? tc_apply_launch<16>(a, base, N, kv, st)
+         : dkv == 32 ? tc_apply_launch<32>(a, base, N, kv, st)
+         : dkv == 48 ? tc_apply_launch<48>(a, base, N, kv, st)
+                     : tc_apply_launch<64>(a, base, N, kv, st);
+    if (rc) return rc;
+    rc = plan_apply_finalize(part, a.p.n_split, 1 + kv, kv, k0, K, vmax, row_factor, out, N, st);
+    if (rc) return rc;
+  }
   return B200OT_OK;
 }
 

@@ -95,6 +95,17 @@ int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, con
                    bool batched = false, const float** w_absmax_out = nullptr, float clampq = 0.f,
                    const float** coord_absmax_out = nullptr);
 
+// The plan applied to a value matrix v (M, K) (b200ot_plan_apply): the tensor-core pass (b200ot_kernel_conv.cu,
+// tcapply.cuh) and the finalize both paths share (b200ot_plan_apply.cu).
+int64_t plan_apply_tc_scratch_bytes(int64_t N, int64_t M, int D, int K);
+int plan_apply_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                  const float* center, const float* lse2, const float* v, const float* row_factor, float* out,
+                  int64_t N, int64_t M, int D, int K, float eps, void* scratch, cudaStream_t st);
+// out[i, k0 + k] = row_factor_i (sum_s part[s, i, 1 + k]) / (sum_s part[s, i, 0]) / s_k for k < kv, part (n_part, N,
+// nacc); s_k = tc_energy_coord_scale(vmax[k0 + k]) when vmax is given, row_factor_i = 1 when it is null
+int plan_apply_finalize(const float* part, int n_part, int nacc, int kv, int k0, int K, const float* vmax,
+                        const float* row_factor, float* out, int64_t N, cudaStream_t st);
+
 // Block-sparse softmins on the tensor cores (8 < D <= 64, p = 2; b200ot_*_blocks).  blocks_validate checks the host
 // descriptors (tile-aligned, one segment per row tile) and returns the longest segment in column tiles and the number
 // of pieces the segments reference.

@@ -407,11 +407,14 @@ __device__ __forceinline__ TcCta tc_cta_prologue(unsigned char* smem, int kp, in
 }
 
 // The TMA producer (one lane of the warp behind the warpgroups): the row image once, then the CTA's column tiles
-// through the ring
-template <bool BLOCKS>
+// through the ring.  EXTRA: every column tile travels with a second image of e_bytes (tile ct at e_imgs + ct e_bytes)
+// into slot `st` of a ring of its own at e_ring, its bytes in the stage's expect_tx (tcapply.cuh: the value image).
+template <bool BLOCKS, bool EXTRA = false>
 __device__ __forceinline__ void tc_produce(const TcCta& c, const unsigned char* __restrict__ a_imgs,
                                            const unsigned char* __restrict__ b_imgs,
-                                           const int2* __restrict__ bpieces, int NSTAGE, int lane) {
+                                           const int2* __restrict__ bpieces, int NSTAGE, int lane,
+                                           const unsigned char* __restrict__ e_imgs = nullptr,
+                                           unsigned char* e_ring = nullptr, int e_bytes = 0) {
   if (lane == 0) {
     mbar_arrive_expect_tx(c.bar_a, c.a_bytes);
     tma_load_1d(c.sa, a_imgs + (int64_t)c.row_tile * c.a_bytes, c.a_bytes, c.bar_a);
@@ -419,7 +422,7 @@ __device__ __forceinline__ void tc_produce(const TcCta& c, const unsigned char* 
     for (int k = 0; k < c.nt; ++k) {
       const int st = k % NSTAGE;
       if (k >= NSTAGE) mbar_wait(&c.empty_b[st], ((k / NSTAGE) + 1) & 1);
-      mbar_arrive_expect_tx(&c.full_b[st], c.b_bytes);
+      mbar_arrive_expect_tx(&c.full_b[st], EXTRA ? c.b_bytes + e_bytes : c.b_bytes);
       int ct = c.t0 + k;
       if constexpr (BLOCKS) {
         const int2 pp = bpieces[pc];
@@ -430,6 +433,8 @@ __device__ __forceinline__ void tc_produce(const TcCta& c, const unsigned char* 
         }
       }
       tma_load_1d(c.sb + st * c.b_bytes, b_imgs + (int64_t)ct * c.b_bytes, c.b_bytes, &c.full_b[st]);
+      if constexpr (EXTRA)
+        tma_load_1d(e_ring + (int64_t)st * e_bytes, e_imgs + (int64_t)ct * e_bytes, e_bytes, &c.full_b[st]);
     }
   }
 }

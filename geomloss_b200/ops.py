@@ -206,6 +206,35 @@ def softmin_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, ce
     return gx
 
 
+def plan_apply_raw(eps, x, y, h_a, h_b, h_scale_b, lse2, v, *, row_factor=None, center=None):
+    """``out[i, k] = row_factor_i * sum_j w_ij v[j, k]`` with ``w_ij = softmax_j(h_j - |x_i - y_j|^2 / (2 eps))`` and
+    ``h = h_a + h_scale_b * h_b`` (b200ot_plan_apply): the softmin's weights applied to a value matrix without ever
+    forming them.  ``lse2`` is ``softmin_raw(..., want_lse2=True)[1]`` for the same arguments; ``v`` is (M,) or (M, K),
+    any sign, any strides.  p = 2, D <= 64.  One pass over the pairs per slab of value columns (8 for D <= 8, 64
+    above).  No autograd.  Returns (N,) or (N, K)."""
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, lse2, v = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(v, "v")
+    row_factor = _f32c(row_factor, "row_factor")
+    _check_clouds(x, y, MAX_D_TC)
+    N, D = x.shape
+    M = y.shape[0]
+    if v.dim() not in (1, 2) or v.shape[0] != M or v.numel() == 0:
+        raise ValueError(f"v must be (M,) or (M, K) with M = {M} and K >= 1, got {tuple(v.shape)}")
+    if h_a.numel() != M or (h_b is not None and h_b.numel() != M):
+        raise ValueError("h must have one entry per column")
+    if lse2.numel() != N or (row_factor is not None and row_factor.numel() != N):
+        raise ValueError("lse2 and row_factor must have one entry per row")
+    K = 1 if v.dim() == 1 else v.shape[1]
+    dev = x.device
+    with nvtx_range(f"b200ot.plan_apply N={N} M={M} D={D} K={K}"):
+        out = torch.empty((N,) if v.dim() == 1 else (N, K), dtype=torch.float32, device=dev)
+        scratch = _scratch(_query(dev, "b200ot_plan_apply_scratch_bytes", N, M, D, K), dev, "plan_apply")
+        slabs = -(-K // (8 if D <= MAX_D else 64))
+        _call(dev, "b200ot_plan_apply", x, y, h_a, h_b, float(h_scale_b), center, lse2, v, row_factor, out, N, M, D, K,
+              2, float(eps), scratch, scratch.numel(), launches=1 + 3 * slabs)
+    return out
+
+
 class _Softmin(torch.autograd.Function):
     """``scale_out * softmin(eps, (x, y), h_a + h_scale_b*h_b)`` with the reference's autograd contract: the gradient
     flows to the row cloud x only; y and h are treated as constants (they are ``.detach()``-ed at every call site of

@@ -252,6 +252,13 @@ def solve_sample_batch(*args, **kwargs):
 # ----------------------------------------------------------------------------------------------------
 # results                                       ot/_ot_result.py:164-440, sample.py:444-641
 # ----------------------------------------------------------------------------------------------------
+def _fused_operator(s):
+    """Whether ``operator @ s`` runs on the fused kernel (``ops.plan_apply_raw``): every CUDA tensor.  The engine has no
+    CPU path; a host tensor is evaluated through ``ops.softmin_raw`` alone, where the real operator refuses it, so that
+    a stand-in for that one operator drives the whole facade on the CPU (tests/test_host_logic.py)."""
+    return s.is_cuda
+
+
 class LinearOperator:
     """``x -> A @ x`` without the matrix (ot/_ot_result.py:9-160): ``op @ x``, ``op.T``, ``op.shape``."""
 
@@ -294,8 +301,9 @@ class LinearOperator:
 class OTResultSample:
     """Result of :func:`solve_sample`; lazily evaluated, cached attributes named like the reference's
     (``value``, ``potential_a/b/aa/bb``, ``marginal_a/b``, ``plan``, ``density``, ``plan_operator``,
-    ``density_operator``; ``lazy_plan``, ``lazy_density``, ``a_to_b``, ``b_to_a`` are ``None`` as in the reference
-    without KeOps)."""
+    ``density_operator``; ``lazy_plan``, ``lazy_density`` are ``None`` as in the reference without KeOps).  ``a_to_b``
+    / ``b_to_a``, documented and unimplemented in the reference (ot/_ot_result.py:408-418), are the barycentric
+    displacement fields of the plan."""
 
     def __init__(self, *, X_a, X_b, a, b, reg, unbalanced, debias, potentials, softmin):
         self._X_a, self._X_b, self._a, self._b = X_a, X_b, a.detach(), b.detach()
@@ -342,43 +350,106 @@ class OTResultSample:
             G = (rho + eps / 2) * (torch.exp(-g_bb / rho) - torch.exp(-g_ab / rho))
         return ((a * F).sum() + (b * G).sum()).float()
 
-    # ---- the plan as an operator: P s = exp((f - softmin(eps, log s, C, g)) / eps), s >= 0 -----------
-    def _density_matmat(self, s, transpose):
-        """(density @ s) for s of shape (M, V) [or density.T @ s, s of shape (N, V)], one pair of softmins per
-        column: signed inputs are split into positive and negative parts, each a log-weight vector."""
+    # ---- the plan as an operator ---------------------------------------------------------------------
+    # With w_ij = softmax_j(h_j - C_ij / reg), h = log_w + g / reg, and sm the softmin of the same h:
+    #   sum_j w_j exp((f_i + g_j - C_ij) / reg) s_jk = exp((f_i - sm_i) / reg) * sum_j w_ij s_jk      (w = exp(log_w))
+    # so (density @ s) takes log_w = 0 and (plan @ s) takes w = b and the row factor a_i exp((f_i - sm_i) / reg), which
+    # is the plan's marginal.  One forward softmin per (direction, weighting) gives lse2 and the row factor; after
+    # that every application is ONE call of ops.plan_apply_raw, for any number of columns and any signs.
+    def _apply_state(self, transpose, weighted):
+        """(log_w, lse2, row_factor) of the operator's direction, cached until ``cache_clear``."""
+        cache = self.__dict__.setdefault("_apply_cache", {})
+        key = (bool(transpose), bool(weighted))
+        if key not in cache:
+            eps = self._reg
+            rows, cols = (self._X_b, self._X_a) if transpose else (self._X_a, self._X_b)
+            f, g = (self._g_ab, self._f_ba) if transpose else (self._f_ba, self._g_ab)
+            w_rows, w_cols = (self._b, self._a) if transpose else (self._a, self._b)
+            with torch.no_grad():
+                log_w = log_weights(w_cols) if weighted else torch.zeros_like(w_cols)
+                smv, lse2 = ops.softmin_raw(0.5 * eps, rows, cols, log_w, g, 1.0 / eps, p=2, center=self._sm.center,
+                                            beta=2.0, want_lse2=True)
+                factor = torch.exp((f - smv) / eps)
+                if weighted:
+                    factor = w_rows * factor
+            cache[key] = (log_w, lse2, factor.contiguous())
+        return cache[key]
+
+    def _apply(self, s, transpose, weighted, *, normalized=False):
+        """plan @ s (weighted) or density @ s for s of shape (M, K) [``.T @ s`` with ``transpose``, s (N, K)];
+        ``normalized``: rows of weights summing to one (no row factor).  Detached."""
+        rows, cols = (self._X_b, self._X_a) if transpose else (self._X_a, self._X_b)
+        g = self._f_ba if transpose else self._g_ab
+        log_w, lse2, factor = self._apply_state(transpose, weighted)
+        with torch.no_grad():
+            return ops.plan_apply_raw(0.5 * self._reg, rows, cols, log_w, g, 1.0 / self._reg, lse2, s.detach().float(),
+                                      row_factor=None if normalized else factor, center=self._sm.center)
+
+    def _density_matmat(self, s, transpose, weighted=False):
+        """(density @ s), or (plan @ s) when ``weighted``; differentiable w.r.t. s when it requires a gradient."""
+        if not _fused_operator(s):
+            return self._matmat_by_softmins(s, transpose, weighted)
+        if torch.is_grad_enabled() and s.requires_grad:
+            return _PlanApply.apply(self, s, transpose, weighted)
+        return self._apply(s, transpose, weighted)
+
+    def _matmat_by_softmins(self, s, transpose, weighted):
+        """The same product through ``ops.softmin_raw`` alone, P s = exp((f - softmin(eps, log s, C, g)) / eps) for
+        s >= 0: one softmin per column and sign.  Host tensors only (see ``_fused_operator``)."""
         eps = self._reg
         rows, cols = (self._X_b, self._X_a) if transpose else (self._X_a, self._X_b)
         f, g = (self._g_ab, self._f_ba) if transpose else (self._f_ba, self._g_ab)
+        w_rows, w_cols = (self._b, self._a) if transpose else (self._a, self._b)
         out = []
         with torch.no_grad():
             for v in range(s.shape[1]):
-                col = s[:, v].float().contiguous()
+                col = s[:, v].float() * w_cols if weighted else s[:, v].float()
                 acc = torch.zeros(rows.shape[0], dtype=torch.float32, device=rows.device)
                 for sign in (1.0, -1.0):
                     part = (sign * col).clamp_min(0.0)
                     if bool((part > 0).any()):
-                        smv = self._sm(eps, rows, cols, log_weights(part), g)
-                        acc = acc + sign * torch.exp((f - smv) / eps)
-                out.append(acc)
+                        acc = acc + sign * torch.exp((f - self._sm(eps, rows, cols, log_weights(part), g)) / eps)
+                out.append(w_rows * acc if weighted else acc)
         return torch.stack(out, 1)
+
+    def _operator(self, weighted):
+        N, M = self._X_a.shape[0], self._X_b.shape[0]
+        return LinearOperator(matmat=lambda s: self._density_matmat(s, False, weighted),
+                              rmatmat=lambda s: self._density_matmat(s, True, weighted), input_shape=(M,),
+                              output_shape=(N,))
 
     @cached_property
     def density_operator(self):
-        N, M = self._X_a.shape[0], self._X_b.shape[0]
-        return LinearOperator(matmat=lambda s: self._density_matmat(s, False),
-                              rmatmat=lambda s: self._density_matmat(s, True), input_shape=(M,), output_shape=(N,))
+        return self._operator(False)
 
     @cached_property
     def plan_operator(self):
-        return self.density_operator.rescale(input_scaling=self._b, output_scaling=self._a)
+        return self._operator(True)
 
+    # (the plan's marginals are the row factors of the two directions: a_i sum_j b_j density_ij)
     @cached_property
     def marginal_a(self):
-        return self._a * (self.density_operator @ self._b)
+        return self._apply_state(False, True)[2]
 
     @cached_property
     def marginal_b(self):
-        return self._b * (self.density_operator.T @ self._a)
+        return self._apply_state(True, True)[2]
+
+    # ---- barycentric maps: displacement of each point to the conditional mean of its row of the plan ------
+    def _barycentric(self, transpose):
+        src, dst = (self._X_b, self._X_a) if transpose else (self._X_a, self._X_b)
+        c = self._sm.center
+        return self._apply(dst - c, transpose, True, normalized=True) + c - src
+
+    @cached_property
+    def a_to_b(self):
+        """(N, D): sum_j P_ij X_b[j] / sum_j P_ij - X_a[i] (also defined for unbalanced problems); detached."""
+        return self._barycentric(False)
+
+    @cached_property
+    def b_to_a(self):
+        """(M, D): the same on the transposed plan; detached."""
+        return self._barycentric(True)
 
     # ---- dense accessors (small problems only) --------------------------------------------------------
     @cached_property
@@ -396,9 +467,24 @@ class OTResultSample:
 
     lazy_density = None
     lazy_plan = None
-    a_to_b = None
-    b_to_a = None
 
     def cache_clear(self):
-        for k in ("value", "density_operator", "plan_operator", "marginal_a", "marginal_b", "density", "plan"):
+        for k in ("value", "density_operator", "plan_operator", "marginal_a", "marginal_b", "density", "plan",
+                  "a_to_b", "b_to_a", "_apply_cache"):
             self.__dict__.pop(k, None)
+
+
+class _PlanApply(torch.autograd.Function):
+    """``plan @ s`` / ``density @ s`` (or their transposes) as a function of s alone: the operator is linear in s,
+    so the gradient is the transposed operator applied to the upstream gradient.  Clouds and potentials are constants,
+    as for every other accessor of the result."""
+
+    @staticmethod
+    def forward(ctx, res, s, transpose, weighted):
+        ctx.res, ctx.meta = res, (transpose, weighted)
+        return res._apply(s, transpose, weighted)
+
+    @staticmethod
+    def backward(ctx, go):
+        transpose, weighted = ctx.meta
+        return None, ctx.res._apply(go, not transpose, weighted), None, None

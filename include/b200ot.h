@@ -106,6 +106,22 @@ B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float*
                          int64_t M, int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
                          void* stream);
 
+/* The softmax weights of the p = 2 softmin applied to a value matrix, in one reduction over the pairs per slab of
+ * value columns (the transport plan times V: barycentric maps, colour / label / feature transport):
+ *   out[i,k] = row_factor[i] * sum_j w_ij v[j,k],   w_ij = softmax_j(h_j - |x_i - y_j|^2 / (2 eps))
+ *   v (M,K) row-major, any sign, K >= 1;  out (N,K) is overwritten;  row_factor (N, nullable): 1 when null;
+ *   lse2 (N): the lse2_out of b200ot_softmin_fwd for the same x, y, h, center, eps.  The weights are normalised by
+ *       the kernel's own sum over j, so rounding of lse2 cancels and a constant v comes back (to rounding);
+ *   a column with h_j = -1e5 (the engine's log 0) contributes exactly 0;
+ *   1 <= D <= 64, p = 2 only.  D <= 8 runs on the CUDA cores in slabs of 8 value columns, above on the tensor cores
+ *   in slabs of 64 (routing as for b200ot_softmin_bwd_x); every slab is one pass that recomputes the exponent.
+ *   scratch: >= b200ot_plan_apply_scratch_bytes(N, M, D, K) bytes, 16-byte aligned. */
+B200OT_API int64_t b200ot_plan_apply_scratch_bytes(int64_t N, int64_t M, int32_t D, int64_t K);
+B200OT_API int b200ot_plan_apply(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                      const float* center, const float* lse2, const float* v, const float* row_factor, float* out,
+                      int64_t N, int64_t M, int32_t D, int64_t K, int32_t p, float eps, void* scratch,
+                      int64_t scratch_bytes, void* stream);
+
 /* --- the three stages of b200ot_softmin_fwd, exposed for column-sharded (multi-GPU) use --- */
 
 /* Number of floats of a packed column buffer for M columns of dimension D with `extra` per-column

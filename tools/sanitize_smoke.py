@@ -31,7 +31,7 @@ def check(name, got, ref, tol=2e-5):
 
 
 which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "wide", "blocks", "grid", "loss",
-                              "small"}
+                              "small", "apply"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -266,5 +266,19 @@ if "small" in which:
         K = lambda u, w: (-((u[:, :, None].double() - w[:, None].double()) ** 2).sum(-1) / 0.5).exp()  # noqa: E731
         ref = 0.5 * K(x, x).mean((1, 2)) + 0.5 * K(y, y).mean((1, 2)) - K(x, y).mean((1, 2))
         check(f"small_gaussian_B{B}_d{d}", v, ref, 1e-4)
+if "apply" in which:
+    # the plan applied to a value matrix: both CUDA-core tile shapes with both slab widths (K = 11: slabs of 8 and 4),
+    # and the tensor-core kernel with a value image of 16 and of 64 columns plus a second slab (K = 70)
+    for tag, n, m, d, k in (("small", 300, 500, 2, 11), ("big", 4200, 4300, 3, 11), ("big_d8", 4100, 4100, 8, 3),
+                            ("tc_d16", 700, 900, 16, 5), ("tc_d64", 300, 1000, 64, 70)):
+        x, y, h = torch.rand(n, d, generator=g), torch.rand(m, d, generator=g), torch.randn(m, generator=g)
+        v = torch.randn(m, k, generator=g)
+        xd, yd, hd = x.to(DEV), y.to(DEV), h.to(DEV)
+        eps = 0.02 * d
+        center = ops.default_center(xd, yd)
+        _, lse2 = ops.softmin_raw(eps, xd, yd, hd, p=2, center=center, want_lse2=True)
+        out = ops.plan_apply_raw(eps, xd, yd, hd, None, 0.0, lse2, v.to(DEV), center=center)
+        d2 = ((x[:, None, :].double() - y[None, :, :].double()) ** 2).sum(-1)
+        check("apply_" + tag, out, torch.softmax(h.double()[None, :] - d2 / (2 * eps), dim=1) @ v.double(), 2e-4)
 torch.cuda.synchronize()
 print("sanitize_smoke: all launches completed")
