@@ -267,36 +267,6 @@ bool tc_any_routed(int D, int64_t N, int64_t M) {
   return false;
 }
 
-// Tuning of the row-gradient kernels (tcbwd.cuh), $B200OT_TC_BWD = "p_terms,epi,ldall,merge" for A/B timing and the
-// variants' parity tests (the settings string of the C ABI, see b200ot.h):
-//   p_terms  fp16 terms of P in GEMM 2 (PT).  PT = 1 saves a third of the GEMM-2 work but feeds GEMM 2 an 11-bit image
-//            of P (every weight perturbed by <= 2^-12) — kept as a knob, not the default.  Measured on an
-//            H100 80GB HBM3 (400 W) at N = M = 4e5, gaussian / softmin row gradients, ms: D = 16 119.5 / 111.9 (PT = 2)
-//            against 107.7 / 91.3 (PT = 1); D = 64 260 / 222 against 229 / 196.
-//   merge    hi.[Y_h | Y_l] as one N = 2 dk instruction per K step (1) or two N = dk instructions (0): the same
-//            products and the same fp32 accumulation, so the choice does not change the result.
-//   epi, ldall  the epilogue-warp count (8 or 16) and the single-load TMEM read-back of tensor-memory kernels.  The
-//            wgmma kernels keep S and P in the registers of their two consumer warpgroups, so neither has a counterpart
-//            here: both are validated and otherwise leave the kernel unchanged.
-struct TcBwdTuning {
-  int p_terms, epi, ldall, merge;
-};
-static const TcBwdTuning kTcBwdDefault = {2, 8, 0, 1};
-static TcBwdTuning tc_bwd_tuning() {
-  TcBwdTuning t = kTcBwdDefault;
-  if (const char* e = getenv("B200OT_TC_BWD")) {
-    int a, b, c, d;
-    if (sscanf(e, "%d,%d,%d,%d", &a, &b, &c, &d) == 4 && (a == 1 || a == 2) && (b == 8 || b == 16) &&
-        (c == 0 || c == 1) && (d == 0 || d == 1)) {
-      t.p_terms = a;
-      t.epi = b;
-      t.ldall = c;
-      t.merge = d;
-    }
-  }
-  return t;
-}
-
 // The plan of a launch group: `ctas` row CTAs, each reading up to `tiles` (>= 1) column tiles.  The split count is
 // chosen for the whole grid and cuts those tiles.  Behind the images: the partials of `rows` rows ((m, s) pairs forward, D+1
 // sums per row backward, D+2 for the p = 1 softmin: `head` sums ahead of the D), then a misc block of misc_bytes.
@@ -435,27 +405,14 @@ static int tc_launch(TcKernel kern, const TcPlan& p, unsigned char* base, int64_
 }
 
 // tc_bwd_kernel at the padded dimension of D
-template <int MODE, int PT, bool MERGE, bool BATCH, bool BLOCKS = false>
+template <int MODE, bool BATCH, bool BLOCKS = false>
 static TcKernel tc_bwd_dk(int D) {
   switch (tc_dk(D)) {
-    case 16: return tc_bwd_kernel<MODE, PT, MERGE, 16, BATCH, BLOCKS>;
-    case 32: return tc_bwd_kernel<MODE, PT, MERGE, 32, BATCH, BLOCKS>;
-    case 48: return tc_bwd_kernel<MODE, PT, MERGE, 48, BATCH, BLOCKS>;
-    default: return tc_bwd_kernel<MODE, PT, MERGE, 64, BATCH, BLOCKS>;
+    case 16: return tc_bwd_kernel<MODE, 16, BATCH, BLOCKS>;
+    case 32: return tc_bwd_kernel<MODE, 32, BATCH, BLOCKS>;
+    case 48: return tc_bwd_kernel<MODE, 48, BATCH, BLOCKS>;
+    default: return tc_bwd_kernel<MODE, 64, BATCH, BLOCKS>;
   }
-}
-
-// The row-gradient instantiation of MODE: the $B200OT_TC_BWD variant for the gaussian and the softmin of one problem,
-// the default variant (PT = 2, MERGE) for the laplacian, the energy and every batch
-template <int MODE>
-static TcKernel tc_bwd_variant(int D, bool batched) {
-  if (batched) return tc_bwd_dk<MODE, 2, true, true>(D);
-  if constexpr (MODE == 2 || MODE == 3) {
-    const TcBwdTuning tn = tc_bwd_tuning();
-    if (tn.merge) return tn.p_terms == 1 ? tc_bwd_dk<MODE, 1, true, false>(D) : tc_bwd_dk<MODE, 2, true, false>(D);
-    return tn.p_terms == 1 ? tc_bwd_dk<MODE, 1, false, false>(D) : tc_bwd_dk<MODE, 2, false, false>(D);
-  }
-  return tc_bwd_dk<MODE, 2, true, false>(D);
 }
 
 // Row gradients on the tensor-core path; `mode` is the MODE of tc_bwd_kernel (2 gaussian conv, 3 softmin p = 2,
@@ -473,10 +430,10 @@ int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, con
   int rc = tc_pack(p, base, {x, y, center, scale, N, M, D, B, w, h_a, h_b, h_scale_b, lse2}, st, &w_absmax,
                    mode == 5 ? &coord_absmax : nullptr);
   if (rc) return rc;
-  const TcKernel kern = mode == 2   ? tc_bwd_variant<2>(D, batched)
-                        : mode == 3 ? tc_bwd_variant<3>(D, batched)
-                        : mode == 4 ? tc_bwd_variant<4>(D, batched)
-                                    : tc_bwd_variant<5>(D, batched);
+  const TcKernel kern = mode == 2   ? (batched ? tc_bwd_dk<2, true>(D) : tc_bwd_dk<2, false>(D))
+                        : mode == 3 ? (batched ? tc_bwd_dk<3, true>(D) : tc_bwd_dk<3, false>(D))
+                        : mode == 4 ? (batched ? tc_bwd_dk<4, true>(D) : tc_bwd_dk<4, false>(D))
+                                    : (batched ? tc_bwd_dk<5, true>(D) : tc_bwd_dk<5, false>(D));
   const int self_mode = (mode != 3 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
   rc = tc_launch(kern, p, base, B * N, N, D, self_mode, clampq, coord_absmax, st);
   if (rc) return rc;
@@ -592,7 +549,7 @@ int softmin_l1_tc(bool bwd, const float* x, const float* y, const float* h_a, co
   o.l1_c = kLog2e / eps;
   int rc = tc_pack(pl, base, o, st, nullptr, &coord_absmax);
   if (rc) return rc;
-  const TcKernel kern = bwd ? tc_bwd_dk<7, 2, true, true>(D) : tc_reduce_kernel<6, true>;
+  const TcKernel kern = bwd ? tc_bwd_dk<7, true>(D) : tc_reduce_kernel<6, true>;
   const int self_mode = (x == y && N == M) ? 1 : 0;  // xx / yy: the diagonal takes d = sqrt(clamp) exactly
   rc = tc_launch(kern, pl, base, B * N, N, D, self_mode, cost_clamp(p), coord_absmax, st);
   if (rc) return rc;
@@ -806,8 +763,7 @@ int softmin_blocks_tc(bool bwd, const float* x, const float* y, const float* h_a
                     h_scale_b, bwd ? lse2 : nullptr, row_src, col_src},
                    st);
   if (rc) return rc;
-  // the row gradient runs its default variant (PT = 2, MERGE)
-  const TcKernel kern = bwd ? tc_bwd_dk<3, 2, true, false, true>(D) : tc_reduce_kernel<1, false, true>;
+  const TcKernel kern = bwd ? tc_bwd_dk<3, false, true>(D) : tc_reduce_kernel<1, false, true>;
   rc = tc_launch(kern, p, base, N, 0, D, 0, 0.f, nullptr, st, d_seg, d_pieces, row_src);
   if (rc) return rc;
   *part_out = reinterpret_cast<float*>(base + p.off_part);

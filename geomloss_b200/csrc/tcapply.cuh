@@ -3,7 +3,7 @@
 // image.
 //
 //   S_ij = the softmin exponent - lse2_i + 14                      GEMM 1, tc_exponent_gemm, as tc_bwd_kernel<3>
-//   P_ij = 2^S_ij = hi + lo (two fp16 terms, in registers)         tc_bwd_tile<3, 2>
+//   P_ij = 2^S_ij = hi + lo (two fp16 terms, in registers)         tc_bwd_tile<3>
 //   G_ik = sum_j P_ij s_k V_jk                                     GEMM 2: A = P, B = the value image of the tile
 //   part[(split N + i)(1 + KV) + {0, 1 + k}] = {sum_j P_ij, G_ik}  tc_bwd_store
 //
@@ -93,7 +93,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     wgmma_wait<0>();
     reg_fence(s);
     uint32_t ph[32], pl[32];
-    tc_bwd_tile<3, 2>(s, c, st, kp, k, row0, tb, rt, 0.f, 0, cq, ph, pl, sum, sumq);
+    tc_bwd_tile<3>(s, c, st, kp, k, row0, tb, rt, 0.f, 0, cq, ph, pl, sum, sumq);
     // ---- GEMM 2: G += P . V, K = the 128 columns of the tile, 16 per instruction ----
     const uint32_t v_addr = smem_u32(sv + st * v_bytes);
     wgmma_fence();

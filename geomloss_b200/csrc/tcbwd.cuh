@@ -24,8 +24,8 @@
 // * The column image of tcconv.cuh ([kgroup][column][8 halves], K-major for GEMM 1) is, read with k = column,
 //   exactly the canonical MN-major no-swizzle layout (core matrix = 8 columns x 16 B of one 8-dim group), so
 //   GEMM 2 needs no second copy of Y: only a descriptor read MN-major, LBO = 128 B (next 8 columns),
-//   SBO = BN*16 B (next 8 dims).  The l term of Y follows its h term in the image, so hi.[Y_h | Y_l] can be ONE
-//   instruction with N = 2 dk per K step (MERGE), accumulating [G_a | G_b] (added at the end); lo.Y_h is an N = dk
+//   SBO = BN*16 B (next 8 dims).  The l term of Y follows its h term in the image, so hi.[Y_h | Y_l] is ONE
+//   instruction with N = 2 dk per K step, accumulating [G_a | G_b] (added at the end); lo.Y_h is an N = dk
 //   instruction into G_a alone.
 #pragma once
 #include "tcconv.cuh"
@@ -60,13 +60,6 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t d
 // by these modes only).  The gradient is then coef (sum_j P_ij Y_j - X_i sum_j P_ij): the finalize of the gaussian.
 // part[(split*N + row)*(D+1) + {0, 1+k}] = sum_j P_ij {1, Y_jk}
 // DK = the padded dimension tc_dk(D) (N of GEMM 2 is a compile-time constant).
-// MERGE: hi.Y_h and hi.Y_l as one N = 2 DK instruction per K step, or as two N = DK instructions into G_a and G_b.
-//
-// PT = fp16 terms of P fed to GEMM 2.  PT = 2: P = hi + lo, products hi.h, hi.l, lo.h (error ~2^-22 |P||Y|).
-// PT = 1: P = hi only, products hi.h, hi.l — a third less GEMM-2 work and no lo split.  Every weight is then
-// perturbed by <= 2^-12 relative (round to nearest, unbiased); the row sum of P is taken over the SAME rounded
-// values, so the gradient (sum_j P_ij Y_j) - X_i (sum_j P_ij) = sum_j hi_ij (Y_j - X_i) stays a combination of exact
-// differences — the perturbation never meets the cancellation between the two sums.
 //
 // self_mode: rows and columns are the same cloud (the K_xx term): the exponent of pair (i, i) is exactly 0, as in
 // tc_reduce_kernel — matters when sum_j P_ij is used as the forward VALUE (b200ot_kernel_conv_fwd_bwd_x).
@@ -93,13 +86,13 @@ __device__ __forceinline__ float2 tc_l1_pq(float s, float t, float clampq, float
 }
 
 // S -> P of one column tile, packed as the A fragments of GEMM 2 (ph[2 n8 + h] = the pair of row h in 8-column block
-// n8; pl the lo terms when PT = 2), and the tile's contribution to the row sums (sum: P, sumq: Q for MODE 7).  The
-// column slot, tile and rows as for tc_reduce_tile (tcconv.cuh).
-template <int MODE, int PT>
+// n8; pl the lo terms), and the tile's contribution to the row sums (sum: P, sumq: Q for MODE 7).  The column slot,
+// tile and rows as for tc_reduce_tile (tcconv.cuh).
+template <int MODE>
 __device__ __forceinline__ void tc_bwd_tile(float (&s)[64], const TcCta& c, int st, int kp, int k, int64_t row0,
                                             const float (&tb)[2], const float2 (&rt)[2], float clampq, int self_mode,
-                                            int cq, uint32_t (&ph)[32], uint32_t (&pl)[PT == 2 ? 32 : 1],
-                                            float (&sum)[2], float (&sumq)[2]) {
+                                            int cq, uint32_t (&ph)[32], uint32_t (&pl)[32], float (&sum)[2],
+                                            float (&sumq)[2]) {
   if constexpr (MODE != 3) {
     if (self_mode) tc_zero_diagonal(s, row0 - (int64_t)(c.t0 + k) * kTcBN, cq);
   }
@@ -138,16 +131,12 @@ __device__ __forceinline__ void tc_bwd_tile(float (&s)[64], const TcCta& c, int 
       const uint32_t hh = pack_f16x2(p0, p1);
       ph[2 * n8 + h] = hh;
       const float2 hf = unpack_f16x2(hh);
-      if constexpr (PT == 2) {
-        if constexpr (MODE == 7) {
-          tq[h] += p0 + p1;
-        } else {
-          ts[h] += p0 + p1;
-        }
-        pl[2 * n8 + h] = pack_f16x2(p0 - hf.x, p1 - hf.y);
+      if constexpr (MODE == 7) {
+        tq[h] += p0 + p1;
       } else {
-        ts[h] += hf.x + hf.y;  // the sums see exactly what GEMM 2 sees
+        ts[h] += p0 + p1;
       }
+      pl[2 * n8 + h] = pack_f16x2(p0 - hf.x, p1 - hf.y);
     }
   }
   sum[0] += ts[0];
@@ -197,7 +186,7 @@ __device__ __forceinline__ void tc_bwd_store(float* __restrict__ part, const flo
 // BATCH: B problems side by side, laid out and mapped to rows and column tiles as in tc_reduce_kernel (tcconv.cuh).
 // BLOCKS: block-sparse softmin (MODE 3), segments, pieces and row_src as in tc_reduce_kernel; a split without a tile
 // writes zero sums.
-template <int MODE, int PT, bool MERGE, int DK, bool BATCH = false, bool BLOCKS = false>
+template <int MODE, int DK, bool BATCH = false, bool BLOCKS = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
     tc_bwd_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
                   float* __restrict__ part, int64_t N, int kp, int ntiles_b, int tiles_per_split, int NSTAGE, int D,
@@ -205,10 +194,8 @@ __global__ void __launch_bounds__(kTcThreads, 1)
                   const int4* __restrict__ bseg = nullptr, const int2* __restrict__ bpieces = nullptr,
                   const int* __restrict__ row_src = nullptr) {
   static_assert(MODE == 2 || MODE == 3 || MODE == 4 || MODE == 5 || MODE == 7, "row-gradient modes");
-  static_assert(PT == 1 || PT == 2, "P is fed to GEMM 2 as one or two fp16 terms");
   static_assert(DK % 16 == 0 && DK <= 64, "padded dimension");
   static_assert(!BLOCKS || (MODE == 3 && !BATCH), "the block-sparse layout serves the softmin of one problem");
-  static_assert(MODE != 7 || PT == 2, "the p = 1 row gradient sums P and Q apart: two fp16 terms of Q");
   extern __shared__ __align__(1024) unsigned char smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const TcCta c = tc_cta_prologue<BATCH, BLOCKS>(smem, kp, NSTAGE, ntiles_b, tiles_per_split, rtpe, bseg, bpieces);
@@ -247,21 +234,15 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     tc_exponent_gemm(s, a_addr, b_addr, DK / 8);
     wgmma_wait<0>();
     reg_fence(s);
-    uint32_t ph[32], pl[PT == 2 ? 32 : 1];
-    tc_bwd_tile<MODE, PT>(s, c, st, kp, k, row0, tb, rt, clampq, self_mode, cq, ph, pl, sum, sumq);
+    uint32_t ph[32], pl[32];
+    tc_bwd_tile<MODE>(s, c, st, kp, k, row0, tb, rt, clampq, self_mode, cq, ph, pl, sum, sumq);
     // ---- GEMM 2: G += P . Y, K = the 128 columns of the tile, 16 per instruction ----
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < kTcBN / 16; ++kk) {
       const uint64_t db = make_smem_desc(b_addr + (2 * kk) * 128, 128, kTcBN * 16);
-      if constexpr (MERGE) {
-        wgmma_rs<2 * DK>(g, &ph[4 * kk], db);
-      } else {
-        wgmma_rs<DK>(g, &ph[4 * kk], db);
-        wgmma_rs<DK>(g + DK / 2, &ph[4 * kk], make_smem_desc(b_addr + (DK / 8) * (kTcBN * 16) + (2 * kk) * 128, 128,
-                                                              kTcBN * 16));
-      }
-      if constexpr (PT == 2) wgmma_rs<DK>(g, &pl[4 * kk], db);
+      wgmma_rs<2 * DK>(g, &ph[4 * kk], db);
+      wgmma_rs<DK>(g, &pl[4 * kk], db);
     }
     wgmma_commit();
     wgmma_wait<0>();

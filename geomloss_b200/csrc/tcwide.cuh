@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     float s[64];
     const int st = tc_wide_exponent(s, c, ring, seg, own, nslab, NSTAGE, wg, lane, step);
     uint32_t ph[32], pl[32];
-    tc_bwd_tile<MODE, 2>(s, c, st, 16, k, row0, tb, rt, clampq, self_mode, cq, ph, pl, sum, sumq);
+    tc_bwd_tile<MODE>(s, c, st, 16, k, row0, tb, rt, clampq, self_mode, cq, ph, pl, sum, sumq);
     // GEMM 2 against the slice's column slab (the last one loaded): K = the tile's 128 columns, 16 per instruction.
     // In a partial last slab the columns of G past the slab's chunks read stale shared memory; they lie at or above
     // tc_dk(D) and are never written out.

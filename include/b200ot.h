@@ -26,8 +26,6 @@
  *   B200OT_TC_MIN_D      "d" or "softmin_fwd,softmin_bwd,conv_fwd,conv_bwd": smallest D <= B200OT_MAX_D an operator
  *                        hands to the tensor-core kernels (default "7,9,5,9": forward softmin from 7, gaussian from 5)
  *   B200OT_TC_MIN_PAIRS  smallest N*M for that hand-over (default 8e8)
- *   B200OT_TC_BWD        "p_terms,epilogue_warps,ldall,merge" of the tensor-core row-gradient kernel (default "2,8,0,1");
- *                        on sm_90a p_terms and merge select the kernel, epilogue_warps and ldall are validated only
  */
 #ifndef B200OT_H_
 #define B200OT_H_
@@ -243,7 +241,6 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
  * element; p = 2 only (the p = 1 softmin has entries of its own, b200ot_softmin_l1_*); D <= 8 batches go through the
  * ranges entry points.
  * EINVAL for B < 1, D <= 8 or D > 64; scratch: b200ot_batched_scratch_bytes(B, N, M, D) bytes, 16-byte aligned.
- * The batched row gradients run the default variant of the row-gradient kernel ($B200OT_TC_BWD is not read).
  * ------------------------------------------------------------------------------------------- */
 B200OT_API int64_t b200ot_batched_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D);
 B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -336,7 +333,7 @@ B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, con
  *             `stream` (from pageable memory that copy waits for the stream's earlier work).
  * Each row is reduced over exactly the columns of its segment's pieces.  Results are indexed by row (x, lse2, out,
  * grad_x: N rows), h_a / h_b by column of y.  The column tiles of a segment are cut into splits like a dense problem's
- * ($B200OT_FORCE_SPLITS applies); the row gradients run the default variant of the row-gradient kernel.
+ * ($B200OT_FORCE_SPLITS applies).
  * EINVAL (before any launch) for null pointers, N <= 0, n_seg <= 0, D <= 8 or D > 64, p other than 2, and descriptors
  * off the tile grid; EALIGN for misaligned descriptor arrays or scratch; ESCRATCH below b200ot_blocks_scratch_bytes
  * (0 for invalid descriptors).

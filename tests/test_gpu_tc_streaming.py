@@ -62,9 +62,10 @@ def _assert_close(got, ref, atol, what):
                            f"(bar {np.broadcast_to(atol, err.shape).flat[np.argmax(err)]:.3e})")
 
 
-def _softmin_checks(eps, x, y, h, go, what, rows=None, tol_grad=5e-5):
+def _softmin_checks(eps, x, y, h, go, what, rows=None):
     """Forward softmin (bar of test_softmin_tensor_core_path) and its row gradient from the forward's lse2 (bar of
-    test_row_gradient_kernel_variants); rows: the sampled row indices checked against the oracle (default: all)."""
+    test_row_gradient_kernel_at_padded_dimensions); rows: the sampled row indices checked against the oracle (default:
+    all)."""
     from geomloss_b200 import ops
     from oracle import geomloss_oracle as O
 
@@ -76,13 +77,13 @@ def _softmin_checks(eps, x, y, h, go, what, rows=None, tol_grad=5e-5):
     ref = O.softmin_points(eps, x[rows], y, h, p=2)
     _assert_close(out[rows], ref, 5e-6 * max(1.0, ref.abs().max().item()), f"{what} softmin eps={eps}")
     gref = O.softmin_grad_rows(eps, x[rows], y, h, go[rows], p=2)
-    _assert_close(gx[rows], gref, tol_grad * max(1.0, gref.abs().max().item()), f"{what} softmin gradient eps={eps}")
+    _assert_close(gx[rows], gref, 5e-5 * max(1.0, gref.abs().max().item()), f"{what} softmin gradient eps={eps}")
 
 
 def _gauss_checks(blur, x, y, w, go, what, rows=None, tol_grad=5e-5):
     """Gaussian convolution (rtol 2e-5 + the exponent's rounding slack, of sum |w| k as weights may have mixed signs:
     test_value_and_unit_gradient_in_one_pass) and its row gradient (5e-5 of the largest entry + 1e-5 of the natural
-    scale, test_row_gradient_kernel_variants)."""
+    scale, test_row_gradient_kernel_at_padded_dimensions)."""
     from geomloss_b200 import ops
 
     xd, yd, wd, god = _f32(x, y, w, go)
@@ -249,22 +250,17 @@ def test_tile_and_padding_edges(d):
 # ------------------------------------------------------------------------------------------------
 # 5. large M: P below fp16's normal range
 # ------------------------------------------------------------------------------------------------
-BWD_SETTINGS = {"2,8,0,1": 5e-5, "1,8,0,1": 2.0**-12}  # P as two fp16 terms (default) / one term (bars of the variants)
-
-
-@pytest.mark.parametrize("combo", sorted(BWD_SETTINGS))
 @pytest.mark.parametrize("d", [16, 64])
 @pytest.mark.parametrize("cloud", ["distinct", "atoms"])
-def test_softmin_row_gradient_at_large_m(cloud, d, combo):
+def test_softmin_row_gradient_at_large_m(cloud, d):
     """N = 256 rows against M = 65536 columns: the softmax weights are ~1/M = 1.5e-5, below fp16's smallest normal
     number (6.1e-5), where they would sit on the fixed 6e-8 subnormal grid if tc_bwd_kernel fed them to GEMM 2
     unscaled.  With 128 atoms x 512 copies the rounding repeats identically for every copy: a bias, not noise."""
     n, m = 256, 65536
     x, y, h, _, go = _clouds(n, m, d, seed=5 * d + (1 if cloud == "atoms" else 0),
                              atoms=128 if cloud == "atoms" else None)
-    with env(B200OT_TC_BWD=combo):
-        for eps in (2.0, 0.3):
-            _softmin_checks(eps, x, y, h, go, f"{cloud} D={d} PT={combo[0]}", tol_grad=BWD_SETTINGS[combo])
+    for eps in (2.0, 0.3):
+        _softmin_checks(eps, x, y, h, go, f"{cloud} D={d}")
 
 
 @pytest.mark.parametrize("cloud", ["distinct", "atoms"])

@@ -1,6 +1,6 @@
-"""GPU parity of the tensor-core kernels' routing and tuning knobs (csrc/b200ot_kernel_conv.cu: tc_routed,
-tc_bwd_tuning; csrc/tcbwd.cuh: PT / MERGE) and of the one-pass value + row-gradient entry
-(b200ot_kernel_conv_fwd_bwd_x).  Every setting — not only the shipped default — is held to the same bars against the
+"""GPU parity of the tensor-core kernels' routing knobs (csrc/b200ot_kernel_conv.cu: tc_routed), of the row-gradient
+kernel at every padded dimension (csrc/tcbwd.cuh) and of the one-pass value + row-gradient entry
+(b200ot_kernel_conv_fwd_bwd_x).  Every route — not only the shipped default — is held to the same bars against the
 fp64 oracle as the default kernels in test_gpu_parity.py, so that a default can be flipped from a measurement
 (tools/ab_tc_route.py) without changing what is tested."""
 import os
@@ -112,17 +112,10 @@ def test_whole_losses_on_the_tensor_core_route_d5():
         sinkhorn_small.SMALL_MAX = keep
 
 
-COMBOS = ["2,8,0,0", "2,8,0,1", "2,8,1,0", "2,8,1,1", "2,16,0,0", "2,16,0,1", "1,8,0,0", "1,8,0,1", "1,8,1,1",
-          "1,16,0,0", "1,16,0,1"]
-
-
-@pytest.mark.parametrize("combo", COMBOS)
 @pytest.mark.parametrize("shape", [(300, 500, 16), (131, 67, 40), (1500, 2300, 64), (257, 300, 24)])
-def test_row_gradient_kernel_variants(combo, shape):
-    """$B200OT_TC_BWD = "p_terms,epi,ldall,merge" -> tc_bwd_kernel<MODE, PT, MERGE, DK> (D = 16, 40, 64, 24: padded dimensions 16, 48, 64, 32; epi and ldall
-    are accepted settings without a counterpart in the wgmma kernels): gaussian and softmin row gradients against
-    fp64.  PT = 2 (P = hi + lo in GEMM 2) keeps the bar of the default kernels; PT = 1 (P = hi only) perturbs every
-    weight by <= 2^-12 relative, unbiased, with consistent row sums (tcbwd.cuh): bar 2^-12 of the largest entry."""
+def test_row_gradient_kernel_at_padded_dimensions(shape):
+    """tc_bwd_kernel<MODE, DK> at D = 16, 40, 64, 24 (padded dimensions 16, 48, 64, 32): gaussian and softmin row
+    gradients against fp64, at the bar of the default kernels."""
     from geomloss_b200 import ops
     from oracle import geomloss_oracle as O
 
@@ -134,28 +127,25 @@ def test_row_gradient_kernel_variants(combo, shape):
     go = torch.randn(n, generator=g)
     xd, yd, hd, wd, god = (t.to(DEV) for t in (x, y, h, w, go))
     center = ops.default_center(xd, yd)
-    tol = 5e-5 if combo.startswith("2") else 2.0**-12
-    with env(B200OT_TC_BWD=combo):
-        for eps in (2.0, 0.3):
-            _, lse2 = ops.softmin_raw(eps, xd, yd, hd, p=2, center=center, want_lse2=True)
-            ref = O.softmin_grad_rows(eps, x.double(), y.double(), h.double(), go.double(), p=2).numpy()
-            gx = ops.softmin_grad_rows(eps, xd, yd, hd, None, 0.0, lse2, god, p=2, center=center)
-            np.testing.assert_allclose(gx.cpu().numpy(), ref, atol=tol * max(1.0, np.abs(ref).max()),
-                                       err_msg=f"softmin eps={eps}")
-        for blur in (2.0, 0.7):
-            xr = x.double().requires_grad_(True)
-            km = O.kernel_matrix("gaussian", xr, y.double(), blur)
-            (ref,) = torch.autograd.grad(km @ w.double(), xr, go.double())
-            # natural scale of the gradient (its terms cancel in the sum): sum_j w_j k_ij |y_j - x_i| / blur^2
-            gscale = ((km.detach() @ w.double()) * go.double().abs()).max().item() * np.sqrt(d) / blur**2
-            gx = ops.kernel_conv_grad_rows("gaussian", xd, yd, wd, blur, god, center=center)
-            np.testing.assert_allclose(gx.cpu().numpy(), ref.numpy(),
-                                       atol=tol * ref.abs().max().item() + 1e-5 * gscale, err_msg=f"gaussian blur={blur}")
+    for eps in (2.0, 0.3):
+        _, lse2 = ops.softmin_raw(eps, xd, yd, hd, p=2, center=center, want_lse2=True)
+        ref = O.softmin_grad_rows(eps, x.double(), y.double(), h.double(), go.double(), p=2).numpy()
+        gx = ops.softmin_grad_rows(eps, xd, yd, hd, None, 0.0, lse2, god, p=2, center=center)
+        np.testing.assert_allclose(gx.cpu().numpy(), ref, atol=5e-5 * max(1.0, np.abs(ref).max()),
+                                   err_msg=f"softmin eps={eps}")
+    for blur in (2.0, 0.7):
+        xr = x.double().requires_grad_(True)
+        km = O.kernel_matrix("gaussian", xr, y.double(), blur)
+        (ref,) = torch.autograd.grad(km @ w.double(), xr, go.double())
+        # natural scale of the gradient (its terms cancel in the sum): sum_j w_j k_ij |y_j - x_i| / blur^2
+        gscale = ((km.detach() @ w.double()) * go.double().abs()).max().item() * np.sqrt(d) / blur**2
+        gx = ops.kernel_conv_grad_rows("gaussian", xd, yd, wd, blur, god, center=center)
+        np.testing.assert_allclose(gx.cpu().numpy(), ref.numpy(),
+                                   atol=5e-5 * ref.abs().max().item() + 1e-5 * gscale, err_msg=f"gaussian blur={blur}")
 
 
-@pytest.mark.parametrize("combo", ["2,8,0,0", "2,8,0,1", "2,16,0,1"])
 @pytest.mark.parametrize("shape", [(700, 900, 3), (1300, 800, 8), (300, 500, 16), (1000, 2100, 64)])
-def test_value_and_unit_gradient_in_one_pass(combo, shape):
+def test_value_and_unit_gradient_in_one_pass(shape):
     """b200ot_kernel_conv_fwd_bwd_x: out = K(x, y) w and the unit row gradient from one reduction, CUDA-core and
     tensor-core dimensions, cross and self terms (the exact zero exponent of the diagonal included)."""
     from geomloss_b200 import ops
@@ -167,19 +157,18 @@ def test_value_and_unit_gradient_in_one_pass(combo, shape):
     w, a = torch.rand(m, generator=g) / m, torch.rand(n, generator=g) / n
     xd, yd, wd, ad = (t.to(DEV) for t in (x, y, w, a))
     blurs = (2.0, 0.7) if d > 8 else (0.5, 0.1)
-    with env(B200OT_TC_BWD=combo):
-        for blur in blurs:
-            for cols, wts, cd, wdv in ((y, w, yd, wd), (x, a, xd, ad)):  # cross term, self term (same buffer)
-                center = ops.default_center(xd, cd)
-                xr = x.double().requires_grad_(True)
-                ref = O.kernel_matrix("gaussian", xr, cols.double(), blur) @ wts.double()
-                (gref,) = torch.autograd.grad(ref.sum(), xr)
-                out, gunit = ops.kernel_conv_value_and_grad_rows("gaussian", xd, cd, wdv, blur, center=center)
-                slack = np.log(2.0) * _exponent_slack(d, np.sqrt(np.log2(np.e)) / blur)
-                np.testing.assert_allclose(out.cpu().numpy(), ref.detach().numpy(), rtol=2e-5 + slack, atol=1e-30)
-                gscale = ref.detach().max().item() * np.sqrt(d) / blur**2  # natural scale, as above
-                np.testing.assert_allclose(gunit.cpu().numpy(), gref.numpy(),
-                                           atol=5e-5 * gref.abs().max().item() + (2e-5 + slack) * gscale)
+    for blur in blurs:
+        for cols, wts, cd, wdv in ((y, w, yd, wd), (x, a, xd, ad)):  # cross term, self term (same buffer)
+            center = ops.default_center(xd, cd)
+            xr = x.double().requires_grad_(True)
+            ref = O.kernel_matrix("gaussian", xr, cols.double(), blur) @ wts.double()
+            (gref,) = torch.autograd.grad(ref.sum(), xr)
+            out, gunit = ops.kernel_conv_value_and_grad_rows("gaussian", xd, cd, wdv, blur, center=center)
+            slack = np.log(2.0) * _exponent_slack(d, np.sqrt(np.log2(np.e)) / blur)
+            np.testing.assert_allclose(out.cpu().numpy(), ref.detach().numpy(), rtol=2e-5 + slack, atol=1e-30)
+            gscale = ref.detach().max().item() * np.sqrt(d) / blur**2  # natural scale, as above
+            np.testing.assert_allclose(gunit.cpu().numpy(), gref.numpy(),
+                                       atol=5e-5 * gref.abs().max().item() + (2e-5 + slack) * gscale)
     if d == 64:
         # BASELINE configs[2] regime: the value of the self term is its diagonal, which the kernel takes exactly
         out, _ = ops.kernel_conv_value_and_grad_rows("gaussian", xd, xd, torch.ones(n, device=DEV), 0.05,

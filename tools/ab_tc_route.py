@@ -1,14 +1,12 @@
-"""A/B timing of the routing / tuning knobs of the tensor-core kernels, inside ONE process and ONE build of the library
+"""A/B timing of the routing knobs of the tensor-core kernels, inside ONE process and ONE build of the library
 (the knobs are environment variables the C entry points read on every call):
 
   part A  CUDA-core vs tensor-core path for D <= 8 (B200OT_TC_MIN_D / B200OT_TC_MIN_PAIRS), per operator and size —
           the cross-over that csrc/b200ot_kernel_conv.cu::kTcMinDimDefault encodes;
-  part B  row-gradient kernel variants at D = 16 / 64 (B200OT_TC_BWD = "p_terms,epi_warps,ldall,merge";
-          on sm_90a p_terms and merge select the kernel);
   part C  value + unit gradient in one pass (b200ot_kernel_conv_fwd_bwd_x) against the two separate reductions;
-  part D  BASELINE configs[2] (gaussian MMD, N = M = 1e6, D = 64, forward + gradient) with the settings B and C favour.
+  part D  BASELINE configs[2] (gaussian MMD, N = M = 1e6, D = 64, forward + gradient), two-pass and one-pass.
 
-Every variant's result is compared with the default path's result on the same inputs (and, for part B/C, with an fp64
+Every variant's result is compared with the default path's result on the same inputs (and, for part C, with an fp64
 brute force on sampled rows).  One JSON line per measurement.
 
     python tools/ab_tc_route.py [--quick] > ab_tc_route.jsonl
@@ -59,11 +57,7 @@ SIMT = dict(B200OT_TC_MIN_D="9", B200OT_TC_MIN_PAIRS="0")
 TC = dict(B200OT_TC_MIN_D="1", B200OT_TC_MIN_PAIRS="0")
 
 
-RESULTS = []
-
-
 def emit(**kw):
-    RESULTS.append(kw)
     print(json.dumps(kw), flush=True)
 
 
@@ -114,42 +108,6 @@ def brute_rows(x, y, w, blur, rows):
     return val, grad
 
 
-def part_b(dev, N, dims, reps):
-    g = torch.Generator().manual_seed(1)
-    M = N
-    combos = ["2,8,0,0", "2,8,0,1", "1,8,0,0", "1,8,0,1"]
-    for D in dims:
-        x = torch.rand(N, D, generator=g).to(dev)
-        y = torch.rand(M, D, generator=g).to(dev)
-        h = (torch.rand(M, generator=g) * 0.1).to(dev)
-        w = (torch.rand(M, generator=g) / M).to(dev)
-        go = torch.rand(N, generator=g).to(dev)
-        ones = torch.ones(N, device=dev)
-        blur = 0.25 * (D / 3.0) ** 0.5  # kernel values of all sizes: the gradient is not just the nearest neighbour
-        eps = blur * blur
-        center = ops.default_center(x, y)
-        _, lse2 = ops.softmin_raw(eps, x, y, h, p=2, want_lse2=True, center=center)
-        rows = torch.randint(0, N, (64,), generator=g).to(dev)
-        _, gref = brute_rows(x, y, w, blur, rows)
-        base = {}
-        for combo in combos:
-            with env(B200OT_TC_BWD=combo):
-                for name, fn in (
-                    ("conv_bwd", lambda: ops.kernel_conv_grad_rows("gaussian", x, y, w, blur, go, center=center)),
-                    ("softmin_bwd", lambda: ops.softmin_grad_rows(eps, x, y, h, None, 0.0, lse2, go, p=2,
-                                                                  center=center)),
-                ):
-                    ms = best_ms(fn, reps)
-                    out = fn()
-                    base.setdefault(name, out)
-                    rec = dict(part="B", op=name, D=D, N=N, combo=combo, ms=round(ms, 3),
-                               Tpairs_s=round(N * M / ms * 1e-9, 3), vs_default_relmax=relmax(out, base[name]))
-                    if name == "conv_bwd":
-                        gu = ops.kernel_conv_grad_rows("gaussian", x, y, w, blur, ones, center=center)[rows].double()
-                        rec["vs_fp64_relmax_64rows"] = relmax(gu, gref)
-                    emit(**rec)
-
-
 def part_c(dev, N, dims, reps):
     g = torch.Generator().manual_seed(2)
     M = N
@@ -164,42 +122,32 @@ def part_c(dev, N, dims, reps):
         for self_term in (False, True):
             yy, ww = (x, (torch.rand(N, generator=g) / N).to(dev)) if self_term else (y, w)
             vref, gref = brute_rows(x, yy, ww, blur, rows)
-            for combo in ("2,8,0,0", "2,8,0,1", "1,8,0,1"):
-                with env(B200OT_TC_BWD=combo):
-                    t_two = best_ms(lambda: (ops.kernel_conv_raw("gaussian", x, yy, ww, blur, center=center),
-                                             ops.kernel_conv_grad_rows("gaussian", x, yy, ww, blur, ones,
-                                                                       center=center)), reps)
-                    t_one = best_ms(lambda: ops.kernel_conv_value_and_grad_rows("gaussian", x, yy, ww, blur,
-                                                                                center=center), reps)
-                    v2 = ops.kernel_conv_raw("gaussian", x, yy, ww, blur, center=center)
-                    g2 = ops.kernel_conv_grad_rows("gaussian", x, yy, ww, blur, ones, center=center)
-                    v1, g1 = ops.kernel_conv_value_and_grad_rows("gaussian", x, yy, ww, blur, center=center)
-                emit(part="C", D=D, N=N, self_term=self_term, combo=combo, two_pass_ms=round(t_two, 3),
-                     one_pass_ms=round(t_one, 3), value_vs_fwd_relmax=relmax(v1, v2), grad_vs_bwd_relmax=relmax(g1, g2),
-                     value_vs_fp64_relmax_64rows=relmax(v1[rows].double(), vref),
-                     fwd_value_vs_fp64_relmax_64rows=relmax(v2[rows].double(), vref),
-                     grad_vs_fp64_relmax_64rows=relmax(g1[rows].double(), gref))
+            t_two = best_ms(lambda: (ops.kernel_conv_raw("gaussian", x, yy, ww, blur, center=center),
+                                     ops.kernel_conv_grad_rows("gaussian", x, yy, ww, blur, ones, center=center)), reps)
+            t_one = best_ms(lambda: ops.kernel_conv_value_and_grad_rows("gaussian", x, yy, ww, blur, center=center),
+                            reps)
+            v2 = ops.kernel_conv_raw("gaussian", x, yy, ww, blur, center=center)
+            g2 = ops.kernel_conv_grad_rows("gaussian", x, yy, ww, blur, ones, center=center)
+            v1, g1 = ops.kernel_conv_value_and_grad_rows("gaussian", x, yy, ww, blur, center=center)
+            emit(part="C", D=D, N=N, self_term=self_term, two_pass_ms=round(t_two, 3),
+                 one_pass_ms=round(t_one, 3), value_vs_fwd_relmax=relmax(v1, v2), grad_vs_bwd_relmax=relmax(g1, g2),
+                 value_vs_fp64_relmax_64rows=relmax(v1[rows].double(), vref),
+                 fwd_value_vs_fp64_relmax_64rows=relmax(v2[rows].double(), vref),
+                 grad_vs_fp64_relmax_64rows=relmax(g1[rows].double(), gref))
         # the configs[2] regime (blur = .05 at D = 64: the loss IS the diagonal of K_xx): value from the one-pass kernel
         if D == 64:
             a = torch.full((N,), 1.0 / N, device=dev)
             v2 = ops.kernel_conv_raw("gaussian", x, x, a, 0.05, center=center)
-            for combo in ("2,8,0,0", "2,8,0,1", "1,8,0,1"):
-                with env(B200OT_TC_BWD=combo):
-                    v1, _ = ops.kernel_conv_value_and_grad_rows("gaussian", x, x, a, 0.05, center=center)
-                emit(part="C", D=D, N=N, regime="configs[2] blur=.05 self term", combo=combo,
-                     value_vs_fwd_relmax=relmax(v1, v2), value_vs_exact_diag_relmax=relmax(v1, a))
+            v1, _ = ops.kernel_conv_value_and_grad_rows("gaussian", x, x, a, 0.05, center=center)
+            emit(part="C", D=D, N=N, regime="configs[2] blur=.05 self term", value_vs_fwd_relmax=relmax(v1, v2),
+                 value_vs_exact_diag_relmax=relmax(v1, a))
 
 
 def part_d(dev, N, reps):
     """BASELINE configs[2] itself: SamplesLoss("gaussian", blur=.05) on N = M = 1e6, D = 64, forward + gradient w.r.t. x,
-    with the two-pass and the one-pass evaluation and the fastest row-gradient variants part B found."""
+    with the two-pass and the one-pass evaluation."""
     from geomloss_b200 import SamplesLoss
 
-    def best_combo(pred):
-        rows = [r for r in RESULTS if r.get("part") == "B" and r["op"] == "conv_bwd" and r["D"] == 64 and pred(r["combo"])]
-        return min(rows, key=lambda r: r["ms"])["combo"] if rows else "2,8,0,0"
-
-    exact, any_ = best_combo(lambda c: c.startswith("2")), best_combo(lambda c: True)
     g = torch.Generator().manual_seed(0)
     x = torch.rand(N, 64, generator=g).to(dev)
     y = torch.rand(N, 64, generator=g).to(dev)
@@ -213,16 +161,10 @@ def part_d(dev, N, reps):
 
     t_fwd = best_ms(lambda: L(x, y), reps)
     emit(part="D", what="forward only (3 reductions)", N=N, ms=round(t_fwd, 2), Tpairs_s=round(3.0 * N * N / t_fwd * 1e-9, 3))
-    settings = [("two-pass, default kernel", False, "2,8,0,0"), ("one-pass, default kernel", True, "2,8,0,0")]
-    if exact != "2,8,0,0":
-        settings.append((f"one-pass, best PT=2 variant {exact}", True, exact))
-    if any_ not in ("2,8,0,0", exact):
-        settings.append((f"one-pass, best variant {any_}", True, any_))
-    for label, fused, combo in settings:
+    for label, fused in (("two-pass", False), ("one-pass", True)):
         ops.FUSED_CONV_GRAD = fused
-        with env(B200OT_TC_BWD=combo):
-            ms = best_ms(fwd_bwd, reps)
-            v = fwd_bwd().item()
+        ms = best_ms(fwd_bwd, reps)
+        v = fwd_bwd().item()
         emit(part="D", what=label, N=N, fwd_bwd_ms=round(ms, 2), value=v)
     ops.FUSED_CONV_GRAD = False
 
@@ -249,12 +191,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--quick", action="store_true", help="small sizes (functional check of the script)")
     ap.add_argument("--reps", type=int, default=2)
-    ap.add_argument("--parts", default="BCDEA")
+    ap.add_argument("--parts", default="CDEA")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     big = 20000 if args.quick else 400000
-    if "B" in args.parts:
-        part_b(dev, big, (16, 64), args.reps)
     if "C" in args.parts:
         part_c(dev, big, (3, 64), args.reps)
     if "D" in args.parts:

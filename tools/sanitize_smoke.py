@@ -132,7 +132,7 @@ if "tc" in which:
             (gx,) = torch.autograd.grad(out.sum(), xg)
             assert torch.isfinite(gx).all()
 if "batched" in which:
-    # the batched tensor-core kernels (tc_reduce_kernel<0/1/4/5, BATCH>, tc_bwd_kernel<2/3/4/5, ..., BATCH>), each
+    # the batched tensor-core kernels (tc_reduce_kernel<0/1/4/5, BATCH>, tc_bwd_kernel<2/3/4/5, dk, BATCH>), each
     # element checked against its own columns
     B, n = 3, 300
     for d in (16, 64):
@@ -156,7 +156,7 @@ if "batched" in which:
         check(f"batched_conv_value_d{d}", val, ((-d2 / 8.0).exp() @ w.double()[:, :, None])[..., 0], 1e-4)
         assert torch.isfinite(gu).all()
 if "l1" in which:
-    # the p = 1 softmin (tc_reduce_kernel<6, BATCH>, tc_bwd_kernel<7, 2, MERGE, dk, BATCH> at every dk)
+    # the p = 1 softmin (tc_reduce_kernel<6, BATCH>, tc_bwd_kernel<7, dk, BATCH> at every dk)
     B, n = 2, 300
     for d in (16, 32, 48, 64):
         x, y, h = torch.rand(B, n, d, generator=g), torch.rand(B, n, d, generator=g), torch.randn(B, n, generator=g)
@@ -194,8 +194,8 @@ if "wide" in which:
             gx = ops.kernel_conv_wide_grad_rows(kind, xd, yd, wd, 2.0, ones, center=center)
             assert torch.isfinite(gx).all()
 if "blocks" in which:
-    # the block-sparse tensor-core softmins (tc_reduce_kernel<1, false, BLOCKS>, tc_bwd_kernel<3, 2, true, dk, false,
-    # BLOCKS>): clusters of 1, 127, 128, 129 and 300 points, a row cluster that keeps nothing, a self problem
+    # the block-sparse tensor-core softmins (tc_reduce_kernel<1, false, BLOCKS>, tc_bwd_kernel<3, dk, false, BLOCKS>):
+    # clusters of 1, 127, 128, 129 and 300 points, a row cluster that keeps nothing, a self problem
     for d in (16, 64):
         rc, cc = torch.tensor([1, 129, 300, 128]), torch.tensor([127, 1, 300, 129, 128])
         keep = torch.rand(4, 5, generator=g) < 0.6
