@@ -65,27 +65,50 @@ __global__ void softmin_finalize_kernel(const float2* __restrict__ part, int n_p
 // -------------------------------------------------------------------------------------------------
 // dispatch
 // -------------------------------------------------------------------------------------------------
-// 2 rows/thread, 3 CTAs/SM (2 for D > 4), sum-guarded lazy max.  What matters is the length of the straight-line chunk
-// between two max checks: longer chunks give the scheduler more independent MUFU work, but cost registers, and on a
-// short column shard (multi-GPU) the tail of the last chunk.  16 column pairs at D = 3, 4 (the exponent is MUFU-bound
-// and needs no FMA-pipe off-load), 8 pairs with one polynomial exp2 in eight at D = 1, 2 (so little FMA work per pair
-// that the off-load pays), 8 pairs at D >= 5 (2 CTAs/SM: no registers to spare); p = 1 (DIRECT) always takes 16.
-// These choices are not re-tuned for H100; tools/ab_ops.py times the alternatives (B200OT_BIG_CH / B200OT_BIG_POLY).
-// Ranges mode keeps 8-pair chunks: its pieces must be multiples of 2*CH columns, and 16-slot cluster padding
+// Dense big shape: sum-guarded lazy max, 512 rows per CTA (the plan's kBigNT * kBigR) split as NT threads x R rows.
+// What matters is the length of the straight-line chunk between two max checks (longer chunks give the scheduler more
+// independent MUFU work, but cost registers, and on a short column shard the tail of the last chunk) and, at D = 3, 4,
+// how many shared-memory packet loads feed one MUFU.EX2: both go through the MIO queue.
+//   D = 3, p = 2:  4 rows x 128 threads, 32-pair chunks, 4 CTAs/SM (94 registers);
+//   D = 4, p = 2:  2 rows x 256 threads, 32-pair chunks, 3 CTAs/SM, 2-stage ring;
+//   D = 1, 2:      2 x 256, 8 pairs with one polynomial exp2 in eight (so little FMA work per pair that it pays);
+//   D >= 5:        2 x 256, 8 pairs, 2 CTAs/SM (no registers to spare); p = 1 (DIRECT) 2 x 256, 16 pairs.
+// D = 3, 4 were chosen on an H100 SXM (700 W) by tools/bench_softmin_sm90.py: 0.85 / 0.75 of the MUFU.EX2 rate at the
+// sampled clock, against 0.81 / 0.72 for the 2 x 256 / 16-pair / 3-CTA shape; an FMA-pipe share of the exponentials
+// (ex2_poly2) was slower at every shape tried (DESIGN.md §3.1 has the sweep).
+// Ranges mode keeps 2 x 256 and 8-pair chunks: its pieces must be multiples of 2*CH columns, and 16-slot cluster padding
 // (kRangesAlign) costs less than the longer chunk gains on cluster-sized pieces.
+// A/B builds (tools/ab_ops.py, tools/bench_softmin_sm90.py) override the dense shape with -DB200OT_BIG_CH (every D),
+// -DB200OT_BIG_POLY (D <= 4, p = 2), -DB200OT_BIG_R / _MINB / _STAGES (D = 3, 4, p = 2).
 template <int D, int P, bool DIRECT>
 struct Variants {
-#ifdef B200OT_BIG_CH  // A/B builds (tools/ab_ops.py)
-#ifndef B200OT_BIG_POLY
-#define B200OT_BIG_POLY 0u
-#endif
+  static constexpr bool kD34 = (D == 3 || D == 4) && P == 2 && !DIRECT;
+#ifdef B200OT_BIG_CH
   static constexpr int kCH = B200OT_BIG_CH;
+#else
+  static constexpr int kCH = (DIRECT || D == 3 || D == 4) ? (kD34 ? 32 : 16) : 8;
+#endif
+#ifdef B200OT_BIG_POLY
   static constexpr unsigned kPoly = (D <= 4 && P == 2 && !DIRECT) ? B200OT_BIG_POLY : 0u;
 #else
-  static constexpr int kCH = (DIRECT || D == 3 || D == 4) ? 16 : 8;
   static constexpr unsigned kPoly = (D <= 2 && P == 2 && !DIRECT) ? 0x01u : 0u;
 #endif
-  using Big = SoftminCfg<D, kBigR, P, DIRECT, kPoly, kBigNT, kBigTJ, 3, kCH, (D <= 4 ? 3 : 2), true>;
+#ifdef B200OT_BIG_R
+  static constexpr int kR = kD34 ? B200OT_BIG_R : kBigR;
+#else
+  static constexpr int kR = (kD34 && D == 3) ? 4 : kBigR;
+#endif
+#ifdef B200OT_BIG_MINB
+  static constexpr int kMinB = kD34 ? B200OT_BIG_MINB : (D <= 4 ? 3 : 2);
+#else
+  static constexpr int kMinB = (kD34 && D == 3) ? 4 : (D <= 4 ? 3 : 2);
+#endif
+#ifdef B200OT_BIG_STAGES
+  static constexpr int kStages = kD34 ? B200OT_BIG_STAGES : 3;
+#else
+  static constexpr int kStages = (kD34 && D == 4) ? 2 : 3;
+#endif
+  using Big = SoftminCfg<D, kR, P, DIRECT, kPoly, kBigNT * kBigR / kR, kBigTJ, kStages, kCH, kMinB, true>;
   using BigRanges = SoftminCfg<D, kBigR, P, DIRECT, 0u, kBigNT, kBigTJ, 3, 8, (D <= 4 ? 3 : 2), true>;
   using Small = SoftminCfg<D, kSmallR, P, DIRECT, 0u, kSmallNT, kSmallTJ, 3, 4, 4, true>;
   static_assert(2 * BigRanges::CH <= kRangesAlign && 2 * Small::CH <= kRangesAlign,
@@ -96,8 +119,8 @@ template <class C, class CR = C>
 static int launch_partial(const float* x, const float* center, float scale, float clampq, const float* cols,
                           float* part, const ReducePlan& pl, int64_t N, cudaStream_t st, const int4* seg,
                           const int2* pieces) {
-  static_assert(C::SMEM_BYTES == CR::SMEM_BYTES && C::NT == CR::NT && C::ROWS_PER_CTA == CR::ROWS_PER_CTA,
-                "dense and ranges instantiations share one ReducePlan");
+  // the plan fixes rows per CTA and the shared-memory opt-in; the CTA shape (NT x R) may differ
+  static_assert(C::ROWS_PER_CTA == CR::ROWS_PER_CTA && C::TJ == CR::TJ, "dense and ranges instantiations share one ReducePlan");
   if (seg != nullptr)
     return launch_reduce<CR>(softmin_partial_kernel<CR, true>, pl, st, x, center, scale, clampq, cols,
                              reinterpret_cast<float2*>(part), N, pl.ntiles, pl.tiles_per_split, 0, seg, pieces);

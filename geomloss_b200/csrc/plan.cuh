@@ -8,13 +8,13 @@
 namespace b200ot {
 
 // Tile shapes (must match the Cfg instantiations in the .cu files):
-//   big   : 256 consumer threads x 2 rows, 1024-column tiles, 2 CTAs / SM
+//   big   : 512 rows (256 consumer threads x 2 rows; the dense D = 3 softmin: 128 x 4), 1024-column tiles
 //   small : 128 consumer threads x 1 row,   256-column tiles  — a few thousand points still spread
 //           over every SM (132 on an H100 SXM)
 constexpr int kBigNT = 256, kBigR = 2, kBigTJ = 1024;
 constexpr int kSmallNT = 128, kSmallR = 1, kSmallTJ = 256;
 constexpr int kPackPad = 1024;  // packed column buffers are padded to this many columns
-constexpr int kPlanWaves = 16;  // waves (of 2 CTAs/SM) a launch is cut into when the problem is large enough
+constexpr int kPlanWaves = 16;  // waves (counted as 2 CTAs/SM) a launch is cut into when the problem is large enough
 
 struct ReducePlan {
   int tj;        // columns per tile
@@ -33,7 +33,8 @@ struct ReducePlan {
 // Column splits: as FEW as fill the machine for ~16 waves of 2 CTAs/SM (the SM count is read from the device).  A
 // partial last wave costs little once the CTAs drift out of lock-step, while every extra CTA costs its prologue and a
 // cold TMA ring — which matters most on the short column shards of the multi-GPU engine.
-// consumers visit whole chunks: 32 columns = 16 column pairs, the longest chunk of any dense instantiation
+// consumers visit whole chunks: 32 columns = 16 column pairs.  The D = 3, 4 softmin runs 32-pair chunks and may read up
+// to 16 pairs past last_pairs — neutral padding of the same tile, which the producer always loads whole
 constexpr int kTailAlign = 32;
 
 // Test hook ($B200OT_FORCE_SPLITS, tools/sanitize_smoke.py and the streaming tests): force the number of column splits of

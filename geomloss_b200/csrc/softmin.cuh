@@ -282,12 +282,14 @@ __global__ void __launch_bounds__(C::NT + 32, C::MINB)
 
 #pragma unroll 1
     for (int jp = 0; jp < npairs; jp += CH) {
-      // speculative pass: exponentials against the (possibly stale) max, chunk max on the side
+      // speculative pass: exponentials against the (possibly stale) max, chunk max on the side.  p = 2: the chunk sum
+      // starts from the first column pair's terms (no 0 + e); p = 1 keeps the zero start (measured 2 % faster at D = 1, 2)
+      constexpr bool kFirst = !C::DIRECT;
       float2 cs[R];
       float cm[R];
 #pragma unroll
       for (int r = 0; r < R; ++r) {
-        cs[r] = dup2(0.f);
+        if (!kFirst) cs[r] = dup2(0.f);
         cm[r] = kNegBig;
       }
 #pragma unroll
@@ -306,7 +308,7 @@ __global__ void __launch_bounds__(C::NT + 32, C::MINB)
             e.x = ex2_approx(a.x);
             e.y = ex2_approx(a.y);
           }
-          cs[r] = fadd2(cs[r], e);
+          cs[r] = (kFirst && c == 0) ? e : fadd2(cs[r], e);
         }
       }
 #pragma unroll
