@@ -19,7 +19,6 @@
 #include <stdlib.h>
 
 #include <algorithm>
-#include <type_traits>
 #include <vector>
 
 namespace b200ot {
@@ -144,39 +143,6 @@ __global__ void coord_absmax_kernel(const float* __restrict__ a, int64_t na, con
   if ((threadIdx.x & 31) == 0 && m > 0.f && !(m != m)) atomicMax(reinterpret_cast<unsigned int*>(out), __float_as_uint(m));
 }
 
-template <int MODE, int D>
-static int launch_rowsum(const ReducePlan& pl, cudaStream_t st, const float* x, const float* center, float scale,
-                         float clampq, const float* cols, float* part, int64_t N, const int4* seg = nullptr,
-                         const int2* pieces = nullptr) {
-  if (pl.small) {
-    using C = RowSumCfg<MODE, D, kSmallR, kSmallNT, kSmallTJ, 3, 4>;
-    return launch_rowsum_kernel<C>(pl, st, x, center, scale, clampq, cols,
-                            (const float*)nullptr, part, N, pl.ntiles, pl.tiles_per_split, seg, pieces);
-  }
-  // D >= 5: one row per thread (same 512 rows per CTA) keeps the 2 x (D+1) accumulator pairs in registers
-  using C = std::conditional_t<(D <= 4), RowSumCfg<MODE, D, kBigR, kBigNT, kBigTJ, 3, 2>,
-                               RowSumCfg<MODE, D, 1, kBigR * kBigNT, kBigTJ, 3, 1>>;
-  return launch_rowsum_kernel<C>(pl, st, x, center, scale, clampq, cols, (const float*)nullptr,
-                          part, N, pl.ntiles, pl.tiles_per_split, seg, pieces);
-}
-
-template <int MODE>
-static int launch_rowsum_d(int D, const ReducePlan& pl, cudaStream_t st, const float* x, const float* center,
-                           float scale, float clampq, const float* cols, float* part, int64_t N,
-                           const int4* seg = nullptr, const int2* pieces = nullptr) {
-  switch (D) {
-    case 1: return launch_rowsum<MODE, 1>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 2: return launch_rowsum<MODE, 2>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 3: return launch_rowsum<MODE, 3>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 4: return launch_rowsum<MODE, 4>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 5: return launch_rowsum<MODE, 5>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 6: return launch_rowsum<MODE, 6>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 7: return launch_rowsum<MODE, 7>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    case 8: return launch_rowsum<MODE, 8>(pl, st, x, center, scale, clampq, cols, part, N, seg, pieces);
-    default: return B200OT_EINVAL;
-  }
-}
-
 static int conv_pack(const float* y, const float* w, const float* center, int64_t M, int D, const ConvScales& cs,
                      float* cols, cudaStream_t st, const int* src = nullptr) {
   const int nf2 = colfmt_nf2(D, cs.extra);
@@ -193,14 +159,15 @@ static int conv_partial(int kind_flags, bool bwd, const ReducePlan& pl, cudaStre
                         const float* center, const ConvScales& cs, const float* cols, float* part, int64_t N, int D,
                         const int4* seg = nullptr, const int2* pieces = nullptr) {
   const int kind = kind_base(kind_flags);
+  const float s = cs.scale, c = cs.clampq;
   if (kind == B200OT_KERNEL_GAUSSIAN)
-    return bwd ? launch_rowsum_d<kGaussBwd>(D, pl, st, x, center, cs.scale, cs.clampq, cols, part, N, seg, pieces)
-               : launch_rowsum_d<kGaussFwd>(D, pl, st, x, center, cs.scale, cs.clampq, cols, part, N, seg, pieces);
+    return bwd ? launch_rowsum_d<kGaussBwd>(D, pl, st, x, center, s, c, cols, nullptr, part, N, seg, pieces)
+               : launch_rowsum_d<kGaussFwd>(D, pl, st, x, center, s, c, cols, nullptr, part, N, seg, pieces);
   if (kind == B200OT_KERNEL_LAPLACIAN)
-    return bwd ? launch_rowsum_d<kLaplaceBwd>(D, pl, st, x, center, cs.scale, cs.clampq, cols, part, N, seg, pieces)
-               : launch_rowsum_d<kLaplaceFwd>(D, pl, st, x, center, cs.scale, cs.clampq, cols, part, N, seg, pieces);
-  return bwd ? launch_rowsum_d<kEnergyBwd>(D, pl, st, x, center, cs.scale, cs.clampq, cols, part, N, seg, pieces)
-             : launch_rowsum_d<kEnergyFwd>(D, pl, st, x, center, cs.scale, cs.clampq, cols, part, N, seg, pieces);
+    return bwd ? launch_rowsum_d<kLaplaceBwd>(D, pl, st, x, center, s, c, cols, nullptr, part, N, seg, pieces)
+               : launch_rowsum_d<kLaplaceFwd>(D, pl, st, x, center, s, c, cols, nullptr, part, N, seg, pieces);
+  return bwd ? launch_rowsum_d<kEnergyBwd>(D, pl, st, x, center, s, c, cols, nullptr, part, N, seg, pieces)
+             : launch_rowsum_d<kEnergyFwd>(D, pl, st, x, center, s, c, cols, nullptr, part, N, seg, pieces);
 }
 
 static float conv_bwd_coef(int kind_flags, const ConvScales& cs, float blur) {
@@ -210,13 +177,14 @@ static float conv_bwd_coef(int kind_flags, const ConvScales& cs, float blur) {
   return -1.0f;
 }
 
+
 // ---------------------------------------------------------------------------------------------------
 // tensor-core path (gaussian, and laplacian / energy for 8 < D <= 64): see tcconv.cuh
 // ---------------------------------------------------------------------------------------------------
-// A launch group: `ctas` x n_split CTAs over a_tiles row images and b_tiles column images, then the partials and a misc
-// block in the scratch
+// A launch group: `ctas` x n_split x slices CTAs over a_tiles row images and b_tiles column images, then the partials
+// and a misc block in the scratch
 struct TcPlan {
-  int kp, nstage, n_split, tiles_per_split;
+  int kp, nstage, n_split, tiles_per_split, slices;
   int rtpe, ctpe;  // row / column tiles per batch element (0 for a block-sparse problem)
   int64_t a_tiles, b_tiles, ctas, smem;
   int64_t off_b, off_part, off_misc, total;
@@ -270,18 +238,18 @@ bool tc_any_routed(int D, int64_t N, int64_t M) {
 // The plan of a launch group: `ctas` row CTAs, each reading up to `tiles` (>= 1) column tiles.  The split count is
 // chosen for the whole grid and cuts those tiles.  Behind the images: the partials of `rows` rows ((m, s) pairs forward, D+1
 // sums per row backward, D+2 for the p = 1 softmin: `head` sums ahead of the D), then a misc block of misc_bytes.
-// `slices` > 0: the K-slab ring of the kernels above D = 64 (tcwide.cuh), whose row gradients run `slices` CTAs per
-// row tile and split.
+// Above D = 64 the K-slab ring of tcwide.cuh, whose row gradients run `slices` CTAs per row tile and split.
 static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, int64_t ctas, int64_t tiles, int64_t rows,
-                           int64_t misc_bytes, int head = 1, int slices = 0) {
+                           int64_t misc_bytes, int head = 1, int slices = 1) {
   TcPlan p;
   p.kp = tc_kp(D);
+  p.slices = slices;
   p.rtpe = p.ctpe = 0;
   p.a_tiles = a_tiles;
   p.b_tiles = b_tiles;
   p.ctas = ctas;
   const int64_t b_bytes = tc_b_img_bytes(p.kp, kTcBN);
-  if (slices > 0) {
+  if (D > 64) {
     // row tail, column tails and slab ring (tcwide.cuh): as many stages as fit, whatever D
     int ns = kTcMaxStage;
     while (ns > 0 && tc_wide_smem(ns) > 227 * 1024) --ns;
@@ -295,7 +263,7 @@ static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, in
     p.nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
     p.smem = tc_a_span(p.kp) + p.nstage * b_bytes + bar_bytes;
   }
-  int64_t want = ceil_div64((int64_t)num_sms() * 4, ctas * std::max(slices, 1));
+  int64_t want = ceil_div64((int64_t)num_sms() * 4, ctas * slices);
   const int forced = forced_splits();  // test hook (plan.cuh)
   if (forced > 0) want = forced;
   if (want < 1) want = 1;
@@ -312,23 +280,32 @@ static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, in
 
 // B problems of N rows x M columns side by side (B = 1: one problem), each element padded to whole tiles on its own
 // (tc_pack_kernel).  The splits cut each element's ctpe column tiles, so a CTA never reads another element's columns.
-// Misc block: [0] the energy coordinate maximum, [1 + b] max|w| of element b.
+// Above D = 64 the row gradients run one slice per K slab.  Misc block: [0] the energy coordinate maximum, [1 + b]
+// max|w| of element b.
 static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B = 1, int head = 1) {
   const int rtpe = (int)ceil_div64(N, kTcM), ctpe = (int)ceil_div64(M, kTcBN);
-  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4, head);
+  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4, head,
+                          bwd && D > 64 ? tc_wide_slabs(D) : 1);
   p.rtpe = rtpe;
   p.ctpe = ctpe;
   return p;
 }
 
-int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
+int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B, int head) {
   // forward and row-gradient launches split the columns differently: size for the larger of the two
-  return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B).total);
+  return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B, head).total);
 }
 
-// the p = 1 softmin's row gradient keeps D + 2 sums per row
-int64_t tc_l1_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
-  return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B, 2).total);
+// The plan of one block-sparse problem: a CTA per segment, images of n_row_slots / n_col_slots points, segments cut
+// into splits from the longest one.  Misc block: the segment descriptors, then the pieces.
+static int64_t tc_blocks_seg_bytes(int64_t n_seg) { return round_up64(n_seg * 16, 256); }
+static TcPlan make_tc_blocks_plan(int64_t N, int D, bool bwd, const TcBlocks& b) {
+  return make_tc_plan(D, bwd, b.n_row_slots / kTcM, b.n_col_slots / kTcBN, b.n_seg, std::max(b.max_tiles, 1), N,
+                      tc_blocks_seg_bytes(b.n_seg) + std::max<int64_t>(b.n_pieces, 1) * 8);
+}
+
+int64_t tc_blocks_scratch_bytes(int64_t N, int D, const TcBlocks& b) {
+  return std::max(make_tc_blocks_plan(N, D, false, b).total, make_tc_blocks_plan(N, D, true, b).total);
 }
 
 // What the images of a launch group hold (tc_pack_kernel): the row cloud x and the column cloud y, centred at `center`
@@ -390,74 +367,171 @@ static int tc_pack(const TcPlan& p, unsigned char* base, const TcOperands& o, cu
   return B200OT_OK;
 }
 
-// One launch of a reduction or row-gradient kernel over plan p, into the plan's partials: `rows` rows (n_local per
-// batch element; block-sparse problems: seg / pieces / row_src)
-static int tc_launch(TcKernel kern, const TcPlan& p, unsigned char* base, int64_t rows, int64_t n_local, int D,
-                     int self_mode, float clampq, const float* coord_absmax, cudaStream_t st,
-                     const int4* seg = nullptr, const int2* pieces = nullptr, const int* row_src = nullptr) {
+// tc_reduce_kernel<FWD> (forward) or tc_bwd_kernel<BWD> at the padded dimension of D (row gradients)
+template <int FWD, int BWD, bool BATCH, bool BLOCKS = false>
+static TcKernel tc_kernel_of(bool bwd, int D) {
+  if (!bwd) return tc_reduce_kernel<FWD, BATCH, BLOCKS>;
+  switch (tc_dk(D)) {
+    case 16: return tc_bwd_kernel<BWD, 16, BATCH, BLOCKS>;
+    case 32: return tc_bwd_kernel<BWD, 32, BATCH, BLOCKS>;
+    case 48: return tc_bwd_kernel<BWD, 48, BATCH, BLOCKS>;
+    default: return tc_bwd_kernel<BWD, 64, BATCH, BLOCKS>;
+  }
+}
+
+// The kernel of `mode` (the MODE of tc_reduce_kernel forward, of tc_bwd_kernel for the row gradients: 0 / 2 gaussian
+// conv, 1 / 3 softmin p = 2, 4 laplacian, 5 energy, 6 / 7 softmin p = 1) for D and the layout; null for a pair that
+// has none.  Above D = 64 the K-slab kernels, whatever the layout.
+static TcKernel tc_kernel(int mode, bool bwd, int D, TcLayout layout) {
+  if (D > 64) return tc_wide_kernel(mode, bwd);
+  const bool one = layout == TcLayout::kOne, batch = layout == TcLayout::kBatch;
+  switch (mode) {
+    case 0:
+    case 2: return one ? tc_kernel_of<0, 2, false>(bwd, D) : batch ? tc_kernel_of<0, 2, true>(bwd, D) : nullptr;
+    case 1:
+    case 3:
+      return one     ? tc_kernel_of<1, 3, false>(bwd, D)
+             : batch ? tc_kernel_of<1, 3, true>(bwd, D)
+                     : tc_kernel_of<1, 3, false, true>(bwd, D);
+    case 4: return one ? tc_kernel_of<4, 4, false>(bwd, D) : batch ? tc_kernel_of<4, 4, true>(bwd, D) : nullptr;
+    case 5: return one ? tc_kernel_of<5, 5, false>(bwd, D) : batch ? tc_kernel_of<5, 5, true>(bwd, D) : nullptr;
+    default: return batch ? tc_kernel_of<6, 7, true>(bwd, D) : nullptr;
+  }
+}
+
+// One tensor-core pass of `mode` (tc_kernel) over B elements of o.N rows / o.M columns, or over the block-sparse
+// problem `blocks` of o.N rows: plan, images, kernel and launch.  The row gradients normalise the weights (when the
+// operator has any) and the energy's coordinates (modes 5, 6, 7) take a power-of-two scale from their maximum
+// (tc_pack); the finalize undoes both.
+static int tc_pass(int mode, bool bwd, TcLayout layout, TcOperands o, float clampq, const TcBlocks* blocks,
+                   void* scratch, cudaStream_t st, TcPass* r) {
+  const TcPlan p = blocks ? make_tc_blocks_plan(o.N, o.D, bwd, *blocks)
+                          : make_tc_plan(o.N, o.M, o.D, bwd, o.B, mode == 7 ? 2 : 1);
+  const TcKernel kern = tc_kernel(mode, bwd, o.D, layout);
+  if (p.nstage < 1 || kern == nullptr) return B200OT_EINVAL;
+  // K_xx / K_yy and the p = 1 xx / yy: the diagonal exponent is exact (tcconv.cuh)
+  const int self_mode = (mode != 1 && mode != 3 && o.x == o.y && o.N == o.M) ? 1 : 0;
+  const int64_t rows = o.B * o.N, n_local = blocks ? 0 : o.N;
+  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
+  const int4* seg = nullptr;
+  const int2* pieces = nullptr;
+  if (blocks) {
+    // the host descriptors travel in the misc block
+    int4* d_seg = reinterpret_cast<int4*>(base + p.off_misc);
+    int2* d_pieces = reinterpret_cast<int2*>(base + p.off_misc + tc_blocks_seg_bytes(blocks->n_seg));
+    B200OT_CUDA_TRY(cudaMemcpyAsync(d_seg, blocks->seg, blocks->n_seg * 16, cudaMemcpyHostToDevice, st));
+    if (blocks->n_pieces > 0)
+      B200OT_CUDA_TRY(cudaMemcpyAsync(d_pieces, blocks->pieces, blocks->n_pieces * 8, cudaMemcpyHostToDevice, st));
+    seg = d_seg;
+    pieces = d_pieces;
+    o.N = blocks->n_row_slots;
+    o.M = blocks->n_col_slots;
+    o.row_src = blocks->row_src;
+    o.col_src = blocks->col_src;
+  }
+  *r = TcPass{};
+  int rc = tc_pack(p, base, o, st, bwd ? &r->w_absmax : nullptr, mode >= 5 ? &r->coord_absmax : nullptr);
+  if (rc) return rc;
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  const dim3 grid((unsigned)p.ctas, (unsigned)p.n_split);
+  const dim3 grid((unsigned)p.ctas, (unsigned)p.n_split, (unsigned)p.slices);
   kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(base, base + p.off_b, reinterpret_cast<float*>(base + p.off_part),
-                                                 rows, p.kp, p.ctpe, p.tiles_per_split, p.nstage, D, self_mode, clampq,
-                                                 coord_absmax, p.rtpe, n_local, seg, pieces, row_src);
+                                                 rows, p.kp, p.ctpe, p.tiles_per_split, p.nstage, o.D, self_mode,
+                                                 clampq, r->coord_absmax, p.rtpe, n_local, seg, pieces, o.row_src);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  r->part = reinterpret_cast<float*>(base + p.off_part);
+  // row gradients: G of a CTA is complete over its column split (both column halves feed one GEMM)
+  r->n_part = bwd ? p.n_split : p.n_split * kTcParts;
+  return B200OT_OK;
+}
+
+// The softmin, p = 2 (MODE 1 / 3) or p = 1 (MODE 6 / 7, on the energy's coordinates with the clamp of p)
+int softmin_pass_tc(bool bwd, TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, void* scratch,
+                    cudaStream_t st, TcPass* r) {
+  const bool l1 = p_exponent(s.p) == 1;
+  TcOperands o{s.x, s.y, s.center, l1 ? 1.f : softmin_coord_scale(2, s.eps), s.N, s.M, s.D, s.B, nullptr, s.h_a, s.h_b,
+               s.h_scale_b, s.lse2};
+  if (l1) o.l1_c = kLog2e / s.eps;
+  return tc_pass(l1 ? (bwd ? 7 : 6) : (bwd ? 3 : 1), bwd, layout, o, l1 ? cost_clamp(s.p) : 0.f, blocks, scratch, st,
+                 r);
+}
+
+int softmin_fwd_tc(TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, const float* out_old, float alpha_old,
+                   float beta, float* out, float* lse2_out, void* scratch, void* stream) {
+  TcPass r;
+  const int rc = softmin_pass_tc(false, layout, s, blocks, scratch, (cudaStream_t)stream, &r);
+  if (rc) return rc;
+  return b200ot_softmin_finalize(r.part, r.n_part, out_old, alpha_old, beta, out, lse2_out, s.B * s.N, s.eps, stream);
+}
+
+// p = 1 on the tensor cores: part (n_split, N, D+2) with [0] = sum P, [1] = sum Q, [2+k] = sum Q Y_k (tcbwd.cuh, MODE 7)
+// -> grad_x = go (X_i sum Q - sum Q Y) / sum P, X = scale (x - center) with the pass's coordinate scale
+__global__ void softmin_l1_bwd_finalize_kernel(const float* __restrict__ part, int n_split,
+                                               const float* __restrict__ x, const float* __restrict__ center,
+                                               const float* __restrict__ grad_out, float* __restrict__ grad_x,
+                                               int64_t N, int D, const float* __restrict__ coord_absmax) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int na = D + 2;
+  const float scale = tc_energy_coord_scale(*coord_absmax);
+  float sp = 0.f, sq = 0.f;
+  for (int s = 0; s < n_split; ++s) {
+    sp += part[((int64_t)s * N + i) * na];
+    sq += part[((int64_t)s * N + i) * na + 1];
+  }
+  const float go = sp > 0.f ? grad_out[i] / sp : 0.f;
+  for (int k = 0; k < D; ++k) {
+    float a = 0.f;
+    for (int s = 0; s < n_split; ++s) a += part[((int64_t)s * N + i) * na + 2 + k];
+    const float X = scale * (x[i * D + k] - (center ? center[k] : 0.f));
+    grad_x[i * D + k] = go * (X * sq - a);
+  }
+}
+
+int softmin_bwd_x_tc(TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, const float* grad_out, float* grad_x,
+                     void* scratch, cudaStream_t st) {
+  TcPass r;
+  const int rc = softmin_pass_tc(true, layout, s, blocks, scratch, st, &r);
+  if (rc) return rc;
+  // P carries kTcPScale (p = 2) or 2^k_i (p = 1), which cancel: both finalizes divide by each row's sum of P
+  const int64_t rows = s.B * s.N;
+  if (p_exponent(s.p) == 2)
+    return softmin_bwd_finalize_tc(r.part, r.n_part, s.x, s.center, grad_out, grad_x, rows, s.D, s.eps, st);
+  softmin_l1_bwd_finalize_kernel<<<(unsigned)ceil_div64(rows, 256), 256, 0, st>>>(r.part, r.n_part, s.x, s.center,
+                                                                                  grad_out, grad_x, rows, s.D,
+                                                                                  r.coord_absmax);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
 
-// tc_bwd_kernel at the padded dimension of D
-template <int MODE, bool BATCH, bool BLOCKS = false>
-static TcKernel tc_bwd_dk(int D) {
-  switch (tc_dk(D)) {
-    case 16: return tc_bwd_kernel<MODE, 16, BATCH, BLOCKS>;
-    case 32: return tc_bwd_kernel<MODE, 32, BATCH, BLOCKS>;
-    case 48: return tc_bwd_kernel<MODE, 48, BATCH, BLOCKS>;
-    default: return tc_bwd_kernel<MODE, 64, BATCH, BLOCKS>;
+// The kernel convolution of B elements of N rows / M columns on the tensor cores: out (forward) or grad_x (bwd) and,
+// with value_out, the forward values from the same pass (gaussian only).  Every row-gradient kernel leaves the
+// gaussian's sums: grad = coef (sum_j P Y_j - X_i sum_j P) with coef = 1 / (scale blur^2) for the gaussian; the
+// laplacian and energy P = w k'(d) / d carries 2^-kTcNormPLog2 (tcbwd.cuh), so coef = 2^kTcNormPLog2 / blur (laplacian,
+// X = x log2e / blur) or 2^kTcNormPLog2 (energy).  Arguments already validated.
+static int conv_tc(bool bwd, TcLayout layout, int kind, const float* x, const float* y, const float* w,
+                   const float* center, const float* grad_out, float* res, float* value_out, int64_t B, int64_t N,
+                   int64_t M, int D, float blur, void* scratch, cudaStream_t st) {
+  const int kb = kind_base(kind);
+  // gaussian: 2^(-|X-Y|^2/2) with X = x sqrt(log2e) / blur; laplacian / energy: conv_scales' coordinates and clamp
+  const ConvScales cs = conv_scales(kind, blur);
+  const int mode = kb == B200OT_KERNEL_GAUSSIAN ? (bwd ? 2 : 0) : (kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5);
+  TcPass r;
+  const int rc = tc_pass(mode, bwd, layout, {x, y, center, cs.scale, N, M, D, B, w}, cs.clampq, nullptr, scratch, st, &r);
+  if (rc) return rc;
+  const unsigned blocks = (unsigned)ceil_div64(B * N, 256);
+  if (!bwd) {
+    conv_fwd_finalize_kernel<<<blocks, 256, 0, st>>>(r.part, r.n_part, kb == B200OT_KERNEL_ENERGY ? -1.f : 1.f, res,
+                                                    B * N, r.coord_absmax);
+  } else {
+    const float coef = kb == B200OT_KERNEL_GAUSSIAN
+                           ? 1.0f / (cs.scale * blur * blur)
+                           : (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
+    // n_per = N: the finalize undoes each element's weight scale
+    conv_bwd_finalize_kernel<<<blocks, 256, 0, st>>>(r.part, r.n_part, x, center, grad_out, res, B * N, D,
+                                                    B200OT_KERNEL_GAUSSIAN, cs.scale, coef, r.w_absmax, value_out,
+                                                    r.coord_absmax, N);
   }
-}
-
-// Row gradients on the tensor-core path; `mode` is the MODE of tc_bwd_kernel (2 gaussian conv, 3 softmin p = 2,
-// 4 laplacian, 5 energy; clampq: see there).  Leaves n_part sets of (B N, D+1) partial sums in *part_out, and the
-// scales the finalize undoes in *w_absmax_out and *coord_absmax_out (tc_pack; null when the pass has none).
-// `batched`: B elements of N rows / M columns (make_tc_plan), the weights normalised per element.
-int bwd_partial_tc(int mode, const float* x, const float* y, const float* w, const float* h_a, const float* h_b,
-                   float h_scale_b, const float* lse2, const float* center, float scale, int64_t N, int64_t M, int D,
-                   void* scratch, float** part_out, int* n_part_out, cudaStream_t st, int64_t B, bool batched,
-                   const float** w_absmax_out, float clampq, const float** coord_absmax_out) {
-  const TcPlan p = make_tc_plan(N, M, D, true, B);
-  if (p.nstage < 1) return B200OT_EINVAL;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  const float *w_absmax = nullptr, *coord_absmax = nullptr;
-  int rc = tc_pack(p, base, {x, y, center, scale, N, M, D, B, w, h_a, h_b, h_scale_b, lse2}, st, &w_absmax,
-                   mode == 5 ? &coord_absmax : nullptr);
-  if (rc) return rc;
-  const TcKernel kern = mode == 2   ? (batched ? tc_bwd_dk<2, true>(D) : tc_bwd_dk<2, false>(D))
-                        : mode == 3 ? (batched ? tc_bwd_dk<3, true>(D) : tc_bwd_dk<3, false>(D))
-                        : mode == 4 ? (batched ? tc_bwd_dk<4, true>(D) : tc_bwd_dk<4, false>(D))
-                                    : (batched ? tc_bwd_dk<5, true>(D) : tc_bwd_dk<5, false>(D));
-  const int self_mode = (mode != 3 && x == y && N == M) ? 1 : 0;  // K_xx: exact zero exponent on the diagonal
-  rc = tc_launch(kern, p, base, B * N, N, D, self_mode, clampq, coord_absmax, st);
-  if (rc) return rc;
-  if (w_absmax_out) *w_absmax_out = w_absmax;
-  if (coord_absmax_out) *coord_absmax_out = coord_absmax;
-  *part_out = reinterpret_cast<float*>(base + p.off_part);
-  *n_part_out = p.n_split;  // G of a CTA is complete over its column split (both column halves feed one GEMM)
-  return B200OT_OK;
-}
-
-// Tensor-core softmin partials (p = 2): packs both clouds, runs the reduction, leaves n_part (m, s) sets in
-// `*part_out` (inside scratch) for b200ot_softmin_finalize.  `batched`: B elements (make_tc_plan), B N rows of partials.
-int softmin_partial_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
-                       const float* center, int64_t N, int64_t M, int D, float eps, void* scratch,
-                       float** part_out, int* n_part_out, cudaStream_t st, int64_t B, bool batched) {
-  const TcPlan p = make_tc_plan(N, M, D, false, B);
-  if (p.nstage < 1) return B200OT_EINVAL;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  int rc = tc_pack(p, base, {x, y, center, softmin_coord_scale(2, eps), N, M, D, B, nullptr, h_a, h_b, h_scale_b}, st);
-  if (rc) return rc;
-  rc = tc_launch(batched ? tc_reduce_kernel<1, true> : tc_reduce_kernel<1>, p, base, B * N, N, D, 0, 0.f, nullptr, st);
-  if (rc) return rc;
-  *part_out = reinterpret_cast<float*>(base + p.off_part);
-  *n_part_out = p.n_split * kTcParts;
+  B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
 
@@ -534,165 +608,22 @@ int plan_apply_tc(const float* x, const float* y, const float* h_a, const float*
   return B200OT_OK;
 }
 
-// The p = 1 softmin of B elements of N rows / M columns (B = 1: one problem) on the tensor cores (tcconv.cuh, MODE 6 / 7):
-// packs both clouds on the energy's coordinates and runs the forward reduction (bwd = false: n_part (m, s) sets for
-// b200ot_softmin_finalize) or the row-gradient sums (bwd, lse2 = the forward's: n_part sets of (B N, D+2) sums).
-// *coord_absmax_out: the coordinate maximum the pass derived its scale from.  Arguments already validated.
-int softmin_l1_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
-                  const float* center, const float* lse2, int64_t B, int64_t N, int64_t M, int D, int p, float eps,
-                  void* scratch, float** part_out, int* n_part_out, const float** coord_absmax_out, cudaStream_t st) {
-  const TcPlan pl = make_tc_plan(N, M, D, bwd, B, bwd ? 2 : 1);
-  if (pl.nstage < 1) return B200OT_EINVAL;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  const float* coord_absmax = nullptr;
-  TcOperands o{x, y, center, 1.f, N, M, D, B, nullptr, h_a, h_b, h_scale_b, bwd ? lse2 : nullptr};
-  o.l1_c = kLog2e / eps;
-  int rc = tc_pack(pl, base, o, st, nullptr, &coord_absmax);
-  if (rc) return rc;
-  const TcKernel kern = bwd ? tc_bwd_dk<7, true>(D) : tc_reduce_kernel<6, true>;
-  const int self_mode = (x == y && N == M) ? 1 : 0;  // xx / yy: the diagonal takes d = sqrt(clamp) exactly
-  rc = tc_launch(kern, pl, base, B * N, N, D, self_mode, cost_clamp(p), coord_absmax, st);
-  if (rc) return rc;
-  *part_out = reinterpret_cast<float*>(base + pl.off_part);
-  *n_part_out = bwd ? pl.n_split : pl.n_split * kTcParts;
-  *coord_absmax_out = coord_absmax;
-  return B200OT_OK;
-}
-
-// p = 1 on the tensor cores: part (n_split, N, D+2) with [0] = sum P, [1] = sum Q, [2+k] = sum Q Y_k (tcbwd.cuh, MODE 7)
-// -> grad_x = go (X_i sum Q - sum Q Y) / sum P, X = scale (x - center) with the pass's coordinate scale
-__global__ void softmin_l1_bwd_finalize_kernel(const float* __restrict__ part, int n_split,
-                                               const float* __restrict__ x, const float* __restrict__ center,
-                                               const float* __restrict__ grad_out, float* __restrict__ grad_x,
-                                               int64_t N, int D, const float* __restrict__ coord_absmax) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  const int na = D + 2;
-  const float scale = tc_energy_coord_scale(*coord_absmax);
-  float sp = 0.f, sq = 0.f;
-  for (int s = 0; s < n_split; ++s) {
-    sp += part[((int64_t)s * N + i) * na];
-    sq += part[((int64_t)s * N + i) * na + 1];
-  }
-  const float go = sp > 0.f ? grad_out[i] / sp : 0.f;
-  for (int k = 0; k < D; ++k) {
-    float a = 0.f;
-    for (int s = 0; s < n_split; ++s) a += part[((int64_t)s * N + i) * na + 2 + k];
-    const float X = scale * (x[i * D + k] - (center ? center[k] : 0.f));
-    grad_x[i * D + k] = go * (X * sq - a);
-  }
-}
-
-int softmin_l1_bwd_finalize(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
-                            float* grad_x, int64_t N, int D, const float* coord_absmax, cudaStream_t st) {
-  softmin_l1_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(part, n_part, x, center, grad_out,
-                                                                               grad_x, N, D, coord_absmax);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Above D = 64 (tcwide.cuh): the same images, plans and finalize kernels, the K-slab kernels of b200ot_wide.cu.
-// B elements of N rows / M columns (B = 1: one problem).
-// ---------------------------------------------------------------------------------------------------
-static TcPlan make_tc_wide_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B, int head) {
-  const int rtpe = (int)ceil_div64(N, kTcM), ctpe = (int)ceil_div64(M, kTcBN);
-  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4, head,
-                          bwd ? tc_wide_slabs(D) : 1);
-  p.rtpe = rtpe;
-  p.ctpe = ctpe;
-  return p;
-}
-
-int64_t tc_wide_scratch_bytes(int64_t N, int64_t M, int D, int64_t B) {
-  // the forward and the row gradient (D + 2 sums per row for the p = 1 softmin) split the columns differently
-  return std::max(make_tc_wide_plan(N, M, D, false, B, 1).total, make_tc_wide_plan(N, M, D, true, B, 2).total);
-}
-
-// Pack (with the weight and coordinate maxima asked for) and one wide kernel of MODE over the plan; leaves n_part sets
-// of partials (forward: (m, s) pairs or sums per row; bwd: (B N, D + head) sums) in *part_out.
-static int tc_wide_pass(int mode, bool bwd, const TcOperands& o, int head, int self_mode, float clampq, bool want_wmax,
-                        bool want_cmax, void* scratch, cudaStream_t st, float** part_out, int* n_part_out,
-                        const float** w_absmax_out, const float** coord_absmax_out) {
-  const TcPlan p = make_tc_wide_plan(o.N, o.M, o.D, bwd, o.B, head);
-  if (p.nstage < 1) return B200OT_EINVAL;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  const float *w_absmax = nullptr, *coord_absmax = nullptr;
-  int rc = tc_pack(p, base, o, st, want_wmax ? &w_absmax : nullptr, want_cmax ? &coord_absmax : nullptr);
-  if (rc) return rc;
-  const TcKernel kern = tc_wide_kernel(mode, bwd);
-  if (kern == nullptr) return B200OT_EINVAL;
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  const dim3 grid((unsigned)p.ctas, (unsigned)p.n_split, bwd ? (unsigned)tc_wide_slabs(o.D) : 1u);
-  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(base, base + p.off_b, reinterpret_cast<float*>(base + p.off_part),
-                                                 o.B * o.N, p.kp, p.ctpe, p.tiles_per_split, p.nstage, o.D, self_mode,
-                                                 clampq, coord_absmax, p.rtpe, o.N, nullptr, nullptr, nullptr);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  *part_out = reinterpret_cast<float*>(base + p.off_part);
-  *n_part_out = bwd ? p.n_split : p.n_split * kTcParts;
-  if (w_absmax_out) *w_absmax_out = w_absmax;
-  if (coord_absmax_out) *coord_absmax_out = coord_absmax;
-  return B200OT_OK;
-}
-
-// The softmin above D = 64, p = 2 (MODE 1 / 3) or p = 1 (MODE 6 / 7, the energy's coordinates as in softmin_l1_tc).
-// Forward: n_part (m, s) sets for b200ot_softmin_finalize.  bwd (lse2 = the forward's): n_part sets of (B N, D + 1)
-// sums for softmin_bwd_finalize_tc (p = 2), or (B N, D + 2) for softmin_l1_bwd_finalize (p = 1, *coord_absmax_out).
-int softmin_wide_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
-                    const float* center, const float* lse2, int64_t B, int64_t N, int64_t M, int D, int p, float eps,
-                    void* scratch, float** part_out, int* n_part_out, const float** coord_absmax_out,
-                    cudaStream_t st) {
-  if (p_exponent(p) == 2) {
-    TcOperands o{x, y, center, softmin_coord_scale(2, eps), N, M, D, B, nullptr, h_a, h_b, h_scale_b,
-                 bwd ? lse2 : nullptr};
-    return tc_wide_pass(bwd ? 3 : 1, bwd, o, 1, 0, 0.f, false, false, scratch, st, part_out, n_part_out, nullptr,
-                        nullptr);
-  }
-  TcOperands o{x, y, center, 1.f, N, M, D, B, nullptr, h_a, h_b, h_scale_b, bwd ? lse2 : nullptr};
-  o.l1_c = kLog2e / eps;
-  const int self_mode = (x == y && N == M) ? 1 : 0;  // xx / yy: the diagonal takes d = sqrt(clamp) exactly
-  return tc_wide_pass(bwd ? 7 : 6, bwd, o, bwd ? 2 : 1, self_mode, cost_clamp(p), false, true, scratch, st, part_out,
-                      n_part_out, nullptr, coord_absmax_out);
-}
-
-// The kernel convolutions above D = 64: out (forward) or grad_x (bwd, grad_out given), as conv_fwd_tc / conv_bwd_tc
-static int conv_wide_tc(bool bwd, int kind, const float* x, const float* y, const float* w, const float* center,
-                        const float* grad_out, float* res, int64_t B, int64_t N, int64_t M, int D, float blur,
-                        void* scratch, cudaStream_t st) {
-  const int kb = kind_base(kind);
-  const ConvScales cs = conv_scales(kind, blur);
-  const int mode = kb == B200OT_KERNEL_GAUSSIAN ? (bwd ? 2 : 0) : (kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5);
-  const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
-  float* part = nullptr;
-  int n_part = 0;
-  const float *w_absmax = nullptr, *coord_absmax = nullptr;
-  const int rc = tc_wide_pass(mode, bwd, {x, y, center, cs.scale, N, M, D, B, w}, 1, self_mode, cs.clampq, bwd,
-                              kb == B200OT_KERNEL_ENERGY, scratch, st, &part, &n_part, &w_absmax, &coord_absmax);
-  if (rc) return rc;
-  if (!bwd) {
-    conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-        part, n_part, kb == B200OT_KERNEL_ENERGY ? -1.f : 1.f, res, B * N, coord_absmax);
-  } else {
-    const float coef = kb == B200OT_KERNEL_GAUSSIAN
-                           ? 1.0f / (cs.scale * blur * blur)
-                           : (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
-    conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-        part, n_part, x, center, grad_out, res, B * N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax, nullptr,
-        coord_absmax, N);
-  }
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
 // ---------------------------------------------------------------------------------------------------
 // Block-sparse softmins (the fine phase of the two-scale Sinkhorn above D = 8): every row cluster and every column
 // cluster is padded to whole 128-point tiles on its own, slot -> point through row_src / col_src (-1: padding).  One
-// segment per row tile; the host descriptors are validated here and copied into the scratch behind the partials.
+// segment per row tile; the host descriptors are validated here and copied into the scratch behind the partials
+// (tc_pass).
 // ---------------------------------------------------------------------------------------------------
 static_assert(kTcBlocksTile == kTcM && kTcBlocksTile == kTcBN, "segments are one row tile, pieces whole column tiles");
 
-int blocks_validate(int64_t n_row_slots, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
-                    const b200ot_piece* pieces, int* max_tiles, int64_t* n_pieces) {
+int blocks_check(int64_t N, int D, int p, float eps, const void* scratch, TcBlocks& b) {
+  const b200ot_segment* seg = b.seg;
+  const b200ot_piece* pieces = b.pieces;
+  const int64_t n_row_slots = b.n_row_slots, n_col_slots = b.n_col_slots, n_seg = b.n_seg;
+  if (!seg || !pieces || N <= 0 || n_seg <= 0 || n_seg > 0x7fffffff || !tc_blocks_dims(D) || !valid_p(p) ||
+      p_exponent(p) != 2 || !(eps > 0.f))
+    return B200OT_EINVAL;
+  if ((((uintptr_t)seg) & 15) || (((uintptr_t)pieces) & 7) || (((uintptr_t)scratch) & 15)) return B200OT_EALIGN;
   if (n_row_slots <= 0 || n_col_slots <= 0 || n_row_slots % kTcM || n_col_slots % kTcBN ||
       n_row_slots / kTcM != n_seg || n_col_slots / kTcBN > 0x7fffffff)
     return B200OT_EINVAL;
@@ -723,106 +654,8 @@ int blocks_validate(int64_t n_row_slots, int64_t n_col_slots, const b200ot_segme
     mt = std::max(mt, before[seg[s].piece_end] - before[seg[s].piece_begin]);
   }
   if (mt > 0x7fffffff) return B200OT_EINVAL;
-  *max_tiles = (int)mt;
-  *n_pieces = np;
-  return B200OT_OK;
-}
-
-// The plan of one block-sparse problem: a CTA per segment, images of n_row_slots / n_col_slots points, segments cut
-// into splits from the longest one.  Misc block: the segment descriptors, then the pieces.
-static int64_t tc_blocks_seg_bytes(int64_t n_seg) { return round_up64(n_seg * 16, 256); }
-static TcPlan make_tc_blocks_plan(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
-                                  int max_tiles, int D, bool bwd) {
-  return make_tc_plan(D, bwd, n_row_slots / kTcM, n_col_slots / kTcBN, n_seg, std::max(max_tiles, 1), N,
-                      tc_blocks_seg_bytes(n_seg) + std::max<int64_t>(n_pieces, 1) * 8);
-}
-
-int64_t tc_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots, int64_t n_seg, int64_t n_pieces,
-                                int max_tiles, int D) {
-  return std::max(make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, false).total,
-                  make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, true).total);
-}
-
-// Pack, descriptor copy and reduction of one block-sparse softmin (bwd: the row-gradient sums, lse2 = the forward's);
-// arguments already validated.  Leaves n_part partial sets of N rows in *part_out, like softmin_partial_tc (forward)
-// and bwd_partial_tc (backward).
-int softmin_blocks_tc(bool bwd, const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
-                      const float* center, const float* lse2, int64_t N, const int* row_src, int64_t n_row_slots,
-                      const int* col_src, int64_t n_col_slots, const b200ot_segment* seg, int64_t n_seg,
-                      const b200ot_piece* pieces, int64_t n_pieces, int max_tiles, int D, float eps, void* scratch,
-                      float** part_out, int* n_part_out, cudaStream_t st) {
-  const TcPlan p = make_tc_blocks_plan(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D, bwd);
-  if (p.nstage < 1) return B200OT_EINVAL;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  int4* d_seg = reinterpret_cast<int4*>(base + p.off_misc);
-  int2* d_pieces = reinterpret_cast<int2*>(base + p.off_misc + tc_blocks_seg_bytes(n_seg));
-  B200OT_CUDA_TRY(cudaMemcpyAsync(d_seg, seg, n_seg * 16, cudaMemcpyHostToDevice, st));
-  if (n_pieces > 0) B200OT_CUDA_TRY(cudaMemcpyAsync(d_pieces, pieces, n_pieces * 8, cudaMemcpyHostToDevice, st));
-  int rc = tc_pack(p, base,
-                   {x, y, center, softmin_coord_scale(2, eps), n_row_slots, n_col_slots, D, 1, nullptr, h_a, h_b,
-                    h_scale_b, bwd ? lse2 : nullptr, row_src, col_src},
-                   st);
-  if (rc) return rc;
-  const TcKernel kern = bwd ? tc_bwd_dk<3, false, true>(D) : tc_reduce_kernel<1, false, true>;
-  rc = tc_launch(kern, p, base, N, 0, D, 0, 0.f, nullptr, st, d_seg, d_pieces, row_src);
-  if (rc) return rc;
-  *part_out = reinterpret_cast<float*>(base + p.off_part);
-  *n_part_out = bwd ? p.n_split : p.n_split * kTcParts;
-  return B200OT_OK;
-}
-
-static int conv_fwd_tc(int kind_flags, const float* x, const float* y, const float* w, const float* center, float* out,
-                       int64_t N, int64_t M, int D, float blur, void* scratch, cudaStream_t st, int64_t B,
-                       bool batched) {
-  const int kind = kind_base(kind_flags);
-  const TcPlan p = make_tc_plan(N, M, D, false, B);
-  if (p.nstage < 1) return B200OT_EINVAL;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  // gaussian: 2^(-|X-Y|^2/2) with X = x sqrt(log2e) / blur; laplacian / energy: conv_scales' coordinates and clamp
-  const ConvScales cs = conv_scales(kind_flags, blur);
-  const float* coord_absmax = nullptr;
-  int rc = tc_pack(p, base, {x, y, center, cs.scale, N, M, D, B, w}, st, nullptr,
-                   kind == B200OT_KERNEL_ENERGY ? &coord_absmax : nullptr);
-  if (rc) return rc;
-  const TcKernel kern = kind == B200OT_KERNEL_GAUSSIAN    ? (batched ? tc_reduce_kernel<0, true> : tc_reduce_kernel<0>)
-                        : kind == B200OT_KERNEL_LAPLACIAN ? (batched ? tc_reduce_kernel<4, true> : tc_reduce_kernel<4>)
-                                                          : (batched ? tc_reduce_kernel<5, true> : tc_reduce_kernel<5>);
-  const int self_mode = (x == y && N == M) ? 1 : 0;  // K_xx / K_yy: the diagonal exponent is exactly 0 (tcconv.cuh)
-  rc = tc_launch(kern, p, base, B * N, N, D, self_mode, cs.clampq, coord_absmax, st);
-  if (rc) return rc;
-  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-      reinterpret_cast<const float*>(base + p.off_part), p.n_split * kTcParts,
-      kind == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, B * N, coord_absmax);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
-// Row gradients on the tensor cores (and, with value_out, the forward values from the same pass: gaussian only), of one
-// problem or (`batched`) of B elements of N rows / M columns.  Arguments already validated.  Every kernel leaves the
-// gaussian's sums: grad = coef (sum_j P Y_j - X_i sum_j P) with coef = 1 / (scale blur^2) for the gaussian; the
-// laplacian and energy P = w k'(d) / d carries 2^-kTcNormPLog2 (tcbwd.cuh), so coef = 2^kTcNormPLog2 / blur (laplacian,
-// X = x log2e / blur) or 2^kTcNormPLog2 (energy).
-static int conv_bwd_tc(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
-                       float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
-                       void* scratch, void* stream, int64_t B, bool batched) {
-  cudaStream_t st = (cudaStream_t)stream;
-  const int kb = kind_base(kind);
-  const ConvScales cs = conv_scales(kind, blur);
-  const int mode = kb == B200OT_KERNEL_GAUSSIAN ? 2 : (kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5);
-  const float coef = kb == B200OT_KERNEL_GAUSSIAN
-                         ? 1.0f / (cs.scale * blur * blur)
-                         : (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
-  float* tc_part = nullptr;
-  int n_part = 0;
-  const float *w_absmax = nullptr, *coord_absmax = nullptr;
-  const int rc = bwd_partial_tc(mode, x, y, w, nullptr, nullptr, 0.f, nullptr, center, cs.scale, N, M, D, scratch,
-                                &tc_part, &n_part, st, B, batched, &w_absmax, cs.clampq, &coord_absmax);
-  if (rc) return rc;
-  const int64_t n_per = batched ? N : 0;  // rows per element: the finalize undoes each element's weight scale
-  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(B * N, 256), 256, 0, st>>>(
-      tc_part, n_part, x, center, grad_out, grad_x, B * N, D, B200OT_KERNEL_GAUSSIAN, cs.scale, coef, w_absmax,
-      value_out, coord_absmax, n_per);
-  B200OT_CUDA_TRY(cudaGetLastError());
+  b.max_tiles = (int)mt;
+  b.n_pieces = np;
   return B200OT_OK;
 }
 
@@ -834,13 +667,13 @@ extern "C" {
 
 B200OT_API int64_t b200ot_kernel_conv_scratch_bytes(int64_t N, int64_t M, int32_t D) {
   if (N <= 0 || M <= 0 || D <= 0) return 0;
-  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D) : 0;
+  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D, 1, 1) : 0;
   const ReducePlan pl = make_plan(N, M, D);
   const int64_t cols = b200ot_packed_cols_floats(M, D, 2) * 4;
   const int64_t part = (int64_t)pl.n_split * N * 4 * (D + 1);
   const int64_t simt = round_up64(cols, 256) + round_up64(part, 256);
   // (one size for every operator of the shape: the caller does not say which one it is about to run)
-  return tc_any_routed(D, N, M) ? std::max(simt, tc_scratch_bytes(N, M, D)) : simt;
+  return tc_any_routed(D, N, M) ? std::max(simt, tc_scratch_bytes(N, M, D, 1, 1)) : simt;
 }
 
 B200OT_API int b200ot_kernel_conv_finalize(const float* part, int32_t n_part, float* out, int64_t N, int32_t kind,
@@ -907,10 +740,12 @@ static int conv_fwd_impl(const float* x, const float* y, const float* w, const f
   const bool shape = batched ? tc_batched_dims(B, N, M, D) : (N > 0 && M > 0 && (supported_simt_dim(D) || tc));
   if (!x || !y || !w || !out || !scratch || !shape || !valid_kind(kind)) return B200OT_EINVAL;
   if (!blur_ok(kind, blur)) return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < (batched ? b200ot_batched_scratch_bytes(B, N, M, D) : b200ot_kernel_conv_scratch_bytes(N, M, D)))
-    return B200OT_ESCRATCH;
-  if (tc) return conv_fwd_tc(kind, x, y, w, center, out, N, M, D, blur, scratch, (cudaStream_t)stream, B, batched);
+  if (const int rc = scratch_check(scratch, scratch_bytes, batched ? b200ot_batched_scratch_bytes(B, N, M, D)
+                                                                   : b200ot_kernel_conv_scratch_bytes(N, M, D)))
+    return rc;
+  if (tc)
+    return conv_tc(false, batched ? TcLayout::kBatch : TcLayout::kOne, kind, x, y, w, center, nullptr, out, nullptr, B,
+                   N, M, D, blur, scratch, (cudaStream_t)stream);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -942,11 +777,12 @@ static int conv_bwd_x_impl(const float* x, const float* y, const float* w, const
   if (!x || !y || !w || !grad_x || !scratch || !shape || !valid_kind(kind) || (value_out && !gauss))
     return B200OT_EINVAL;
   if (!blur_ok(kind, blur)) return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < (batched ? b200ot_batched_scratch_bytes(B, N, M, D) : b200ot_kernel_conv_scratch_bytes(N, M, D)))
-    return B200OT_ESCRATCH;
+  if (const int rc = scratch_check(scratch, scratch_bytes, batched ? b200ot_batched_scratch_bytes(B, N, M, D)
+                                                                   : b200ot_kernel_conv_scratch_bytes(N, M, D)))
+    return rc;
   if (tc)
-    return conv_bwd_tc(x, y, w, center, grad_out, grad_x, value_out, N, M, D, kind, blur, scratch, stream, B, batched);
+    return conv_tc(true, batched ? TcLayout::kBatch : TcLayout::kOne, kind, x, y, w, center, grad_out, grad_x,
+                   value_out, B, N, M, D, blur, scratch, (cudaStream_t)stream);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -984,7 +820,7 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
 
 // ---- batches of B problems in the tensor-core dimensions (tc_reduce_kernel / tc_bwd_kernel with BATCH) ----
 B200OT_API int64_t b200ot_batched_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
-  return tc_batched_dims(B, N, M, D) ? tc_scratch_bytes(N, M, D, B) : 0;
+  return tc_batched_dims(B, N, M, D) ? tc_scratch_bytes(N, M, D, B, 1) : 0;
 }
 
 B200OT_API int b200ot_kernel_conv_fwd_batched(const float* x, const float* y, const float* w, const float* center,
@@ -1013,7 +849,7 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float*
 
 // ---- above D = 64: the K-slab tensor-core kernels (tcwide.cuh), B >= 1 elements ----
 B200OT_API int64_t b200ot_wide_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
-  return tc_wide_dims(B, N, M, D) ? tc_wide_scratch_bytes(N, M, D, B) : 0;
+  return tc_wide_dims(B, N, M, D) ? tc_scratch_bytes(N, M, D, B, 2) : 0;
 }
 
 B200OT_API int b200ot_wide_softmin_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -1023,15 +859,9 @@ B200OT_API int b200ot_wide_softmin_fwd(const float* x, const float* y, const flo
                                        void* stream) {
   if (!x || !y || !h_a || !scratch || !tc_wide_dims(B, N, M, D) || !valid_p(p) || !(eps > 0.f) || (!out && !lse2_out))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  const float* coord_absmax = nullptr;
-  const int rc = softmin_wide_tc(false, x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps, scratch, &part,
-                                 &n_part, &coord_absmax, (cudaStream_t)stream);
-  if (rc) return rc;
-  return b200ot_softmin_finalize(part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
+  return softmin_fwd_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps}, nullptr,
+                        out_old, alpha_old, beta, out, lse2_out, scratch, stream);
 }
 
 B200OT_API int b200ot_wide_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -1042,19 +872,9 @@ B200OT_API int b200ot_wide_softmin_bwd_x(const float* x, const float* y, const f
   if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_wide_dims(B, N, M, D) || !valid_p(p) ||
       !(eps > 0.f))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  const float* coord_absmax = nullptr;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int rc = softmin_wide_tc(true, x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps, scratch, &part,
-                                 &n_part, &coord_absmax, st);
-  if (rc) return rc;
-  // P carries kTcPScale (p = 2) or 2^k_i (p = 1), which cancel: both finalizes divide by each row's sum of P
-  if (p_exponent(p) == 1)
-    return softmin_l1_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, coord_absmax, st);
-  return softmin_bwd_finalize_tc(part, n_part, x, center, grad_out, grad_x, B * N, D, eps, st);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
+  return softmin_bwd_x_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps}, nullptr,
+                          grad_out, grad_x, scratch, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_wide_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
@@ -1062,9 +882,9 @@ B200OT_API int b200ot_wide_kernel_conv_fwd(const float* x, const float* y, const
                                            float blur, void* scratch, int64_t scratch_bytes, void* stream) {
   if (!x || !y || !w || !out || !scratch || !tc_wide_dims(B, N, M, D) || !valid_kind(kind) || !blur_ok(kind, blur))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  return conv_wide_tc(false, kind, x, y, w, center, nullptr, out, B, N, M, D, blur, scratch, (cudaStream_t)stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
+  return conv_tc(false, TcLayout::kBatch, kind, x, y, w, center, nullptr, out, nullptr, B, N, M, D, blur, scratch,
+                 (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, const float* w, const float* center,
@@ -1074,9 +894,9 @@ B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, con
   if (!x || !y || !w || !grad_out || !grad_x || !scratch || !tc_wide_dims(B, N, M, D) || !valid_kind(kind) ||
       !blur_ok(kind, blur))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_wide_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  return conv_wide_tc(true, kind, x, y, w, center, grad_out, grad_x, B, N, M, D, blur, scratch, (cudaStream_t)stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
+  return conv_tc(true, TcLayout::kBatch, kind, x, y, w, center, grad_out, grad_x, nullptr, B, N, M, D, blur, scratch,
+                 (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -197,13 +197,15 @@ B200OT_API int32_t b200ot_softmin_num_splits(int64_t N, int64_t M, int32_t D) {
 
 B200OT_API int64_t b200ot_softmin_scratch_bytes(int64_t N, int64_t M, int32_t D) {
   if (N <= 0 || M <= 0 || D <= 0) return 0;
-  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D) : 0;
+  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D, 1, 1) : 0;
   const ReducePlan pl = make_plan(N, M, D);
   const int64_t cols = b200ot_packed_cols_floats(M, D, 1) * 4;
   // forward partials are (m, s) pairs; the backward pass keeps D+1 sums per (split, row)
   const int64_t part = (int64_t)pl.n_split * N * 4 * (D + 1 > 2 ? D + 1 : 2);
   const int64_t simt = round_up64(cols, 256) + round_up64(part, 256);
-  return tc_any_routed(D, N, M) ? (simt > tc_scratch_bytes(N, M, D) ? simt : tc_scratch_bytes(N, M, D)) : simt;
+  if (!tc_any_routed(D, N, M)) return simt;
+  const int64_t tc = tc_scratch_bytes(N, M, D, 1, 1);
+  return simt > tc ? simt : tc;
 }
 
 B200OT_API int b200ot_softmin_pack(const float* y, const float* h_a, const float* h_b, float h_scale_b,
@@ -289,16 +291,10 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
   if (!x || !y || !h_a || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) || !valid_p(p) ||
       !(eps > 0.f) || (!out && !lse2_out))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_softmin_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
-  if (tc) {
-    float* tc_part = nullptr;
-    int n_part = 0;
-    const int rc = softmin_partial_tc(x, y, h_a, h_b, h_scale_b, center, N, M, D, eps, scratch, &tc_part, &n_part,
-                                      (cudaStream_t)stream);
-    if (rc) return rc;
-    return b200ot_softmin_finalize(tc_part, n_part, out_old, alpha_old, beta, out, lse2_out, N, eps, stream);
-  }
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_scratch_bytes(N, M, D))) return rc;
+  if (tc)
+    return softmin_fwd_tc(TcLayout::kOne, {x, y, h_a, h_b, h_scale_b, center, nullptr, 1, N, M, D, p, eps}, nullptr,
+                          out_old, alpha_old, beta, out, lse2_out, scratch, stream);
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
@@ -320,19 +316,14 @@ B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const 
   if (!x || !y || !h_a || !scratch || !tc_batched_dims(B, N, M, D) || !valid_p(p) || p_exponent(p) != 2 ||
       !(eps > 0.f) || (!out && !lse2_out))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  float* tc_part = nullptr;
-  int n_part = 0;
-  const int rc = softmin_partial_tc(x, y, h_a, h_b, h_scale_b, center, N, M, D, eps, scratch, &tc_part, &n_part,
-                                    (cudaStream_t)stream, B, true);
-  if (rc) return rc;
-  return b200ot_softmin_finalize(tc_part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_batched_scratch_bytes(B, N, M, D))) return rc;
+  return softmin_fwd_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps}, nullptr,
+                        out_old, alpha_old, beta, out, lse2_out, scratch, stream);
 }
 
 // ---- the p = 1 softmin in the tensor-core dimensions (tc_reduce_kernel<6> / tc_bwd_kernel<7>, batched flavour) ----
 B200OT_API int64_t b200ot_softmin_l1_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
-  return tc_l1_args(B, N, M, D, 1) ? tc_l1_scratch_bytes(N, M, D, B) : 0;
+  return tc_l1_args(B, N, M, D, 1) ? tc_scratch_bytes(N, M, D, B, 2) : 0;
 }
 
 B200OT_API int b200ot_softmin_l1_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -342,15 +333,9 @@ B200OT_API int b200ot_softmin_l1_fwd(const float* x, const float* y, const float
                                      void* stream) {
   if (!x || !y || !h_a || !scratch || !tc_l1_args(B, N, M, D, p) || !(eps > 0.f) || (!out && !lse2_out))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_softmin_l1_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  const float* coord_absmax = nullptr;
-  const int rc = softmin_l1_tc(false, x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps, scratch, &part,
-                               &n_part, &coord_absmax, (cudaStream_t)stream);
-  if (rc) return rc;
-  return b200ot_softmin_finalize(part, n_part, out_old, alpha_old, beta, out, lse2_out, B * N, eps, stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_l1_scratch_bytes(B, N, M, D))) return rc;
+  return softmin_fwd_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps}, nullptr,
+                        out_old, alpha_old, beta, out, lse2_out, scratch, stream);
 }
 
 B200OT_API void b200ot_blocks_shape(int32_t* rows_per_segment, int32_t* col_align) {
@@ -361,11 +346,8 @@ B200OT_API void b200ot_blocks_shape(int32_t* rows_per_segment, int32_t* col_alig
 B200OT_API int64_t b200ot_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots,
                                                const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
                                                int32_t D) {
-  int max_tiles = 0;
-  int64_t n_pieces = 0;
-  if (blocks_check(N, n_row_slots, n_col_slots, seg, n_seg, pieces, D, 2, 1.f, nullptr, &max_tiles, &n_pieces))
-    return 0;
-  return tc_blocks_scratch_bytes(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D);
+  TcBlocks b{nullptr, nullptr, n_row_slots, n_col_slots, seg, n_seg, pieces};
+  return blocks_check(N, D, 2, 1.f, nullptr, b) ? 0 : tc_blocks_scratch_bytes(N, D, b);
 }
 
 B200OT_API int b200ot_softmin_fwd_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -376,20 +358,11 @@ B200OT_API int b200ot_softmin_fwd_blocks(const float* x, const float* y, const f
                                          int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
                                          void* stream) {
   if (!x || !y || !h_a || !row_src || !col_src || !scratch || (!out && !lse2_out)) return B200OT_EINVAL;
-  int max_tiles = 0;
-  int64_t n_pieces = 0;
-  const int rc =
-      blocks_check(N, n_row_slots, n_col_slots, seg, n_seg, pieces, D, p, eps, scratch, &max_tiles, &n_pieces);
-  if (rc) return rc;
-  if (scratch_bytes < tc_blocks_scratch_bytes(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D))
-    return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  const int rc2 = softmin_blocks_tc(false, x, y, h_a, h_b, h_scale_b, center, nullptr, N, row_src, n_row_slots, col_src,
-                                    n_col_slots, seg, n_seg, pieces, n_pieces, max_tiles, D, eps, scratch, &part,
-                                    &n_part, (cudaStream_t)stream);
-  if (rc2) return rc2;
-  return b200ot_softmin_finalize(part, n_part, out_old, alpha_old, beta, out, lse2_out, N, eps, stream);
+  TcBlocks b{row_src, col_src, n_row_slots, n_col_slots, seg, n_seg, pieces};
+  if (const int rc = blocks_check(N, D, p, eps, scratch, b)) return rc;
+  if (scratch_bytes < tc_blocks_scratch_bytes(N, D, b)) return B200OT_ESCRATCH;
+  return softmin_fwd_tc(TcLayout::kBlocks, {x, y, h_a, h_b, h_scale_b, center, nullptr, 1, N, 0, D, p, eps}, &b, out_old,
+                        alpha_old, beta, out, lse2_out, scratch, stream);
 }
 
 }  // extern "C"

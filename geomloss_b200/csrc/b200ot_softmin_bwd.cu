@@ -11,8 +11,6 @@
 #include "rowsum.cuh"
 #include "rowsum_launch.cuh"
 
-#include <type_traits>
-
 namespace b200ot {
 
 // part: (n_split, N, D+1) with [0] = sum w, [1+k] = sum w Y_k (p=2, scaled centred coords) or sum w u_k (p=1)
@@ -66,39 +64,6 @@ int softmin_bwd_finalize_tc(const float* part, int n_part, const float* x, const
       part, n_part, x, center, grad_out, grad_x, N, D, 2, 1.0f / softmin_coord_scale(2, eps));
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
-}
-
-template <int MODE, int D>
-static int launch_rowsum(const ReducePlan& pl, cudaStream_t st, const float* x, const float* center, float scale,
-                         float clampq, const float* cols, const float* lse2, float* part, int64_t N,
-                         const int4* tile_ptr = nullptr, const int2* tile_list = nullptr) {
-  if (pl.small) {
-    using C = RowSumCfg<MODE, D, kSmallR, kSmallNT, kSmallTJ, 3, 4>;
-    return launch_rowsum_kernel<C>(pl, st, x, center, scale, clampq, cols, lse2, part, N,
-                            pl.ntiles, pl.tiles_per_split, tile_ptr, tile_list);
-  }
-  // D >= 5: one row per thread (same 512 rows per CTA) keeps the 2 x (D+1) accumulator pairs in registers
-  using C = std::conditional_t<(D <= 4), RowSumCfg<MODE, D, kBigR, kBigNT, kBigTJ, 3, 2>,
-                               RowSumCfg<MODE, D, 1, kBigR * kBigNT, kBigTJ, 3, 1>>;
-  return launch_rowsum_kernel<C>(pl, st, x, center, scale, clampq, cols, lse2, part, N, pl.ntiles,
-                          pl.tiles_per_split, tile_ptr, tile_list);
-}
-
-template <int MODE>
-static int launch_rowsum_d(int D, const ReducePlan& pl, cudaStream_t st, const float* x, const float* center,
-                           float scale, float clampq, const float* cols, const float* lse2, float* part,
-                           int64_t N, const int4* seg = nullptr, const int2* pieces = nullptr) {
-  switch (D) {
-    case 1: return launch_rowsum<MODE, 1>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 2: return launch_rowsum<MODE, 2>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 3: return launch_rowsum<MODE, 3>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 4: return launch_rowsum<MODE, 4>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 5: return launch_rowsum<MODE, 5>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 6: return launch_rowsum<MODE, 6>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 7: return launch_rowsum<MODE, 7>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    case 8: return launch_rowsum<MODE, 8>(pl, st, x, center, scale, clampq, cols, lse2, part, N, seg, pieces);
-    default: return B200OT_EINVAL;
-  }
 }
 
 }  // namespace b200ot
@@ -163,22 +128,21 @@ B200OT_API int b200ot_softmin_bwd_finalize(const float* part, int32_t n_part, co
   return B200OT_OK;
 }
 
-// Runs pack + partial reduction of the row-gradient pass and leaves n_part sets of (N, D+1) sums in scratch, each
+// Runs pack + partial reduction of the row-gradient pass and leaves r->n_part sets of (N, D+1) sums in scratch, each
 // `*scale_out` times the softmax-weighted sums (kTcPScale on the tensor-core path, common.cuh; 1 otherwise).
 static int softmin_bwd_partials(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
                                 const float* center, const float* lse2, int64_t N, int64_t M, int32_t D, int32_t p,
-                                float eps, void* scratch, int64_t scratch_bytes, void* stream, float** part_out,
-                                int* n_part_out, float* scale_out) {
+                                float eps, void* scratch, int64_t scratch_bytes, void* stream, TcPass* r,
+                                float* scale_out) {
   const bool tc = p_exponent(p) == 2 && tc_routed(kTcSoftminBwd, D, N, M);
   if (!x || !y || !h_a || !lse2 || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) || !valid_p(p) ||
       !(eps > 0.f))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_softmin_scratch_bytes(N, M, D)) return B200OT_ESCRATCH;
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_scratch_bytes(N, M, D))) return rc;
   *scale_out = tc ? kTcPScale : 1.f;
   if (tc)
-    return bwd_partial_tc(3, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M, D,
-                          scratch, part_out, n_part_out, (cudaStream_t)stream);
+    return softmin_pass_tc(true, TcLayout::kOne, {x, y, h_a, h_b, h_scale_b, center, lse2, 1, N, M, D, p, eps}, nullptr,
+                           scratch, (cudaStream_t)stream, r);
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
@@ -186,8 +150,8 @@ static int softmin_bwd_partials(const float* x, const float* y, const float* h_a
   int rc = softmin_pack_impl(y, h_a, h_b, h_scale_b, center, M, D, p, eps, cols, (cudaStream_t)stream, nullptr);
   if (rc) return rc;
   rc = b200ot_softmin_bwd_partial(x, center, cols, lse2, part, pl.n_split, N, M, D, p, eps, stream);
-  *part_out = part;
-  *n_part_out = pl.n_split;
+  r->part = part;
+  r->n_part = pl.n_split;
   return rc;
 }
 
@@ -196,14 +160,13 @@ B200OT_API int b200ot_softmin_bwd_sums(const float* x, const float* y, const flo
                                        int64_t N, int64_t M, int32_t D, int32_t p, float eps, void* scratch,
                                        int64_t scratch_bytes, void* stream) {
   if (!sums) return B200OT_EINVAL;
-  float* part = nullptr;
-  int n_part = 0;
+  TcPass r;
   float p_scale = 1.f;
   const int rc = softmin_bwd_partials(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch,
-                                      scratch_bytes, stream, &part, &n_part, &p_scale);
+                                      scratch_bytes, stream, &r, &p_scale);
   if (rc) return rc;
   // raw sums leave the library (the multi-GPU engine adds them over the column shards): undo the P scale here
-  return rowsum_merge(part, n_part, D + 1, sums, N, 1.f / p_scale, (cudaStream_t)stream);
+  return rowsum_merge(r.part, r.n_part, D + 1, sums, N, 1.f / p_scale, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -211,13 +174,12 @@ B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float*
                                     float* grad_x, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
                                     void* scratch, int64_t scratch_bytes, void* stream) {
   if (!grad_out || !grad_x) return B200OT_EINVAL;
-  float* part = nullptr;
-  int n_part = 0;
+  TcPass r;
   float p_scale = 1.f;  // cancels: the finalize divides by the row sum of P
   const int rc = softmin_bwd_partials(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch,
-                                      scratch_bytes, stream, &part, &n_part, &p_scale);
+                                      scratch_bytes, stream, &r, &p_scale);
   if (rc) return rc;
-  return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
+  return b200ot_softmin_bwd_finalize(r.part, r.n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -228,15 +190,9 @@ B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, cons
   if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_batched_dims(B, N, M, D) || !valid_p(p) ||
       p_exponent(p) != 2 || !(eps > 0.f))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_batched_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  // P carries kTcPScale, which cancels: the finalize divides by each row's sum of P
-  const int rc = bwd_partial_tc(3, x, y, nullptr, h_a, h_b, h_scale_b, lse2, center, softmin_coord_scale(2, eps), N, M,
-                                D, scratch, &part, &n_part, (cudaStream_t)stream, B, true);
-  if (rc) return rc;
-  return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, p, eps, stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_batched_scratch_bytes(B, N, M, D))) return rc;
+  return softmin_bwd_x_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps}, nullptr,
+                          grad_out, grad_x, scratch, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_l1_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -245,16 +201,9 @@ B200OT_API int b200ot_softmin_l1_bwd_x(const float* x, const float* y, const flo
                                        void* scratch, int64_t scratch_bytes, void* stream) {
   if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_l1_args(B, N, M, D, p) || !(eps > 0.f))
     return B200OT_EINVAL;
-  if (((uintptr_t)scratch) & 15) return B200OT_EALIGN;
-  if (scratch_bytes < b200ot_softmin_l1_scratch_bytes(B, N, M, D)) return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  const float* coord_absmax = nullptr;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int rc = softmin_l1_tc(true, x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps, scratch, &part,
-                               &n_part, &coord_absmax, st);
-  if (rc) return rc;
-  return softmin_l1_bwd_finalize(part, n_part, x, center, grad_out, grad_x, B * N, D, coord_absmax, st);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_l1_scratch_bytes(B, N, M, D))) return rc;
+  return softmin_bwd_x_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps}, nullptr,
+                          grad_out, grad_x, scratch, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_x_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -265,21 +214,11 @@ B200OT_API int b200ot_softmin_bwd_x_blocks(const float* x, const float* y, const
                                            int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
                                            void* stream) {
   if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !row_src || !col_src || !scratch) return B200OT_EINVAL;
-  int max_tiles = 0;
-  int64_t n_pieces = 0;
-  const int rc =
-      blocks_check(N, n_row_slots, n_col_slots, seg, n_seg, pieces, D, p, eps, scratch, &max_tiles, &n_pieces);
-  if (rc) return rc;
-  if (scratch_bytes < tc_blocks_scratch_bytes(N, n_row_slots, n_col_slots, n_seg, n_pieces, max_tiles, D))
-    return B200OT_ESCRATCH;
-  float* part = nullptr;
-  int n_part = 0;
-  // P carries kTcPScale, which cancels: the finalize divides by each row's sum of P
-  const int rc2 = softmin_blocks_tc(true, x, y, h_a, h_b, h_scale_b, center, lse2, N, row_src, n_row_slots, col_src,
-                                    n_col_slots, seg, n_seg, pieces, n_pieces, max_tiles, D, eps, scratch, &part,
-                                    &n_part, (cudaStream_t)stream);
-  if (rc2) return rc2;
-  return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
+  TcBlocks b{row_src, col_src, n_row_slots, n_col_slots, seg, n_seg, pieces};
+  if (const int rc = blocks_check(N, D, p, eps, scratch, b)) return rc;
+  if (scratch_bytes < tc_blocks_scratch_bytes(N, D, b)) return B200OT_ESCRATCH;
+  return softmin_bwd_x_tc(TcLayout::kBlocks, {x, y, h_a, h_b, h_scale_b, center, lse2, 1, N, 0, D, p, eps}, &b,
+                          grad_out, grad_x, scratch, (cudaStream_t)stream);
 }
 
 }  // extern "C"
