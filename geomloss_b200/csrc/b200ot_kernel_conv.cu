@@ -535,25 +535,41 @@ static int conv_tc(bool bwd, TcLayout layout, int kind, const float* x, const fl
   return B200OT_OK;
 }
 
-// The plan applied to a value matrix (tcapply.cuh): the images and splits of the softmin row gradient's plan, and
+// The plan applied to a value matrix (tcapply.cuh): the images and splits of the softmin row gradient's plan, one CTA
+// per row tile and split whatever D (no D slices above 64: GEMM 2 reads the value image, not a column slab), and
 // behind the images the partials (n_split, N, 1 + min(K, 64)), one slab's value image and the K column maxima of V.
 // V wider than 64 columns runs in slabs of 64 (the last one padded to a multiple of 16), each a pass of its own over
-// the pairs through the same partials and value image.  A ring stage holds a column tile and the slab's value image:
-// at dk = 64 and 64 value columns 36.5 + 32 KB, two stages next to the 36 KB row image.
+// the pairs through the same images, partials and value image.  A ring stage holds, up to D = 64, a column tile and
+// the slab's value image: at dk = 64 and 64 value columns 36.5 + 32 KB, two stages next to the 36 KB row image.  Above
+// D = 64 it is a K slab of tcwide.cuh (64 KB) with a value slot of its own next to the column tail: at 64 value
+// columns 14 KB (row tail, column tails, barriers) + 2 x (64 + 32) KB = 206 KB, where a third stage would take 302.
 struct TcApplyPlan {
   TcPlan p;
+  bool wide;
   int64_t off_v, off_vmax, total;
 };
 static int tc_apply_dkv(int K, int k0) { return tc_dk(std::min(64, K - k0)); }
-static void tc_apply_stages(int kp, int dkv, int* nstage, int64_t* smem) {
+static void tc_apply_stages(bool wide, int kp, int dkv, int* nstage, int64_t* smem) {
+  const int64_t v_bytes = tc_value_img_bytes(dkv);
+  if (wide) {
+    int ns = kTcMaxStage;
+    while (ns > 0 && tc_wide_smem(ns) + ns * v_bytes > 227 * 1024) --ns;
+    *nstage = ns;
+    *smem = tc_wide_smem(ns) + ns * v_bytes;
+    return;
+  }
   const int64_t bar_bytes = 256, b_bytes = tc_b_img_bytes(kp, kTcBN);
-  const int64_t ns = (227 * 1024 - bar_bytes - tc_a_span(kp)) / (b_bytes + tc_value_img_bytes(dkv));
+  const int64_t ns = (227 * 1024 - bar_bytes - tc_a_span(kp)) / (b_bytes + v_bytes);
   *nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
-  *smem = tc_a_span(kp) + *nstage * (b_bytes + tc_value_img_bytes(dkv)) + bar_bytes;
+  *smem = tc_a_span(kp) + *nstage * (b_bytes + v_bytes) + bar_bytes;
 }
 static TcApplyPlan make_tc_apply_plan(int64_t N, int64_t M, int D, int K) {
   TcApplyPlan a;
-  a.p = make_tc_plan(N, M, D, true);
+  const int64_t rtpe = ceil_div64(N, kTcM), ctpe = ceil_div64(M, kTcBN);
+  a.p = make_tc_plan(D, true, rtpe, ctpe, rtpe, ctpe, N, 2 * 4);
+  a.p.rtpe = (int)rtpe;
+  a.p.ctpe = (int)ctpe;
+  a.wide = D > 64;
   a.off_v = a.p.off_part + round_up64((int64_t)a.p.n_split * N * (1 + std::min(K, 64)) * 4, 256);
   a.off_vmax = a.off_v + round_up64(a.p.b_tiles * tc_value_img_bytes(tc_apply_dkv(K, 0)), 256);
   a.total = a.off_vmax + round_up64((int64_t)K * 4, 256);
@@ -566,13 +582,14 @@ template <int DKV>
 static int tc_apply_launch(const TcApplyPlan& a, unsigned char* base, int64_t N, int kv, cudaStream_t st) {
   int nstage;
   int64_t smem;
-  tc_apply_stages(a.p.kp, DKV, &nstage, &smem);
+  tc_apply_stages(a.wide, a.p.kp, DKV, &nstage, &smem);
   if (nstage < 2) return B200OT_EINVAL;
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(tc_apply_kernel<DKV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const auto kern = a.wide ? tc_wide_apply_kernel<DKV> : tc_apply_kernel<DKV>;
+  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const dim3 grid((unsigned)a.p.ctas, (unsigned)a.p.n_split);
-  tc_apply_kernel<DKV><<<grid, kTcThreads, (size_t)smem, st>>>(base, base + a.p.off_b, base + a.off_v,
-                                                              reinterpret_cast<float*>(base + a.p.off_part), N,
-                                                              a.p.kp, a.p.ctpe, a.p.tiles_per_split, nstage, kv);
+  kern<<<grid, kTcThreads, (size_t)smem, st>>>(base, base + a.p.off_b, base + a.off_v,
+                                               reinterpret_cast<float*>(base + a.p.off_part), N, a.p.kp, a.p.ctpe,
+                                               a.p.tiles_per_split, nstage, kv);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }

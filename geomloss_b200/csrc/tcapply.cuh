@@ -17,8 +17,11 @@
 // s_k is the power of two that puts max_j |V_jk| in [2^9, 2^10) (tc_energy_coord_scale, found on the device by
 // col_absmax_kernel): both fp16 terms of an entry down to 2^-13 of its column's largest stay in fp16's normal
 // range, whatever the unit of the column; the finalize divides by s_k exactly.
+//
+// Above D = 64 (tc_wide_apply_kernel): the same GEMM 2 and epilogue behind the K-slab exponent of tcwide.cuh.
 #pragma once
 #include "tcbwd.cuh"
+#include "tcwide.cuh"
 
 namespace b200ot {
 
@@ -108,6 +111,65 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     reg_fence(g);
     __syncwarp();
     if (lane == 0) mbar_arrive(&c.empty_b[st]);  // column tile and value image may be overwritten
+  }
+  tc_bwd_store<3, DKV, false, false>(part, g, sum, sumq, row0, c.split, 0, 0, 0, nullptr, N, KV, 0, true, cq);
+}
+
+// tc_apply_kernel above D = 64 (64 < D <= B200OT_MAX_D_WIDE), with its arguments (kp is the image's): the exponent of
+// tc_wide_reduce_kernel (row tail resident, slabs streamed in natural order through the ring, lse2 in the row tail as
+// for tc_wide_bwd_kernel<3>), then tc_bwd_tile<3> and GEMM 2 against the value image.  Unlike the D-sliced row
+// gradient, GEMM 2 reads no column slab, so one CTA per row tile and split serves every value column of the slab.
+// The tile's value image rides with its last slab (tc_wide_produce<true>): one value slot per ring stage, behind the
+// ring, released with that stage once GEMM 2 has read it.
+template <int DKV>
+__global__ void __launch_bounds__(kTcThreads, 1)
+    tc_wide_apply_kernel(const unsigned char* __restrict__ a_imgs, const unsigned char* __restrict__ b_imgs,
+                         const unsigned char* __restrict__ v_imgs, float* __restrict__ part, int64_t N, int kp,
+                         int ntiles_b, int tiles_per_split, int NSTAGE, int KV) {
+  static_assert(DKV % 16 == 0 && DKV <= 64, "padded slab width");
+  extern __shared__ __align__(1024) unsigned char smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // the prologue with a 16-wide "image": the row tail in sa, one column tail per stage in sb (as tcwide.cuh)
+  const TcCta c = tc_cta_prologue<false, false>(smem, 16, NSTAGE, ntiles_b, tiles_per_split, 0, nullptr, nullptr);
+  unsigned char* ring = smem + tc_wide_ring_off(NSTAGE);
+  constexpr int v_bytes = kTcTerms * DKV * kTcBN * 2;
+  unsigned char* sv = ring + (int64_t)NSTAGE * kTcWideStageBytes;  // the value slots
+  const int seg = tc_dk_of_kp(kp) / 8;
+  const int nslab = (seg + kTcWideSlabChunks - 1) / kTcWideSlabChunks;
+  if (warp == 4 * kTcWG) {
+    tc_wide_produce<true>(c, a_imgs, b_imgs, ring, kp, nslab - 1, nslab, NSTAGE, lane, v_imgs, sv, v_bytes);
+    return;
+  }
+  const int wg = warp >> 2;
+  const int64_t row0 = (int64_t)c.row_tile * kTcM + wg * 64 + (warp & 3) * 16 + (lane >> 2);  // and row0 + 8
+  const int cq = 2 * (lane & 3);
+  float g[DKV];  // [G_a | G_b], as tc_apply_kernel
+#pragma unroll
+  for (int i = 0; i < DKV; ++i) g[i] = 0.f;
+  float sum[2] = {0.f, 0.f}, sumq[2] = {0.f, 0.f};
+  const float tb[2] = {0.f, 0.f};
+  const float2 rt[2] = {};
+  mbar_wait(c.bar_a, 0);
+  int step = 0;
+  for (int k = 0; k < c.nt; ++k) {
+    float s[64];
+    const int st = tc_wide_exponent(s, c, ring, seg, nslab - 1, nslab, NSTAGE, wg, lane, step);
+    uint32_t ph[32], pl[32];
+    tc_bwd_tile<3>(s, c, st, 16, k, row0, tb, rt, 0.f, 0, cq, ph, pl, sum, sumq);
+    // ---- GEMM 2: G += P . V from the value slot of the last slab's stage ----
+    const uint32_t v_addr = smem_u32(sv + st * v_bytes);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kTcBN / 16; ++kk) {
+      const uint64_t db = make_smem_desc(v_addr + (2 * kk) * 128, 128, kTcBN * 16);
+      wgmma_rs<2 * DKV>(g, &ph[4 * kk], db);
+      wgmma_rs<DKV>(g, &pl[4 * kk], db);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(g);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&c.empty_b[st]);  // slab, column tail and value image may be overwritten
   }
   tc_bwd_store<3, DKV, false, false>(part, g, sum, sumq, row0, c.split, 0, 0, 0, nullptr, N, KV, 0, true, cq);
 }

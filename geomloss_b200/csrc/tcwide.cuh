@@ -67,15 +67,21 @@ __device__ __forceinline__ int tc_wide_slab_at(int j, int own, int nslab) {
 }
 
 // The producer lane: the row tail once, then for every column tile of the CTA its slabs through the ring, the
-// column tail with the last one
+// column tail with the last one.  VALUES (tc_wide_apply_kernel): the tile's value image of e_bytes (tile ct at
+// e_imgs + ct e_bytes) rides with the last slab as well, into slot `st` of a ring of its own at e_ring, its bytes in
+// that stage's expect_tx.
+template <bool VALUES = false>
 __device__ __forceinline__ void tc_wide_produce(const TcCta& c, const unsigned char* __restrict__ a_imgs,
                                                 const unsigned char* __restrict__ b_imgs, unsigned char* ring,
-                                                int kp, int own, int nslab, int NSTAGE, int lane) {
+                                                int kp, int own, int nslab, int NSTAGE, int lane,
+                                                const unsigned char* __restrict__ e_imgs = nullptr,
+                                                unsigned char* e_ring = nullptr, int e_bytes = 0) {
   if (lane != 0) return;
   const int seg = tc_dk_of_kp(kp) / 8;
   const unsigned char* arow = a_imgs + (int64_t)c.row_tile * tc_a_img_bytes(kp);
   mbar_arrive_expect_tx(c.bar_a, c.a_bytes);
   tma_load_1d(c.sa, arow + (int64_t)kTcTerms * seg * kTcM * 16, c.a_bytes, c.bar_a);
+  const int tail = VALUES ? c.b_bytes + e_bytes : c.b_bytes;  // bytes that ride with a tile's last slab
   int step = 0;
   for (int k = 0; k < c.nt; ++k) {
     const unsigned char* bcol = b_imgs + (int64_t)(c.t0 + k) * tc_b_img_bytes(kp, kTcBN);
@@ -85,7 +91,7 @@ __device__ __forceinline__ void tc_wide_produce(const TcCta& c, const unsigned c
       const bool last = j == nslab - 1;
       const int st = step % NSTAGE;
       if (step >= NSTAGE) mbar_wait(&c.empty_b[st], ((step / NSTAGE) + 1) & 1);
-      mbar_arrive_expect_tx(&c.full_b[st], 4 * bytes + (last ? c.b_bytes : 0));
+      mbar_arrive_expect_tx(&c.full_b[st], 4 * bytes + (last ? tail : 0));
       unsigned char* dst = ring + (int64_t)st * kTcWideStageBytes;
 #pragma unroll
       for (int t = 0; t < kTcTerms; ++t) {
@@ -93,8 +99,11 @@ __device__ __forceinline__ void tc_wide_produce(const TcCta& c, const unsigned c
         tma_load_1d(dst + t * kTcWideTermBytes, arow + off, bytes, &c.full_b[st]);
         tma_load_1d(dst + (kTcTerms + t) * kTcWideTermBytes, bcol + off, bytes, &c.full_b[st]);
       }
-      if (last)
+      if (last) {
         tma_load_1d(c.sb + st * c.b_bytes, bcol + (int64_t)kTcTerms * seg * kTcBN * 16, c.b_bytes, &c.full_b[st]);
+        if constexpr (VALUES)
+          tma_load_1d(e_ring + (int64_t)st * e_bytes, e_imgs + (int64_t)(c.t0 + k) * e_bytes, e_bytes, &c.full_b[st]);
+      }
     }
   }
 }

@@ -652,6 +652,34 @@ def softmin_wide_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=
     return gx
 
 
+def plan_apply_wide_raw(eps, x, y, h_a, h_b, h_scale_b, lse2, v, *, row_factor=None, center=None):
+    """``plan_apply_raw`` above D = 64 (b200ot_wide_plan_apply): ``out[i, k] = row_factor_i * sum_j w_ij v[j, k]`` for
+    (N,D) / (M,D) clouds, ``lse2`` from ``softmin_wide_raw(..., want_lse2=True)`` with the same arguments.  ``v`` is
+    (M,) or (M, K), any sign, any strides; p = 2.  One pass over the pairs per slab of 64 value columns, each
+    recomputing the full-K exponent.  No autograd.  Returns (N,) or (N, K)."""
+    if x.dim() != 2 or y.dim() != 2:
+        raise ValueError(f"expected x:(N,D), y:(M,D); got {tuple(x.shape)}, {tuple(y.shape)}")
+    _, (_, N, M, D) = _wide_args(x, y)
+    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
+    center, lse2, v = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(v, "v")
+    row_factor = _f32c(row_factor, "row_factor")
+    if v.dim() not in (1, 2) or v.shape[0] != M or v.numel() == 0:
+        raise ValueError(f"v must be (M,) or (M, K) with M = {M} and K >= 1, got {tuple(v.shape)}")
+    _per_point(h_a, M, "h_a")
+    _per_point(h_b, M, "h_b")
+    if lse2.numel() != N or (row_factor is not None and row_factor.numel() != N):
+        raise ValueError("lse2 and row_factor must have one entry per row")
+    K = 1 if v.dim() == 1 else v.shape[1]
+    dev = x.device
+    with nvtx_range(f"b200ot.plan_apply_wide N={N} M={M} D={D} K={K}"):
+        out = torch.empty((N,) if v.dim() == 1 else (N, K), dtype=torch.float32, device=dev)
+        scratch = _scratch(_query(dev, "b200ot_wide_plan_apply_scratch_bytes", N, M, D, K), dev, "plan_apply")
+        # two packs, the column maxima of v, then value pack, reduction and finalize per slab of 64 columns
+        _call(dev, "b200ot_wide_plan_apply", x, y, h_a, h_b, float(h_scale_b), center, lse2, v, row_factor, out, N, M,
+              D, K, 2, float(eps), scratch, scratch.numel(), launches=3 + 3 * -(-K // 64))
+    return out
+
+
 def softmin_wide(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
     """Differentiable (w.r.t. x) ``scale_out * softmin_wide_raw(...)``, for (N,D) or (B,N,D) clouds."""
     return _softmin_apply(softmin_wide_raw, softmin_wide_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center,

@@ -2,8 +2,9 @@
 
 The reference's "new API" for point clouds (src/geomloss/ot/_implementations/sample.py:190-395) builds dense (N, M)
 cost matrices and runs ``sinkhorn_loop`` (ot/_abstract_solvers/sinkhorn_ot.py:240-447) on them.  Here the same
-iteration runs on the fused on-the-fly softmin of ``ops.softmin_raw`` (never an N x M matrix), so the facade works
-at N = M = 1e6 like the rest of the engine.  Conventions of THIS API (they differ from ``SamplesLoss``):
+iteration runs on the fused on-the-fly softmin of ``ops.softmin_raw`` (``ops.softmin_wide_raw`` for 64 < D <= 1024;
+never an N x M matrix), so the facade works at N = M = 1e6 like the rest of the engine.  Conventions of THIS API (they
+differ from ``SamplesLoss``):
 
 * cost ``"sqeuclidean"`` is ``C(x, y) = |x - y|^2`` — no 1/2 (sample.py:38-66); ``reg`` is the temperature eps and
   ``unbalanced`` the marginal penalty rho, used as given; ``blur`` / ``reach`` are shortcuts for ``2 blur^2`` /
@@ -89,18 +90,43 @@ def annealing_eps(maxmin_cost, eps, n_iter):
 # the solver
 # ----------------------------------------------------------------------------------------------------
 class _Softmin:
-    """``softmin_sample`` (sample.py:91-182) for the four (rows, columns) pairs of one problem, on the kernel."""
+    """``softmin_sample`` (sample.py:91-182) for the four (rows, columns) pairs of one problem, on the kernel.
+
+    It also picks, from D, the three operators every pass of the facade runs: the forward softmin (``fwd``), its row
+    gradient (``grad_rows``) and the plan applied to a value matrix (``apply``) — ``softmin_raw`` / ``softmin_grad_rows``
+    / ``plan_apply_raw`` up to D = 64, ``softmin_wide_raw`` / ``softmin_wide_grad_rows`` / ``plan_apply_wide_raw`` up to
+    D = 1024.  They are looked up in ``ops`` at every call, not bound once."""
 
     def __init__(self, X_a, X_b):
+        self.D = X_a.shape[1]
+        if self.D > ops.MAX_D_WIDE:
+            raise NotImplementedError(f"solve_sample serves D <= {ops.MAX_D_WIDE}, got D = {self.D} (no kernel of this "
+                                      f"build reduces clouds above D = {ops.MAX_D_WIDE})")
         self.center = ops.default_center(X_a, X_b)
         self.X_a, self.X_b = X_a, X_b
+
+    @property
+    def wide(self):
+        return self.D > ops.MAX_D_TC
+
+    @property
+    def fwd(self):
+        return ops.softmin_wide_raw if self.wide else ops.softmin_raw
+
+    @property
+    def grad_rows(self):
+        return ops.softmin_wide_grad_rows if self.wide else ops.softmin_grad_rows
+
+    @property
+    def apply(self):
+        return ops.plan_apply_wide_raw if self.wide else ops.plan_apply_raw
 
     def __call__(self, eps, x, y, log_w, pot, *, damp=1.0, old=None):
         """damp * softmin(eps, log_w, C(x, y), pot), or its average with ``old`` (the symmetric Sinkhorn update)."""
         if old is None:
-            return ops.softmin_raw(0.5 * eps, x, y, log_w, pot, 1.0 / eps, p=2, center=self.center, beta=2.0 * damp)[0]
-        return ops.softmin_raw(0.5 * eps, x, y, log_w, pot, 1.0 / eps, p=2, center=self.center, out_old=old,
-                               alpha_old=0.5, beta=damp)[0]
+            return self.fwd(0.5 * eps, x, y, log_w, pot, 1.0 / eps, p=2, center=self.center, beta=2.0 * damp)[0]
+        return self.fwd(0.5 * eps, x, y, log_w, pot, 1.0 / eps, p=2, center=self.center, out_old=old, alpha_old=0.5,
+                        beta=damp)[0]
 
     def at_infinity(self, x, y, w_rows, w_cols, damp):
         """eps = +inf: f_i = sum_j w_j |x_i - y_j|^2 / sum_j w_j by moments (fp64, centred), then the reference's
@@ -124,22 +150,23 @@ class _LastUpdate(torch.autograd.Function):
       potential softmin_i), one extra softmin for its normaliser W; signed u is split into its two parts."""
 
     @staticmethod
-    def forward(ctx, rows, cols, log_w, pot, eps, damp, center):
-        out, lse2 = ops.softmin_raw(0.5 * eps, rows.detach(), cols.detach(), log_w, pot, 1.0 / eps, p=2, center=center,
-                                    beta=2.0 * damp, want_lse2=True)
-        ctx.save_for_backward(rows.detach(), cols.detach(), log_w, pot, out, lse2, center)
-        ctx.meta = (float(eps), float(damp))
+    def forward(ctx, rows, cols, log_w, pot, eps, damp, sm):
+        out, lse2 = sm.fwd(0.5 * eps, rows.detach(), cols.detach(), log_w, pot, 1.0 / eps, p=2, center=sm.center,
+                           beta=2.0 * damp, want_lse2=True)
+        ctx.save_for_backward(rows.detach(), cols.detach(), log_w, pot, out, lse2)
+        ctx.meta = (float(eps), float(damp), sm)
         return out
 
     @staticmethod
     def backward(ctx, go):
-        rows, cols, log_w, pot, out, lse2, center = ctx.saved_tensors
-        eps, damp = ctx.meta
+        rows, cols, log_w, pot, out, lse2 = ctx.saved_tensors
+        eps, damp, sm = ctx.meta
+        center = sm.center
         e2, inv = 0.5 * eps, 1.0 / eps
         u_all = (damp * go).float().contiguous()
         g_rows = g_cols = None
         if ctx.needs_input_grad[0]:
-            g_rows = ops.softmin_grad_rows(e2, rows, cols, log_w, pot, inv, lse2, 2.0 * u_all, p=2, center=center)
+            g_rows = sm.grad_rows(e2, rows, cols, log_w, pot, inv, lse2, 2.0 * u_all, p=2, center=center)
         if ctx.needs_input_grad[1]:
             sm_und = out / damp  # undamped softmin values, new-API scale
             g_cols = torch.zeros_like(cols)
@@ -148,10 +175,10 @@ class _LastUpdate(torch.autograd.Function):
                 if not bool((u > 0).any()):
                     continue
                 lu = log_weights(u)
-                sm_t, lse2_t = ops.softmin_raw(e2, cols, rows, lu, sm_und, inv, p=2, center=center, want_lse2=True)
+                sm_t, lse2_t = sm.fwd(e2, cols, rows, lu, sm_und, inv, p=2, center=center, want_lse2=True)
                 W = torch.exp((log_w.double() + pot.double() * inv - sm_t.double() / e2)).float()
-                g_cols = g_cols + sign * ops.softmin_grad_rows(e2, cols, rows, lu, sm_und, inv, lse2_t,
-                                                               (2.0 * W).contiguous(), p=2, center=center)
+                g_cols = g_cols + sign * sm.grad_rows(e2, cols, rows, lu, sm_und, inv, lse2_t, (2.0 * W).contiguous(),
+                                                      p=2, center=center)
         return g_rows, g_cols, None, None, None, None, None
 
 
@@ -233,7 +260,7 @@ def solve_sample(X_a, X_b, a=None, b=None, cost="sqeuclidean", debias=False, reg
     if want_grad:
         # the same update, attached to the caller's clouds through the cost (both arguments of every softmin)
         xa, xb = live[0], live[1]
-        last = lambda rows, cols, lw, pot: _LastUpdate.apply(rows, cols, lw, pot, eps, lam, sm.center)  # noqa: E731
+        last = lambda rows, cols, lw, pot: _LastUpdate.apply(rows, cols, lw, pot, eps, lam, sm)  # noqa: E731
         new_f, new_g = last(xa, xb, log_b, g_ab), last(xb, xa, log_a, f_ba)
         f_ba, g_ab = new_f, new_g
         if debias:
@@ -355,7 +382,8 @@ class OTResultSample:
     #   sum_j w_j exp((f_i + g_j - C_ij) / reg) s_jk = exp((f_i - sm_i) / reg) * sum_j w_ij s_jk      (w = exp(log_w))
     # so (density @ s) takes log_w = 0 and (plan @ s) takes w = b and the row factor a_i exp((f_i - sm_i) / reg), which
     # is the plan's marginal.  One forward softmin per (direction, weighting) gives lse2 and the row factor; after
-    # that every application is ONE call of ops.plan_apply_raw, for any number of columns and any signs.
+    # that every application is ONE call of ops.plan_apply_raw (plan_apply_wide_raw above D = 64), for any number of
+    # columns and any signs.
     def _apply_state(self, transpose, weighted):
         """(log_w, lse2, row_factor) of the operator's direction, cached until ``cache_clear``."""
         cache = self.__dict__.setdefault("_apply_cache", {})
@@ -367,8 +395,8 @@ class OTResultSample:
             w_rows, w_cols = (self._b, self._a) if transpose else (self._a, self._b)
             with torch.no_grad():
                 log_w = log_weights(w_cols) if weighted else torch.zeros_like(w_cols)
-                smv, lse2 = ops.softmin_raw(0.5 * eps, rows, cols, log_w, g, 1.0 / eps, p=2, center=self._sm.center,
-                                            beta=2.0, want_lse2=True)
+                smv, lse2 = self._sm.fwd(0.5 * eps, rows, cols, log_w, g, 1.0 / eps, p=2, center=self._sm.center,
+                                         beta=2.0, want_lse2=True)
                 factor = torch.exp((f - smv) / eps)
                 if weighted:
                     factor = w_rows * factor
@@ -382,8 +410,8 @@ class OTResultSample:
         g = self._f_ba if transpose else self._g_ab
         log_w, lse2, factor = self._apply_state(transpose, weighted)
         with torch.no_grad():
-            return ops.plan_apply_raw(0.5 * self._reg, rows, cols, log_w, g, 1.0 / self._reg, lse2, s.detach().float(),
-                                      row_factor=None if normalized else factor, center=self._sm.center)
+            return self._sm.apply(0.5 * self._reg, rows, cols, log_w, g, 1.0 / self._reg, lse2, s.detach().float(),
+                                  row_factor=None if normalized else factor, center=self._sm.center)
 
     def _density_matmat(self, s, transpose, weighted=False):
         """(density @ s), or (plan @ s) when ``weighted``; differentiable w.r.t. s when it requires a gradient."""

@@ -317,6 +317,17 @@ B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, con
                                              const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
                                              int32_t D, int32_t kind, float blur, void* scratch,
                                              int64_t scratch_bytes, void* stream);
+/* The plan applied to a value matrix above D = 64: b200ot_plan_apply's arguments, contract and results for one problem
+ * (B = 1) with 64 < D <= B200OT_MAX_D_WIDE, p = 2 (| B200OT_P_UNCLAMPED), K >= 1; lse2 is the lse2_out of
+ * b200ot_wide_softmin_fwd for the same x, y, h, center, eps.  One pass over the pairs per slab of 64 value columns,
+ * each recomputing the full-K exponent on the K-slab kernels.  EINVAL (before any launch) for null pointers, N or
+ * M <= 0, D <= 64 or D > B200OT_MAX_D_WIDE, K < 1, a bad p, eps <= 0; EALIGN for a misaligned scratch; ESCRATCH below
+ * b200ot_wide_plan_apply_scratch_bytes(N, M, D, K) (0 for a shape this entry refuses). */
+B200OT_API int64_t b200ot_wide_plan_apply_scratch_bytes(int64_t N, int64_t M, int32_t D, int64_t K);
+B200OT_API int b200ot_wide_plan_apply(const float* x, const float* y, const float* h_a, const float* h_b,
+                                      float h_scale_b, const float* center, const float* lse2, const float* v,
+                                      const float* row_factor, float* out, int64_t N, int64_t M, int32_t D, int64_t K,
+                                      int32_t p, float eps, void* scratch, int64_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Block-sparse softmins in the tensor-core dimensions (8 < D <= 64, p = 2 or 2 | B200OT_P_UNCLAMPED): the fine phase

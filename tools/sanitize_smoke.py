@@ -31,7 +31,7 @@ def check(name, got, ref, tol=2e-5):
 
 
 which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "wide", "blocks", "grid", "loss",
-                              "small", "apply"}
+                              "small", "apply", "apply_wide"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -280,5 +280,19 @@ if "apply" in which:
         out = ops.plan_apply_raw(eps, xd, yd, hd, None, 0.0, lse2, v.to(DEV), center=center)
         d2 = ((x[:, None, :].double() - y[None, :, :].double()) ** 2).sum(-1)
         check("apply_" + tag, out, torch.softmax(h.double()[None, :] - d2 / (2 * eps), dim=1) @ v.double(), 2e-4)
+if "apply_wide" in which:
+    # above D = 64 (tc_wide_apply_kernel): a partial last K slab (D = 200), a value image of 16 columns and one of 64
+    # plus a second slab (K = 70)
+    for d, k in ((200, 5), (96, 70)):
+        x, y, h = torch.rand(300, d, generator=g), torch.rand(700, d, generator=g), torch.randn(700, generator=g)
+        v = torch.randn(700, k, generator=g)
+        xd, yd, hd = x.to(DEV), y.to(DEV), h.to(DEV)
+        eps = 0.02 * d
+        center = ops.default_center(xd, yd)
+        _, lse2 = ops.softmin_wide_raw(eps, xd, yd, hd, p=2, center=center, want_lse2=True)
+        out = ops.plan_apply_wide_raw(eps, xd, yd, hd, None, 0.0, lse2, v.to(DEV), center=center)
+        d2 = ((x[:, None, :].double() - y[None, :, :].double()) ** 2).sum(-1)
+        check(f"apply_wide_d{d}_k{k}", out, torch.softmax(h.double()[None, :] - d2 / (2 * eps), dim=1) @ v.double(),
+              2e-4)
 torch.cuda.synchronize()
 print("sanitize_smoke: all launches completed")
