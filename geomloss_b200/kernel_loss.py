@@ -24,8 +24,8 @@ def kernel_points(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=Non
                   **_ignored):
     """1/2 |a - b|_k^2 for unbatched a:(N,) x:(N,D) b:(M,) y:(M,D).        kernel_samples.py:92-146
 
-    ``conv(kind, x, y, w, blur, center=)`` defaults to the single-GPU kernel; distributed.py injects the
-    column-sharded one; above D = 64 the default is the wide tensor-core kernel (ops.kernel_conv_wide).  ``keops``:
+    ``conv(kind, x, y, w, blur, center=)`` defaults to the single-GPU kernel ``ops.kernel_conv_operator`` names for
+    D; distributed.py injects the column-sharded one.  ``keops``:
     the reference's use_keops=True convention (backend "online" / "multiscale"): laplacian and energy take
     sqrt(|x-y|^2) without the 1e-8 clamp of the tensorized `distances` (utils.py:56-61 vs kernel_samples.py:71-82)."""
     if kernel is not None:
@@ -34,7 +34,7 @@ def kernel_points(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=Non
         # the reference maps loss="hausdorff" to kernel_loss(name=None) and dies with KeyError(None)
         # (samples_loss.py:22-26, kernel_samples.py:107-108): keep the error type, say why.
         raise KeyError(name)
-    conv = conv or (ops.kernel_conv_wide if x.shape[-1] > ops.MAX_D_TC else ops.kernel_conv)
+    conv = conv or ops.kernel_conv_operator(x.shape[-1])
     if keops:
         name = ops.KERNEL_KINDS[name] | ops.KERNEL_UNCLAMPED
     dg = _TwiceGrad.apply
@@ -50,9 +50,8 @@ def kernel_points(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=Non
 
 def kernel_points_batched(a, x, b, y, name=None, blur=0.05, potentials=False, kernel=None, keops=False, **_ignored):
     """Batched kernel norms a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D): the three (four) matvecs take one launch group each
-    for the whole batch — for D <= 8 ranges-mode reductions over the block-diagonal stacked problem, for 8 < D <= 64
-    the batched tensor-core operators (ops.kernel_conv_batched), for 64 < D <= 1024 the wide ones
-    (ops.kernel_conv_wide).
+    for the whole batch — the batched operator ``ops.kernel_conv_operator`` names for D, and for D <= 8, where it
+    names none, ranges-mode reductions over the block-diagonal stacked problem.
     Reference: kernel_loss on (B, ...) inputs (kernel_samples.py:92-146)."""
     from . import ranges
 
@@ -67,8 +66,8 @@ def kernel_points_batched(a, x, b, y, name=None, blur=0.05, potentials=False, ke
     xf, yf, af, bf = x.reshape(B * N, D), y.reshape(B * M, D), a.reshape(B * N), b.reshape(B * M)
     center = ops.default_center(xf.detach(), yf.detach())
     dg = _TwiceGrad.apply
-    if D > ops.MAX_D:
-        cv = ops.kernel_conv_wide if D > ops.MAX_D_TC else ops.kernel_conv_batched
+    cv = ops.kernel_conv_operator(D, batched=True)
+    if cv is not None:
         a_x = cv(kid, dg(x), x.detach(), a.detach(), blur, center=center)
         b_y = cv(kid, dg(y), y.detach(), b.detach(), blur, center=center)
         b_x = cv(kid, x, y, b, blur, center=center)

@@ -40,12 +40,14 @@ NVTX = _os.environ.get("B200OT_NVTX", "0") == "1"
 
 
 class nvtx_range:
-    def __init__(self, name):
-        self.name = name
+    """The NVTX range ``fmt.format(*args)``: the name is formatted only when ranges are on, off the enqueue path."""
+
+    def __init__(self, fmt, *args):
+        self.fmt, self.args = fmt, args
 
     def __enter__(self):
         if NVTX:
-            torch.cuda.nvtx.range_push(self.name)
+            torch.cuda.nvtx.range_push(self.fmt.format(*self.args))
 
     def __exit__(self, *exc):
         if NVTX:
@@ -95,6 +97,7 @@ def _f32c(t, name):
 
 MAX_D_TC = 64  # softmin (p = 2, and p = 1 through softmin_l1) and the three kernel convolutions, forward + row
 # gradients: tensor-core path, 8 < D <= 64
+MAX_D_WIDE = 1024  # B200OT_MAX_D_WIDE: the K-slab tensor-core kernels above MAX_D_TC
 
 
 def _check_clouds(x, y, max_d=None):
@@ -162,77 +165,164 @@ def default_center(x, y):
     return (0.5 * (lo + hi)).float().contiguous()
 
 
-# ------------------------------------------------------------------------------------------------
-# softmin
-# ------------------------------------------------------------------------------------------------
+# ---- the operator families, and one body per kind of operator that serves every family ------------------------
+class _Family(NamedTuple):
+    """What one family of library operators serves for one kind of operator, and the C entries that serve it."""
+    label: str  # in NVTX ranges and errors
+    ranks: tuple  # 2: (N,D) / (M,D) clouds, 3: (B,N,D) / (B,M,D) ones (the C entries then take B)
+    dims: tuple  # (lo, hi): lo < D <= hi; lo = 0 is the one-problem family, checked by _check_clouds
+    entries: tuple  # C entries: forward, row gradient, one-pass value + row gradient
+    scratch: str  # the scratch-size query, and the _scratch tag of the buffer it sizes
+    tag: str
+    launches: Callable  # kernels per call, from p (softmins), (kind id, row gradient?) (matvecs) or (K, D) (plans)
+    p: tuple = ()  # softmins that serve one p & 0xFF only: (that p, the error class for another)
+
+
+_SOFTMIN = _Family("softmin", ranks=(2,), dims=(0, MAX_D_TC), scratch="b200ot_softmin_scratch_bytes", tag="softmin",
+                   entries=("b200ot_softmin_fwd", "b200ot_softmin_bwd_x"), launches=lambda p: 3)
+_SOFTMIN_BATCHED = _Family("softmin_batched", ranks=(3,), dims=(MAX_D, MAX_D_TC), p=(2, NotImplementedError),
+                           scratch="b200ot_batched_scratch_bytes", tag="batched", launches=lambda p: 3,
+                           entries=("b200ot_softmin_fwd_batched", "b200ot_softmin_bwd_x_batched"))
+# the coordinate maximum, two packs, reduction, finalize
+_SOFTMIN_L1 = _Family("softmin_l1", ranks=(2, 3), dims=(MAX_D, MAX_D_TC), p=(1, ValueError), launches=lambda p: 5,
+                      scratch="b200ot_softmin_l1_scratch_bytes", tag="softmin_l1",
+                      entries=("b200ot_softmin_l1_fwd", "b200ot_softmin_l1_bwd_x"))
+# two packs, reduction, finalize, and for p = 1 the coordinate maximum
+_SOFTMIN_WIDE = _Family("softmin_wide", ranks=(2, 3), dims=(MAX_D_TC, MAX_D_WIDE), scratch="b200ot_wide_scratch_bytes",
+                        tag="wide", entries=("b200ot_wide_softmin_fwd", "b200ot_wide_softmin_bwd_x"),
+                        launches=lambda p: 5 if (p & 0xFF) == 1 else 4)
+_CONV = _Family("kernel_conv", ranks=(2,), dims=(0, MAX_D_TC), scratch="b200ot_kernel_conv_scratch_bytes", tag="conv",
+                entries=("b200ot_kernel_conv_fwd", "b200ot_kernel_conv_bwd_x", "b200ot_kernel_conv_fwd_bwd_x"),
+                launches=lambda kind, bwd: 3)
+_CONV_BATCHED = _Family("kernel_conv_batched", ranks=(3,), dims=(MAX_D, MAX_D_TC), launches=lambda kind, bwd: 3,
+                        scratch="b200ot_batched_scratch_bytes", tag="batched",
+                        entries=("b200ot_kernel_conv_fwd_batched", "b200ot_kernel_conv_bwd_x_batched",
+                                 "b200ot_kernel_conv_fwd_bwd_x_batched"))
+# (the row gradient's weight maximum,) two packs, reduction, finalize, and for energy the coordinate maximum
+_CONV_WIDE = _Family("kernel_conv_wide", ranks=(2, 3), dims=(MAX_D_TC, MAX_D_WIDE), scratch="b200ot_wide_scratch_bytes",
+                     tag="wide", entries=("b200ot_wide_kernel_conv_fwd", "b200ot_wide_kernel_conv_bwd_x"),
+                     launches=lambda kind, bwd: 4 + bwd + ((kind & 0xFF) == KERNEL_KINDS["energy"]))
+# a pack (and the value maxima), then value pack, reduction, finalize per slab of 8 (D <= 8) or 64 value columns
+_PLAN = _Family("plan_apply", ranks=(2,), dims=(0, MAX_D_TC), tag="plan_apply", entries=("b200ot_plan_apply",),
+                scratch="b200ot_plan_apply_scratch_bytes", launches=lambda K, D: 1 + 3 * -(-K // (8 if D <= 8 else 64)))
+# two packs, the column maxima of v, then value pack, reduction, finalize per slab of 64 value columns
+_PLAN_WIDE = _Family("plan_apply_wide", ranks=(2,), dims=(MAX_D_TC, MAX_D_WIDE), tag="plan_apply",
+                     scratch="b200ot_wide_plan_apply_scratch_bytes", entries=("b200ot_wide_plan_apply",),
+                     launches=lambda K, D: 3 + 3 * -(-K // 64))
+
+
+def _inputs(fam, p, x, y, cols, rows, *more, v=None):
+    """Every operator's checks, in order: (1) the clouds' shapes and D, and p, against ``fam``; (2) one entry per point
+    for each vector of ``cols`` and ``rows`` ((vector, name), ...), and M rows for a value matrix ``v``; (3) device and
+    dtype of every tensor, ``more`` given like ``cols``.  Returns (B, N, M, D), the sizes the family's C entries take,
+    and x, y, the vectors, ``more`` and ``v`` as contiguous float32 CUDA tensors."""
+    lo, hi = fam.dims
+    if lo == 0:  # the one-problem family serves D from 1: _check_clouds' checks, p = 1 up to MAX_D
+        _check_clouds(x, y, hi if (p & 0xFF) == 2 else MAX_D)
+        B, (N, D), M = 1, x.shape, y.shape[0]
+    else:
+        if x.dim() not in fam.ranks or y.dim() != x.dim() or x.shape[:-2] != y.shape[:-2] or x.shape[-1] != y.shape[-1]:
+            shapes = " or ".join({2: "x:(N,D), y:(M,D)", 3: "x:(B,N,D), y:(B,M,D)"}[r] for r in fam.ranks)
+            raise ValueError(f"expected {shapes}; got {tuple(x.shape)}, {tuple(y.shape)}")
+        B, (N, D), M = (x.shape[0] if x.dim() == 3 else 1), x.shape[-2:], y.shape[-2]
+        if B == 0 or N == 0 or M == 0:
+            raise ValueError("empty batch or point cloud")
+        if fam.p and ((p & 0xFF) != fam.p[0] or (p & ~(0xFF | P_UNCLAMPED)) != 0):
+            raise fam.p[1](f"ops.{fam.label} computes the p = {fam.p[0]} softmin (p = {fam.p[0]} or {fam.p[0]} | "
+                           f"P_UNCLAMPED), got p = {p}")
+        if not lo < D <= hi:
+            raise NotImplementedError(f"the {fam.label} operators serve {lo} < D <= {hi}, got D = {D}")
+        if x.device != y.device:
+            raise ValueError("x and y must be on the same device")
+    for vectors, n in ((cols, B * M), (rows, B * N)):
+        for t, name in vectors:
+            if t is not None and t.numel() != n:
+                raise ValueError(f"{name} must have one entry per point of its cloud ({n}), got {tuple(t.shape)}")
+    if v is not None and (v.dim() not in (1, 2) or v.shape[0] != M or v.numel() == 0):
+        raise ValueError(f"v must be (M,) or (M, K) with M = {M} and K >= 1, got {tuple(v.shape)}")
+    ready = [_f32c(x, "x"), _f32c(y, "y")] + [_f32c(t, name) for t, name in cols + rows + more]
+    ready += [] if v is None else [_f32c(v, "v")]
+    return (B, N, M, D), ((B, N, M, D) if 3 in fam.ranks else (N, M, D)), ready
+
+
+def _softmin(fam, eps, x, y, h_a, h_b, h_scale_b, p, center, out_old, alpha_old, beta, out, want_lse2):
+    (B, N, M, D), sizes, (x, y, h_a, h_b, out_old, out_f32, center) = _inputs(
+        fam, p, x, y, ((h_a, "h_a"), (h_b, "h_b")), ((out_old, "out_old"), (out, "out")), (center, "center"))
+    dev = x.device
+    if out is not None and (out_f32 is not out or out.device != dev):  # written in place: refused if it needs a copy
+        raise ValueError(f"out must be contiguous and on {dev}, got strides {out.stride()} on {out.device}")
+    with nvtx_range("b200ot.{} B={} N={} M={} D={} eps={:.3g}", fam.label, B, N, M, D, float(eps)):
+        shape = (B, N) if x.dim() == 3 else N
+        out = torch.empty(shape, dtype=torch.float32, device=dev) if out is None else out
+        lse2 = torch.empty(shape, dtype=torch.float32, device=dev) if want_lse2 else None
+        scratch = _scratch(_query(dev, fam.scratch, *sizes), dev, fam.tag)
+        _call(dev, fam.entries[0], x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
+              float(beta), out, lse2, *sizes, int(p), float(eps), scratch, scratch.numel(), launches=fam.launches(p))
+    return out, lse2
+
+
+def _softmin_grad_rows(fam, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, p, center):
+    (B, N, M, D), sizes, (x, y, h_a, h_b, lse2, grad_out, center) = _inputs(
+        fam, p, x, y, ((h_a, "h_a"), (h_b, "h_b")), ((lse2, "lse2"), (grad_out, "grad_out")), (center, "center"))
+    dev = x.device
+    with nvtx_range("b200ot.{} grad_rows B={} N={} M={} D={} eps={:.3g}", fam.label, B, N, M, D, float(eps)):
+        gx = torch.empty_like(x)
+        scratch = _scratch(_query(dev, fam.scratch, *sizes), dev, fam.tag)
+        _call(dev, fam.entries[1], x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, *sizes, int(p),
+              float(eps), scratch, scratch.numel(), launches=fam.launches(p))
+    return gx
+
+
+def _kernel_conv(fam, mode, kind, x, y, w, blur, center, grad_out=None):
+    """``mode`` 0: the matvec; 1: its row gradient against ``grad_out``; 2: both from one pass (gaussian kernel)."""
+    kid = kind_id(kind)
+    if mode == 2 and (kid & 0xFF) != 0:
+        raise ValueError("the one-pass value + row gradient exists for the gaussian kernel only")
+    (B, N, M, D), sizes, (x, y, w, grad_out, center) = _inputs(
+        fam, 2, x, y, ((w, "w"),), ((grad_out, "grad_out"),), (center, "center"))
+    dev = x.device
+    with nvtx_range("b200ot.{} mode={} kind={} B={} N={} M={} D={}", fam.label, mode, kind, B, N, M, D):
+        out = None if mode == 1 else torch.empty((B, N) if x.dim() == 3 else N, dtype=torch.float32, device=dev)
+        gx = None if mode == 0 else torch.empty_like(x)
+        scratch = _scratch(_query(dev, fam.scratch, *sizes), dev, fam.tag)
+        results = ((out,), (grad_out, gx), (out, gx))[mode]  # what each entry takes after the inputs
+        _call(dev, fam.entries[mode], x, y, w, center, *results, *sizes, kid, float(blur), scratch, scratch.numel(),
+              launches=fam.launches(kid, mode == 1))
+    return (out, gx, (out, gx))[mode]
+
+
+def _plan_apply(fam, eps, x, y, h_a, h_b, h_scale_b, lse2, v, row_factor, center):
+    """``out[i, k] = row_factor_i * sum_j w_ij v[j, k]`` with ``w_ij = softmax_j(h_j - |x_i - y_j|^2 / (2 eps))`` and
+    ``h = h_a + h_scale_b * h_b``: the softmin's weights applied to a value matrix without ever forming them.  ``lse2``
+    is the forward softmin's for the same arguments; ``v`` is (M,) or (M, K), any sign, any strides; p = 2.  One pass
+    over the pairs per slab of value columns.  No autograd.  Returns (N,) or (N, K)."""
+    (_, N, M, D), _, (x, y, h_a, h_b, lse2, row_factor, center, v) = _inputs(fam, 2, x, y,
+        ((h_a, "h_a"), (h_b, "h_b")), ((lse2, "lse2"), (row_factor, "row_factor")), (center, "center"), v=v)
+    dev = x.device
+    K = 1 if v.dim() == 1 else v.shape[1]
+    with nvtx_range("b200ot.{} N={} M={} D={} K={}", fam.label, N, M, D, K):
+        out = torch.empty((N, *v.shape[1:]), dtype=torch.float32, device=dev)
+        scratch = _scratch(_query(dev, fam.scratch, N, M, D, K), dev, fam.tag)
+        _call(dev, fam.entries[0], x, y, h_a, h_b, float(h_scale_b), center, lse2, v, row_factor, out, N, M, D,
+              K, 2, float(eps), scratch, scratch.numel(), launches=fam.launches(K, D))
+    return out
 
 
 def softmin_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, out_old=None, alpha_old=0.0,
                 beta=1.0, out=None, want_lse2=False):
-    """One fused launch group: ``out <- alpha_old*out_old + beta*softmin(eps, (x, y), h_a + h_scale_b*h_b)``.
-
-    No autograd.  Returns ``(out, lse2 | None)``.
-    """
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
-    _check_clouds(x, y, MAX_D_TC if (p & 0xFF) == 2 else MAX_D)
-    N, D = x.shape
-    M = y.shape[0]
-    if h_a.numel() != M or (h_b is not None and h_b.numel() != M):
-        raise ValueError("h must have one entry per column")
-    dev = x.device
-    with nvtx_range(f"b200ot.softmin N={N} M={M} D={D} eps={float(eps):.3g}"):
-        if out is None:
-            out = torch.empty(N, dtype=torch.float32, device=dev)
-        lse2 = torch.empty(N, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = _scratch(_query(dev, "b200ot_softmin_scratch_bytes", N, M, D), dev, "softmin")
-        _call(dev, "b200ot_softmin_fwd", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
-              float(beta), out, lse2, N, M, D, int(p), float(eps), scratch, scratch.numel(), launches=3)
-    return out, lse2
+    """One fused launch group: ``out <- alpha_old*out_old + beta*softmin(eps, (x, y), h_a + h_scale_b*h_b)``.  No
+    autograd.  Returns ``(out, lse2 | None)``."""
+    return _softmin(_SOFTMIN, eps, x, y, h_a, h_b, h_scale_b, p, center, out_old, alpha_old, beta, out, want_lse2)
 
 
 def softmin_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None):
     """grad_x of <grad_out, softmin(eps, (x, y), h)> with y, h constant (b200ot_softmin_bwd_x)."""
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
-    _check_clouds(x, y, MAX_D_TC if (p & 0xFF) == 2 else MAX_D)
-    N, D = x.shape
-    M = y.shape[0]
-    dev = x.device
-    gx = torch.empty_like(x)
-    scratch = _scratch(_query(dev, "b200ot_softmin_scratch_bytes", N, M, D), dev, "softmin")
-    _call(dev, "b200ot_softmin_bwd_x", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, N, M, D, int(p),
-          float(eps), scratch, scratch.numel(), launches=3)
-    return gx
+    return _softmin_grad_rows(_SOFTMIN, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, p, center)
 
 
 def plan_apply_raw(eps, x, y, h_a, h_b, h_scale_b, lse2, v, *, row_factor=None, center=None):
-    """``out[i, k] = row_factor_i * sum_j w_ij v[j, k]`` with ``w_ij = softmax_j(h_j - |x_i - y_j|^2 / (2 eps))`` and
-    ``h = h_a + h_scale_b * h_b`` (b200ot_plan_apply): the softmin's weights applied to a value matrix without ever
-    forming them.  ``lse2`` is ``softmin_raw(..., want_lse2=True)[1]`` for the same arguments; ``v`` is (M,) or (M, K),
-    any sign, any strides.  p = 2, D <= 64.  One pass over the pairs per slab of value columns (8 for D <= 8, 64
-    above).  No autograd.  Returns (N,) or (N, K)."""
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, lse2, v = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(v, "v")
-    row_factor = _f32c(row_factor, "row_factor")
-    _check_clouds(x, y, MAX_D_TC)
-    N, D = x.shape
-    M = y.shape[0]
-    if v.dim() not in (1, 2) or v.shape[0] != M or v.numel() == 0:
-        raise ValueError(f"v must be (M,) or (M, K) with M = {M} and K >= 1, got {tuple(v.shape)}")
-    if h_a.numel() != M or (h_b is not None and h_b.numel() != M):
-        raise ValueError("h must have one entry per column")
-    if lse2.numel() != N or (row_factor is not None and row_factor.numel() != N):
-        raise ValueError("lse2 and row_factor must have one entry per row")
-    K = 1 if v.dim() == 1 else v.shape[1]
-    dev = x.device
-    with nvtx_range(f"b200ot.plan_apply N={N} M={M} D={D} K={K}"):
-        out = torch.empty((N,) if v.dim() == 1 else (N, K), dtype=torch.float32, device=dev)
-        scratch = _scratch(_query(dev, "b200ot_plan_apply_scratch_bytes", N, M, D, K), dev, "plan_apply")
-        slabs = -(-K // (8 if D <= MAX_D else 64))
-        _call(dev, "b200ot_plan_apply", x, y, h_a, h_b, float(h_scale_b), center, lse2, v, row_factor, out, N, M, D, K,
-              2, float(eps), scratch, scratch.numel(), launches=1 + 3 * slabs)
-    return out
+    """``_plan_apply`` for D <= 64 (b200ot_plan_apply), ``lse2`` from ``softmin_raw(..., want_lse2=True)``."""
+    return _plan_apply(_PLAN, eps, x, y, h_a, h_b, h_scale_b, lse2, v, row_factor, center)
 
 
 class _Softmin(torch.autograd.Function):
@@ -274,11 +364,7 @@ def softmin(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_
     return _softmin_apply(softmin_raw, softmin_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)
 
 
-# ------------------------------------------------------------------------------------------------
-# kernel convolutions
-# ------------------------------------------------------------------------------------------------
-
-
+# ---- kernel convolutions ----------------------------------------------------------------------------------------
 def kind_id(kind):
     """Kernel name (tensorized convention) or an integer kind, possibly or-ed with KERNEL_UNCLAMPED."""
     return KERNEL_KINDS[kind] if isinstance(kind, str) else int(kind)
@@ -286,54 +372,18 @@ def kind_id(kind):
 
 def kernel_conv_raw(kind, x, y, w, blur, *, center=None):
     """out_i = sum_j k(x_i, y_j) w_j, no autograd."""
-    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
-    _check_clouds(x, y, MAX_D_TC)
-    N, D = x.shape
-    M = y.shape[0]
-    if w.numel() != M:
-        raise ValueError("w must have one entry per column")
-    dev = x.device
-    with nvtx_range(f"b200ot.kernel_conv kind={kind} N={N} M={M} D={D}"):
-        out = torch.empty(N, dtype=torch.float32, device=dev)
-        scratch = _scratch(_query(dev, "b200ot_kernel_conv_scratch_bytes", N, M, D), dev, "conv")
-        _call(dev, "b200ot_kernel_conv_fwd", x, y, w, center, out, N, M, D, kind_id(kind), float(blur), scratch,
-              scratch.numel(), launches=3)
-    return out
+    return _kernel_conv(_CONV, 0, kind, x, y, w, blur, center)
 
 
 def kernel_conv_grad_rows(kind, x, y, w, blur, grad_out, *, center=None):
-    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
-    grad_out = _f32c(grad_out, "grad_out")
-    _check_clouds(x, y, MAX_D_TC)
-    N, D = x.shape
-    M = y.shape[0]
-    dev = x.device
-    gx = torch.empty_like(x)
-    scratch = _scratch(_query(dev, "b200ot_kernel_conv_scratch_bytes", N, M, D), dev, "conv")
-    _call(dev, "b200ot_kernel_conv_bwd_x", x, y, w, center, grad_out, gx, N, M, D, kind_id(kind), float(blur), scratch,
-          scratch.numel(), launches=3)
-    return gx
+    """grad_x of <grad_out, kernel_conv_raw(kind, x, y, w, blur)> (b200ot_kernel_conv_bwd_x)."""
+    return _kernel_conv(_CONV, 1, kind, x, y, w, blur, center, grad_out)
 
 
 def kernel_conv_value_and_grad_rows(kind, x, y, w, blur, *, center=None):
     """(out, grad_unit) with out_i = sum_j k(x_i, y_j) w_j and grad_unit[i] = sum_j w_j dk(x_i, y_j)/dx_i from ONE
     pass over the pairs (gaussian kernel; b200ot_kernel_conv_fwd_bwd_x).  No autograd."""
-    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
-    if (kind_id(kind) & 0xFF) != 0:
-        raise ValueError("the one-pass value + row gradient exists for the gaussian kernel only")
-    _check_clouds(x, y, MAX_D_TC)
-    N, D = x.shape
-    M = y.shape[0]
-    if w.numel() != M:
-        raise ValueError("w must have one entry per column")
-    dev = x.device
-    with nvtx_range(f"b200ot.kernel_conv value+grad kind={kind} N={N} M={M} D={D}"):
-        out = torch.empty(N, dtype=torch.float32, device=dev)
-        gunit = torch.empty_like(x)
-        scratch = _scratch(_query(dev, "b200ot_kernel_conv_scratch_bytes", N, M, D), dev, "conv")
-        _call(dev, "b200ot_kernel_conv_fwd_bwd_x", x, y, w, center, out, gunit, N, M, D, kind_id(kind), float(blur),
-              scratch, scratch.numel(), launches=3)
-    return out, gunit
+    return _kernel_conv(_CONV, 2, kind, x, y, w, blur, center)
 
 
 # A gaussian matvec whose ROW cloud requires a gradient is evaluated by the row-gradient reduction, which accumulates
@@ -404,68 +454,20 @@ def kernel_conv(kind, x, y, w, blur, *, center=None):
 
 
 # ------------------------------------------------------------------------------------------------
-# batches of B problems in the tensor-core dimensions (8 < D <= 64): x (B,N,D), y (B,M,D), per-column vectors (B,M),
-# per-row vectors (B,N); element b of the rows is reduced over element b of the columns only, the whole batch in one
-# launch group per call (b200ot_*_batched).  Same contracts as the one-problem operators above.
+# the other families, with the contracts of the one-problem operators above: batches (B,N,D) / (B,M,D) with per-column
+# vectors (B,M) and per-row vectors (B,N), element b of the rows reduced over element b of the columns only; the p = 1
+# softmin; above D = 64, the K-slab tensor-core kernels (csrc/tcwide.cuh).  One launch group per call.
 # ------------------------------------------------------------------------------------------------
-def _check_batch(x, y):
-    if x.dim() != 3 or y.dim() != 3 or x.shape[0] != y.shape[0] or x.shape[2] != y.shape[2]:
-        raise ValueError(f"expected x:(B,N,D), y:(B,M,D); got {tuple(x.shape)}, {tuple(y.shape)}")
-    B, N, D = x.shape
-    M = y.shape[1]
-    if B == 0 or N == 0 or M == 0:
-        raise ValueError("empty batch or point cloud")
-    if not MAX_D < D <= MAX_D_TC:
-        raise NotImplementedError(f"the batched tensor-core operators serve {MAX_D} < D <= {MAX_D_TC}, got D = {D} "
-                                  f"(batches with D <= {MAX_D} run as block-diagonal ranges problems, ranges.py)")
-    if x.device != y.device:
-        raise ValueError("x and y must be on the same device")
-    return B, N, M, D
-
-
-def _per_point(t, n, name):
-    if t is not None and t.numel() != n:
-        raise ValueError(f"{name} must have one entry per point of its cloud ({n}), got {tuple(t.shape)}")
-
-
-def _batched_scratch(B, N, M, D, dev):
-    return _scratch(_query(dev, "b200ot_batched_scratch_bytes", B, N, M, D), dev, "batched")
-
-
 def softmin_batched_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, out_old=None, alpha_old=0.0,
                         beta=1.0, out=None, want_lse2=False):
-    """``softmin_raw`` on a batch: out (B,N) <- alpha_old*out_old + beta*softmin(eps, (x[b], y[b]), h[b]).  p = 2 only.
-    No autograd.  Returns ``(out, lse2 | None)``."""
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
-    B, N, M, D = _check_batch(x, y)
-    if (p & 0xFF) != 2:
-        raise NotImplementedError(f"p = {p & 0xFF}: the batched softmin exists for p = 2 only (tensor cores)")
-    _per_point(h_a, B * M, "h_a")
-    _per_point(h_b, B * M, "h_b")
-    _per_point(out_old, B * N, "out_old")
-    dev = x.device
-    with nvtx_range(f"b200ot.softmin_batched B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
-        if out is None:
-            out = torch.empty(B, N, dtype=torch.float32, device=dev)
-        lse2 = torch.empty(B, N, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = _batched_scratch(B, N, M, D, dev)
-        _call(dev, "b200ot_softmin_fwd_batched", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
-              float(beta), out, lse2, B, N, M, D, int(p), float(eps), scratch, scratch.numel(), launches=3)
-    return out, lse2
+    """``softmin_raw`` on a batch: out[b] (B,N) is the softmin of (x[b], y[b], h[b]).  p = 2 only."""
+    return _softmin(_SOFTMIN_BATCHED, eps, x, y, h_a, h_b, h_scale_b, p, center, out_old, alpha_old, beta, out,
+                    want_lse2)
 
 
 def softmin_batched_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None):
     """grad_x (B,N,D) of <grad_out, softmin_batched(eps, x, y, h)> with y, h constant (b200ot_softmin_bwd_x_batched)."""
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
-    B, N, M, D = _check_batch(x, y)
-    dev = x.device
-    gx = torch.empty_like(x)
-    scratch = _batched_scratch(B, N, M, D, dev)
-    _call(dev, "b200ot_softmin_bwd_x_batched", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, B, N, M,
-          D, int(p), float(eps), scratch, scratch.numel(), launches=3)
-    return gx
+    return _softmin_grad_rows(_SOFTMIN_BATCHED, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, p, center)
 
 
 def softmin_batched(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
@@ -474,50 +476,19 @@ def softmin_batched(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None
                           scale_out)
 
 
-def _conv_batched_args(x, y, w, center):
-    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
-    B, N, M, D = _check_batch(x, y)
-    _per_point(w, B * M, "w")
-    return x, y, w, center, B, N, M, D
-
-
 def kernel_conv_batched_raw(kind, x, y, w, blur, *, center=None):
     """out (B,N), out[b, i] = sum_j k(x[b, i], y[b, j]) w[b, j], no autograd."""
-    x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
-    dev = x.device
-    with nvtx_range(f"b200ot.kernel_conv_batched kind={kind} B={B} N={N} M={M} D={D}"):
-        out = torch.empty(B, N, dtype=torch.float32, device=dev)
-        scratch = _batched_scratch(B, N, M, D, dev)
-        _call(dev, "b200ot_kernel_conv_fwd_batched", x, y, w, center, out, B, N, M, D, kind_id(kind), float(blur),
-              scratch, scratch.numel(), launches=3)
-    return out
+    return _kernel_conv(_CONV_BATCHED, 0, kind, x, y, w, blur, center)
 
 
 def kernel_conv_batched_grad_rows(kind, x, y, w, blur, grad_out, *, center=None):
-    x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
-    grad_out = _f32c(grad_out, "grad_out")
-    _per_point(grad_out, B * N, "grad_out")
-    dev = x.device
-    gx = torch.empty_like(x)
-    scratch = _batched_scratch(B, N, M, D, dev)
-    _call(dev, "b200ot_kernel_conv_bwd_x_batched", x, y, w, center, grad_out, gx, B, N, M, D, kind_id(kind),
-          float(blur), scratch, scratch.numel(), launches=3)
-    return gx
+    """grad_x (B,N,D) of <grad_out, kernel_conv_batched_raw(kind, x, y, w, blur)> (b200ot_kernel_conv_bwd_x_batched)."""
+    return _kernel_conv(_CONV_BATCHED, 1, kind, x, y, w, blur, center, grad_out)
 
 
 def kernel_conv_batched_value_and_grad_rows(kind, x, y, w, blur, *, center=None):
     """``kernel_conv_value_and_grad_rows`` on a batch (gaussian only): (out (B,N), grad_unit (B,N,D))."""
-    if (kind_id(kind) & 0xFF) != 0:
-        raise ValueError("the one-pass value + row gradient exists for the gaussian kernel only")
-    x, y, w, center, B, N, M, D = _conv_batched_args(x, y, w, center)
-    dev = x.device
-    with nvtx_range(f"b200ot.kernel_conv_batched value+grad B={B} N={N} M={M} D={D}"):
-        out = torch.empty(B, N, dtype=torch.float32, device=dev)
-        gunit = torch.empty_like(x)
-        scratch = _batched_scratch(B, N, M, D, dev)
-        _call(dev, "b200ot_kernel_conv_fwd_bwd_x_batched", x, y, w, center, out, gunit, B, N, M, D, kind_id(kind),
-              float(blur), scratch, scratch.numel(), launches=3)
-    return out, gunit
+    return _kernel_conv(_CONV_BATCHED, 2, kind, x, y, w, blur, center)
 
 
 def kernel_conv_batched(kind, x, y, w, blur, *, center=None):
@@ -526,55 +497,15 @@ def kernel_conv_batched(kind, x, y, w, blur, *, center=None):
     return _KernelConv.apply(batched, batched, x, y, w, kind, blur, center, _fused(kind, x))
 
 
-# ------------------------------------------------------------------------------------------------
-# the p = 1 softmin in the tensor-core dimensions (8 < D <= 64): f_i = -eps log sum_j exp(h_j - |x_i - y_j| / eps), one
-# problem (N,D) / (M,D) or a batch (B,N,D) / (B,M,D) in one launch group per call (b200ot_softmin_l1_*).
-# ------------------------------------------------------------------------------------------------
-def _l1_args(x, y, p):
-    if (p & 0xFF) != 1 or (p & ~(0xFF | P_UNCLAMPED)) != 0:
-        raise ValueError(f"softmin_l1 computes the p = 1 softmin (p = 1 or 1 | P_UNCLAMPED), got p = {p}")
-    if x.dim() == 2 and y.dim() == 2:
-        return False, _check_batch(x.unsqueeze(0), y.unsqueeze(0))
-    return True, _check_batch(x, y)
-
-
 def softmin_l1_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, out_old=None, alpha_old=0.0,
                    beta=1.0, out=None, want_lse2=False):
-    """``softmin_batched_raw`` for the cost |x - y|: out <- alpha_old*out_old + beta*softmin(eps, (x, y), h), (N,) for
-    (N,D) clouds, (B,N) for (B,N,D) ones.  No autograd.  Returns ``(out, lse2 | None)``."""
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
-    batched, (B, N, M, D) = _l1_args(x, y, p)
-    _per_point(h_a, B * M, "h_a")
-    _per_point(h_b, B * M, "h_b")
-    _per_point(out_old, B * N, "out_old")
-    shape = (B, N) if batched else (N,)
-    dev = x.device
-    with nvtx_range(f"b200ot.softmin_l1 B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
-        if out is None:
-            out = torch.empty(shape, dtype=torch.float32, device=dev)
-        lse2 = torch.empty(shape, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = _scratch(_query(dev, "b200ot_softmin_l1_scratch_bytes", B, N, M, D), dev, "softmin_l1")
-        # coordinate maximum, two packs, reduction, finalize
-        _call(dev, "b200ot_softmin_l1_fwd", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
-              float(beta), out, lse2, B, N, M, D, int(p), float(eps), scratch, scratch.numel(), launches=5)
-    return out, lse2
+    """``softmin_raw`` for the cost |x - y|, (N,) for (N,D) clouds, (B,N) for (B,N,D) ones."""
+    return _softmin(_SOFTMIN_L1, eps, x, y, h_a, h_b, h_scale_b, p, center, out_old, alpha_old, beta, out, want_lse2)
 
 
 def softmin_l1_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=1, center=None):
     """grad_x, shaped like x, of <grad_out, softmin_l1(eps, x, y, h)> with y, h constant (b200ot_softmin_l1_bwd_x)."""
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
-    _, (B, N, M, D) = _l1_args(x, y, p)
-    _per_point(grad_out, B * N, "grad_out")
-    _per_point(lse2, B * N, "lse2")
-    dev = x.device
-    gx = torch.empty_like(x)
-    scratch = _scratch(_query(dev, "b200ot_softmin_l1_scratch_bytes", B, N, M, D), dev, "softmin_l1")
-    # coordinate maximum, two packs, reduction, finalize
-    _call(dev, "b200ot_softmin_l1_bwd_x", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, B, N, M, D,
-          int(p), float(eps), scratch, scratch.numel(), launches=5)
-    return gx
+    return _softmin_grad_rows(_SOFTMIN_L1, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, p, center)
 
 
 def softmin_l1(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, scale_out=1.0):
@@ -582,102 +513,20 @@ def softmin_l1(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=1, center=None, sca
     return _softmin_apply(softmin_l1_raw, softmin_l1_grad_rows, eps, x, y, h_a, h_b, h_scale_b, p, center, scale_out)
 
 
-# ------------------------------------------------------------------------------------------------
-# above D = 64 (64 < D <= MAX_D_WIDE): the p = 2 and p = 1 softmins and the three kernel convolutions on the K-slab
-# tensor-core kernels (csrc/tcwide.cuh, b200ot_wide_*), one problem (N,D) / (M,D) or a batch (B,N,D) / (B,M,D) in one
-# launch group per call.  Same contracts as the one-problem and batched operators above.
-# ------------------------------------------------------------------------------------------------
-MAX_D_WIDE = 1024  # B200OT_MAX_D_WIDE
-
-
-def _wide_args(x, y):
-    """(batched, (B, N, M, D)) of (N,D) / (M,D) or (B,N,D) / (B,M,D) clouds in the wide dimensions."""
-    batched = not (x.dim() == 2 and y.dim() == 2)
-    xb, yb = (x, y) if batched else (x.unsqueeze(0), y.unsqueeze(0))
-    if xb.dim() != 3 or yb.dim() != 3 or xb.shape[0] != yb.shape[0] or xb.shape[2] != yb.shape[2]:
-        raise ValueError(f"expected x:(N,D), y:(M,D) or x:(B,N,D), y:(B,M,D); got {tuple(x.shape)}, {tuple(y.shape)}")
-    B, N, D = xb.shape
-    M = yb.shape[1]
-    if B == 0 or N == 0 or M == 0:
-        raise ValueError("empty batch or point cloud")
-    if not MAX_D_TC < D <= MAX_D_WIDE:
-        raise NotImplementedError(f"the wide tensor-core operators serve {MAX_D_TC} < D <= {MAX_D_WIDE}, got D = {D} "
-                                  f"(no kernel of this build reduces clouds above D = {MAX_D_WIDE})")
-    if x.device != y.device:
-        raise ValueError("x and y must be on the same device")
-    return batched, (B, N, M, D)
-
-
-def _wide_scratch(B, N, M, D, dev):
-    return _scratch(_query(dev, "b200ot_wide_scratch_bytes", B, N, M, D), dev, "wide")
-
-
 def softmin_wide_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, out_old=None, alpha_old=0.0,
                      beta=1.0, out=None, want_lse2=False):
-    """``softmin_raw`` above D = 64 for p = 1 or 2 (| P_UNCLAMPED): out <- alpha_old*out_old + beta*softmin(eps, (x, y),
-    h), (N,) for (N,D) clouds, (B,N) for (B,N,D) ones.  No autograd.  Returns ``(out, lse2 | None)``."""
-    batched, (B, N, M, D) = _wide_args(x, y)
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, out_old = _f32c(center, "center"), _f32c(out_old, "out_old")
-    _per_point(h_a, B * M, "h_a")
-    _per_point(h_b, B * M, "h_b")
-    _per_point(out_old, B * N, "out_old")
-    shape = (B, N) if batched else (N,)
-    dev = x.device
-    with nvtx_range(f"b200ot.softmin_wide B={B} N={N} M={M} D={D} eps={float(eps):.3g}"):
-        if out is None:
-            out = torch.empty(shape, dtype=torch.float32, device=dev)
-        lse2 = torch.empty(shape, dtype=torch.float32, device=dev) if want_lse2 else None
-        scratch = _wide_scratch(B, N, M, D, dev)
-        # two packs, reduction, finalize (p = 1: and the coordinate maximum)
-        _call(dev, "b200ot_wide_softmin_fwd", x, y, h_a, h_b, float(h_scale_b), center, out_old, float(alpha_old),
-              float(beta), out, lse2, B, N, M, D, int(p), float(eps), scratch, scratch.numel(),
-              launches=5 if (p & 0xFF) == 1 else 4)
-    return out, lse2
+    """``softmin_raw`` above D = 64 for p = 1 or 2, (N,) for (N,D) clouds, (B,N) for (B,N,D) ones."""
+    return _softmin(_SOFTMIN_WIDE, eps, x, y, h_a, h_b, h_scale_b, p, center, out_old, alpha_old, beta, out, want_lse2)
 
 
 def softmin_wide_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None):
-    """grad_x, shaped like x, of <grad_out, softmin_wide(eps, x, y, h)> with y, h constant
-    (b200ot_wide_softmin_bwd_x)."""
-    _, (B, N, M, D) = _wide_args(x, y)
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, lse2, grad_out = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(grad_out, "grad_out")
-    _per_point(grad_out, B * N, "grad_out")
-    _per_point(lse2, B * N, "lse2")
-    dev = x.device
-    gx = torch.empty_like(x)
-    scratch = _wide_scratch(B, N, M, D, dev)
-    _call(dev, "b200ot_wide_softmin_bwd_x", x, y, h_a, h_b, float(h_scale_b), center, lse2, grad_out, gx, B, N, M, D,
-          int(p), float(eps), scratch, scratch.numel(), launches=5 if (p & 0xFF) == 1 else 4)
-    return gx
+    """grad_x, shaped like x, of <grad_out, softmin_wide(eps, x, y, h)> with y, h constant."""
+    return _softmin_grad_rows(_SOFTMIN_WIDE, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, p, center)
 
 
 def plan_apply_wide_raw(eps, x, y, h_a, h_b, h_scale_b, lse2, v, *, row_factor=None, center=None):
-    """``plan_apply_raw`` above D = 64 (b200ot_wide_plan_apply): ``out[i, k] = row_factor_i * sum_j w_ij v[j, k]`` for
-    (N,D) / (M,D) clouds, ``lse2`` from ``softmin_wide_raw(..., want_lse2=True)`` with the same arguments.  ``v`` is
-    (M,) or (M, K), any sign, any strides; p = 2.  One pass over the pairs per slab of 64 value columns, each
-    recomputing the full-K exponent.  No autograd.  Returns (N,) or (N, K)."""
-    if x.dim() != 2 or y.dim() != 2:
-        raise ValueError(f"expected x:(N,D), y:(M,D); got {tuple(x.shape)}, {tuple(y.shape)}")
-    _, (_, N, M, D) = _wide_args(x, y)
-    x, y, h_a, h_b = _f32c(x, "x"), _f32c(y, "y"), _f32c(h_a, "h_a"), _f32c(h_b, "h_b")
-    center, lse2, v = _f32c(center, "center"), _f32c(lse2, "lse2"), _f32c(v, "v")
-    row_factor = _f32c(row_factor, "row_factor")
-    if v.dim() not in (1, 2) or v.shape[0] != M or v.numel() == 0:
-        raise ValueError(f"v must be (M,) or (M, K) with M = {M} and K >= 1, got {tuple(v.shape)}")
-    _per_point(h_a, M, "h_a")
-    _per_point(h_b, M, "h_b")
-    if lse2.numel() != N or (row_factor is not None and row_factor.numel() != N):
-        raise ValueError("lse2 and row_factor must have one entry per row")
-    K = 1 if v.dim() == 1 else v.shape[1]
-    dev = x.device
-    with nvtx_range(f"b200ot.plan_apply_wide N={N} M={M} D={D} K={K}"):
-        out = torch.empty((N,) if v.dim() == 1 else (N, K), dtype=torch.float32, device=dev)
-        scratch = _scratch(_query(dev, "b200ot_wide_plan_apply_scratch_bytes", N, M, D, K), dev, "plan_apply")
-        # two packs, the column maxima of v, then value pack, reduction and finalize per slab of 64 columns
-        _call(dev, "b200ot_wide_plan_apply", x, y, h_a, h_b, float(h_scale_b), center, lse2, v, row_factor, out, N, M,
-              D, K, 2, float(eps), scratch, scratch.numel(), launches=3 + 3 * -(-K // 64))
-    return out
+    """``_plan_apply`` above D = 64 (b200ot_wide_plan_apply), lse2 from ``softmin_wide_raw(..., want_lse2=True)``."""
+    return _plan_apply(_PLAN_WIDE, eps, x, y, h_a, h_b, h_scale_b, lse2, v, row_factor, center)
 
 
 def softmin_wide(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, scale_out=1.0):
@@ -686,45 +535,46 @@ def softmin_wide(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, s
                           scale_out)
 
 
-def _conv_wide_args(x, y, w, center):
-    batched, (B, N, M, D) = _wide_args(x, y)  # the shape check first: D > MAX_D_WIDE is refused on any device
-    x, y, w, center = _f32c(x, "x"), _f32c(y, "y"), _f32c(w, "w"), _f32c(center, "center")
-    _per_point(w, B * M, "w")
-    return x, y, w, center, batched, B, N, M, D
-
-
 def kernel_conv_wide_raw(kind, x, y, w, blur, *, center=None):
     """out_i = sum_j k(x_i, y_j) w_j above D = 64, (N,) or (B,N); no autograd."""
-    x, y, w, center, batched, B, N, M, D = _conv_wide_args(x, y, w, center)
-    dev = x.device
-    energy = (kind_id(kind) & 0xFF) == KERNEL_KINDS["energy"]
-    with nvtx_range(f"b200ot.kernel_conv_wide kind={kind} B={B} N={N} M={M} D={D}"):
-        out = torch.empty((B, N) if batched else (N,), dtype=torch.float32, device=dev)
-        scratch = _wide_scratch(B, N, M, D, dev)
-        # two packs, reduction, finalize (energy: and the coordinate maximum)
-        _call(dev, "b200ot_wide_kernel_conv_fwd", x, y, w, center, out, B, N, M, D, kind_id(kind), float(blur), scratch,
-              scratch.numel(), launches=5 if energy else 4)
-    return out
+    return _kernel_conv(_CONV_WIDE, 0, kind, x, y, w, blur, center)
 
 
 def kernel_conv_wide_grad_rows(kind, x, y, w, blur, grad_out, *, center=None):
-    """grad_x, shaped like x, of <grad_out, kernel_conv_wide_raw(kind, x, y, w, blur)>
-    (b200ot_wide_kernel_conv_bwd_x)."""
-    x, y, w, center, _, B, N, M, D = _conv_wide_args(x, y, w, center)
-    grad_out = _f32c(grad_out, "grad_out")
-    _per_point(grad_out, B * N, "grad_out")
-    dev = x.device
-    energy = (kind_id(kind) & 0xFF) == KERNEL_KINDS["energy"]
-    gx = torch.empty_like(x)
-    scratch = _wide_scratch(B, N, M, D, dev)
-    # weight maximum, two packs, reduction, finalize (energy: and the coordinate maximum)
-    _call(dev, "b200ot_wide_kernel_conv_bwd_x", x, y, w, center, grad_out, gx, B, N, M, D, kind_id(kind), float(blur),
-          scratch, scratch.numel(), launches=6 if energy else 5)
-    return gx
+    """grad_x, shaped like x, of <grad_out, kernel_conv_wide_raw(kind, x, y, w, blur)>."""
+    return _kernel_conv(_CONV_WIDE, 1, kind, x, y, w, blur, center, grad_out)
 
 
 def kernel_conv_wide(kind, x, y, w, blur, *, center=None):
-    """out = K(x, y) @ w above D = 64, (N,) or (B,N), differentiable w.r.t. x, y and w (no one-pass value + gradient:
-    the forward and the row gradient are separate launches)."""
+    """out = K(x, y) @ w above D = 64, (N,) or (B,N), differentiable w.r.t. x, y and w, in two passes."""
     wide = _ConvOps(kernel_conv_wide_raw, kernel_conv_wide_grad_rows, None)
     return _KernelConv.apply(wide, wide, x, y, w, kind, blur, center, False)
+
+
+# which operators serve which clouds: the one place that compares D with MAX_D / MAX_D_TC.  The operators are module
+# globals read at every call, so a replaced operator is the one returned.
+def softmin_operators(D, p=2, batched=False):
+    """(raw, differentiable) softmins for one problem of dimension D and cost |x - y|^p / p, or a batch; None for a
+    batch with D <= MAX_D (a block-diagonal ranges problem, ranges.py).  Above MAX_D_WIDE the wide ones refuse."""
+    if D > MAX_D_TC:
+        return softmin_wide_raw, softmin_wide
+    if D <= MAX_D:
+        return None if batched else (softmin_raw, softmin)
+    if (p & 0xFF) == 1:
+        return softmin_l1_raw, softmin_l1
+    return (softmin_batched_raw, softmin_batched) if batched else (softmin_raw, softmin)
+
+
+def kernel_conv_operator(D, batched=False):
+    """The differentiable kernel matvec for one problem of dimension D or a batch; None for a batch with D <= MAX_D."""
+    if D > MAX_D_TC:
+        return kernel_conv_wide
+    return (None if D <= MAX_D else kernel_conv_batched) if batched else kernel_conv
+
+
+def ot_operators(D):
+    """(forward, row gradient, plan apply) of the p = 2 softmin on one problem of dimension D: the operators the
+    entropic OT solver (ot.solve_sample) runs."""
+    if D > MAX_D_TC:
+        return softmin_wide_raw, softmin_wide_grad_rows, plan_apply_wide_raw
+    return softmin_raw, softmin_grad_rows, plan_apply_raw

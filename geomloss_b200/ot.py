@@ -92,10 +92,9 @@ def annealing_eps(maxmin_cost, eps, n_iter):
 class _Softmin:
     """``softmin_sample`` (sample.py:91-182) for the four (rows, columns) pairs of one problem, on the kernel.
 
-    It also picks, from D, the three operators every pass of the facade runs: the forward softmin (``fwd``), its row
-    gradient (``grad_rows``) and the plan applied to a value matrix (``apply``) — ``softmin_raw`` / ``softmin_grad_rows``
-    / ``plan_apply_raw`` up to D = 64, ``softmin_wide_raw`` / ``softmin_wide_grad_rows`` / ``plan_apply_wide_raw`` up to
-    D = 1024.  They are looked up in ``ops`` at every call, not bound once."""
+    It also holds the three operators every pass of the facade runs, as ``ops.ot_operators`` names them for D when
+    the solver starts: the forward softmin (``fwd``), its row gradient (``grad_rows``) and the plan applied to a value
+    matrix (``apply``)."""
 
     def __init__(self, X_a, X_b):
         self.D = X_a.shape[1]
@@ -104,22 +103,7 @@ class _Softmin:
                                       f"build reduces clouds above D = {ops.MAX_D_WIDE})")
         self.center = ops.default_center(X_a, X_b)
         self.X_a, self.X_b = X_a, X_b
-
-    @property
-    def wide(self):
-        return self.D > ops.MAX_D_TC
-
-    @property
-    def fwd(self):
-        return ops.softmin_wide_raw if self.wide else ops.softmin_raw
-
-    @property
-    def grad_rows(self):
-        return ops.softmin_wide_grad_rows if self.wide else ops.softmin_grad_rows
-
-    @property
-    def apply(self):
-        return ops.plan_apply_wide_raw if self.wide else ops.plan_apply_raw
+        self.fwd, self.grad_rows, self.apply = ops.ot_operators(self.D)
 
     def __call__(self, eps, x, y, log_w, pot, *, damp=1.0, old=None):
         """damp * softmin(eps, log_w, C(x, y), pot), or its average with ``old`` (the symmetric Sinkhorn update)."""

@@ -161,18 +161,15 @@ def sinkhorn_points(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scali
     """Sinkhorn divergence between two weighted clouds a:(N,) x:(N,D) b:(M,) y:(M,D) on one CUDA device.
     Counterpart of sinkhorn_tensorized / sinkhorn_online (sinkhorn_samples.py:74-221, :349-424) for a single batch
     element.  ``keops``: the "online" cost convention — for p = 1, Norm2(x-y) without the 1e-8 clamp of the
-    tensorized `distances` (sinkhorn_samples.py:303-306 vs utils.py:56-61).  p = 1 above D = 8 runs on the tensor-core
-    p = 1 softmin (ops.softmin_l1), and every cost above D = 64 on the wide tensor-core softmin (ops.softmin_wide),
-    unless the caller injected its own operators."""
+    tensorized `distances` (sinkhorn_samples.py:303-306 vs utils.py:56-61).  The softmins are the ones
+    ``ops.softmin_operators`` names for D and p, unless the caller injected its own operators."""
     if p not in (1, 2):
         raise KeyError(p)  # the reference's cost table only knows p = 1, 2 (sinkhorn_samples.py:26-29)
     diameter, eps, eps_list, rho = scaling_parameters(x, y, p, blur, reach, diameter, scaling)
     center = ops.default_center(x.detach(), y.detach())
     pk = (p | ops.P_UNCLAMPED) if keops else p
-    if x.shape[-1] > ops.MAX_D_TC and softmin_raw is None and softmin_grad is None:
-        softmin_raw, softmin_grad = ops.softmin_wide_raw, ops.softmin_wide
-    elif p == 1 and x.shape[-1] > ops.MAX_D and softmin_raw is None and softmin_grad is None:
-        softmin_raw, softmin_grad = ops.softmin_l1_raw, ops.softmin_l1
+    if softmin_raw is None and softmin_grad is None:
+        softmin_raw, softmin_grad = ops.softmin_operators(x.shape[-1], p)
     f_aa, g_bb, g_ab, f_ba = sinkhorn_loop_points(log_weights(a.detach()), log_weights(b.detach()), x, y, eps_list,
                                                   rho, p=pk, debias=debias, center=center, softmin_raw=softmin_raw,
                                                   softmin_grad=softmin_grad)
@@ -202,9 +199,8 @@ def sinkhorn_cost_batched(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, B, debias=True
 def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scaling=0.5, debias=True,
                             potentials=False, keops=False, **_ignored):
     """Batched Sinkhorn divergence a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D): every softmin of the loop is ONE launch group
-    over the whole batch, not B launches — for D <= 8 a ranges-mode block-diagonal problem, for 8 < D <= 64 the
-    batched tensor-core operators (ops.softmin_batched_raw / softmin_batched, p = 2; ops.softmin_l1_raw / softmin_l1,
-    p = 1), for 64 < D <= 1024 the wide ones (ops.softmin_wide_raw / softmin_wide, p = 1 and 2).
+    over the whole batch, not B launches — the batched operators ``ops.softmin_operators`` names for D and p, and for
+    D <= 8, where it names none, a ranges-mode block-diagonal problem.
     Reference: sinkhorn_tensorized / sinkhorn_online on (B, ...) inputs, softmin_online_lazytensor
     (sinkhorn_samples.py:74-221, :229-290, :349-424); one shared eps-schedule (diameter over the flattened batch)."""
     from . import ranges
@@ -219,10 +215,9 @@ def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=Non
     dev = x.device
     pk = (p | ops.P_UNCLAMPED) if keops else p
     loop = dict(p=pk, debias=debias, center=center)
-    if D > ops.MAX_D:
-        raw, grad = (ops.softmin_l1_raw, ops.softmin_l1) if p == 1 else (ops.softmin_batched_raw, ops.softmin_batched)
-        if D > ops.MAX_D_TC:
-            raw, grad = ops.softmin_wide_raw, ops.softmin_wide
+    batched_ops = ops.softmin_operators(D, p, batched=True)
+    if batched_ops is not None:
+        raw, grad = batched_ops
 
         # the loop runs on the flattened clouds and potentials; the operators see the (B, n, D) views
         def sm(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
