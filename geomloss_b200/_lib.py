@@ -93,6 +93,11 @@ _SIGNATURES = {
     "b200ot_wide_plan_apply_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32, c_int64]),
     "b200ot_wide_plan_apply": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, _P, _P, _P, c_int64, c_int64, c_int32,
                                          c_int64, c_int32, c_float, _P, c_int64, _P]),
+    "b200ot_dense_scratch_bytes": (c_int64, [c_int64, c_int64, c_int64]),
+    "b200ot_dense_softmin_pair": (c_int32, [_P, _P, _P, _P, _P, c_float, c_float, c_float, _P, _P, _P, _P, c_int64,
+                                            c_int64, c_int64, c_float, _P, c_int64, _P]),
+    "b200ot_dense_softmin_pair_bwd": (c_int32, [_P, _P, _P, _P, _P, c_float, _P, _P, _P, _P, _P, c_int64, c_int64,
+                                                c_int64, _P]),
     "b200ot_blocks_shape": (None, [ctypes.POINTER(c_int32), ctypes.POINTER(c_int32)]),
     "b200ot_blocks_scratch_bytes": (c_int64, [c_int64, c_int64, c_int64, _P, c_int64, _P, c_int32]),
     "b200ot_softmin_fwd_blocks": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, c_float, c_float, _P, _P, c_int64, _P,

@@ -551,6 +551,64 @@ def kernel_conv_wide(kind, x, y, w, blur, *, center=None):
     return _KernelConv.apply(wide, wide, x, y, w, kind, blur, center, False)
 
 
+# ------------------------------------------------------------------------------------------------
+# explicit cost matrices C (N, M) or (B, N, M): both softmins of a symmetric Sinkhorn update from one pass over C
+# (b200ot_dense_*, csrc/b200ot_dense.cu).  No clouds, so no _Family: one body per operator.
+# ------------------------------------------------------------------------------------------------
+def _dense_inputs(C, rows, cols):
+    """The dense operators' checks, in ``_inputs``' order: (1) C is (N, M) or (B, N, M) and not empty; (2) one entry
+    per row (B N) / column (B M) for each vector of ``rows`` / ``cols`` ((vector, name), ...); (3) device and dtype of
+    every tensor.  Returns (B, N, M), the shape of a row / column vector, and C then the vectors as contiguous float32
+    CUDA tensors."""
+    if C.dim() not in (2, 3) or C.numel() == 0:
+        raise ValueError(f"expected a non-empty cost matrix C:(N,M) or (B,N,M); got {tuple(C.shape)}")
+    B, N, M = (1, *C.shape) if C.dim() == 2 else tuple(C.shape)
+    for vectors, n in ((rows, B * N), (cols, B * M)):
+        for t, name in vectors:
+            if t is not None and t.numel() != n:
+                raise ValueError(f"{name} must have one entry per {'row' if n == B * N else 'column'} of C ({n}), "
+                                 f"got {tuple(t.shape)}")
+    ready = [_f32c(C, "C")] + [_f32c(t, name) for t, name in rows + cols]
+    if any(t is not None and t.device != C.device for t in ready):
+        raise ValueError(f"every tensor must live on C's device ({C.device})")
+    lead = (B,) if C.dim() == 3 else ()
+    return (B, N, M), (lead + (N,), lead + (M,)), ready
+
+
+def dense_softmin_pair_raw(eps, C, log_a, log_b, f_old, g_old, *, alpha_old=0.0, beta=1.0, want_lse2=False):
+    """One pass over C for both softmins of a symmetric Sinkhorn update, each averaged / damped like ``softmin_raw``:
+        f <- alpha_old f_old + beta (-eps log sum_j exp(log_b_j + (g_old_j - C_ij) / eps)),
+        g <- alpha_old g_old + beta (-eps log sum_i exp(log_a_i + (f_old_i - C_ij) / eps)).
+    C (N, M) or (B, N, M); the vectors (N,) / (M,) or (B, N) / (B, M).  No autograd.
+    Returns ``(f, g, lse2_row | None, lse2_col | None)``."""
+    (B, N, M), (rshape, cshape), (C, log_a, f_old, log_b, g_old) = _dense_inputs(
+        C, ((log_a, "log_a"), (f_old, "f_old")), ((log_b, "log_b"), (g_old, "g_old")))
+    dev = C.device
+    with nvtx_range("b200ot.dense_pair B={} N={} M={} eps={:.3g}", B, N, M, float(eps)):
+        f, lse2_row = torch.empty(rshape, dtype=torch.float32, device=dev), None
+        g, lse2_col = torch.empty(cshape, dtype=torch.float32, device=dev), None
+        if want_lse2:
+            lse2_row, lse2_col = torch.empty_like(f), torch.empty_like(g)
+        scratch = _scratch(_query(dev, "b200ot_dense_scratch_bytes", B, N, M), dev, "dense")
+        _call(dev, "b200ot_dense_softmin_pair", C, log_a, log_b, f_old, g_old, 1.0 / float(eps), float(alpha_old),
+              float(beta), f, g, lse2_row, lse2_col, B, N, M, float(eps), scratch, scratch.numel(), launches=3)
+    return f, g, lse2_row, lse2_col
+
+
+def dense_softmin_pair_grad(eps, C, log_a, log_b, f, g, lse2_row, lse2_col, go_f, go_g):
+    """grad_C of ``<go_f, f~> + <go_g, g~>`` for ``f~, g~ = dense_softmin_pair_raw(eps, C, log_a, log_b, f, g)``
+    (alpha_old = 0, beta = 1: fold a damping factor into go_f, go_g), lse2_* from that call; one pass over C."""
+    (B, N, M), _, (C, log_a, f, lse2_row, go_f, log_b, g, lse2_col, go_g) = _dense_inputs(
+        C, ((log_a, "log_a"), (f, "f"), (lse2_row, "lse2_row"), (go_f, "go_f")),
+        ((log_b, "log_b"), (g, "g"), (lse2_col, "lse2_col"), (go_g, "go_g")))
+    dev = C.device
+    with nvtx_range("b200ot.dense_pair grad B={} N={} M={} eps={:.3g}", B, N, M, float(eps)):
+        grad_C = torch.empty_like(C)
+        _call(dev, "b200ot_dense_softmin_pair_bwd", C, log_a, log_b, f, g, 1.0 / float(eps), lse2_row, lse2_col,
+              go_f, go_g, grad_C, B, N, M, launches=1)
+    return grad_C
+
+
 # which operators serve which clouds: the one place that compares D with MAX_D / MAX_D_TC.  The operators are module
 # globals read at every call, so a replaced operator is the one returned.
 def softmin_operators(D, p=2, batched=False):

@@ -1,4 +1,4 @@
-"""``geomloss.ot.solve_sample`` over the CUDA softmin kernels (SURVEY.md section 8, row f-3).
+"""``geomloss.ot.solve_sample``, ``solve`` and ``solve_batch`` over the CUDA kernels (SURVEY.md section 8, row f-3).
 
 The reference's "new API" for point clouds (src/geomloss/ot/_implementations/sample.py:190-395) builds dense (N, M)
 cost matrices and runs ``sinkhorn_loop`` (ot/_abstract_solvers/sinkhorn_ot.py:240-447) on them.  Here the same
@@ -37,7 +37,8 @@ import torch
 from . import ops
 from .sinkhorn import log_weights, max_diameter
 
-__all__ = ["solve_sample", "solve_sample_batch", "OTResultSample", "LinearOperator"]
+__all__ = ["solve", "solve_batch", "solve_sample", "solve_sample_batch", "OTResultMatrix", "OTResultSample",
+           "LinearOperator"]
 
 _DENSE_LIMIT = 1 << 27  # entries of a dense (N, M) plan we are willing to materialise on request
 
@@ -74,6 +75,17 @@ def _check_marginal(m, like, size, name):
     if bool((m < 0).any()):
         raise ValueError(f"The marginal '{name}' contains negative values. We require that {name} >= 0.")
     return m
+
+
+def _check_masses(sums_a, sums_b):
+    """Balanced problems: the (B,) total masses of a and b agree to 1e-3 relative (_arguments.py:126-156)."""
+    sa, sb = sums_a.double(), sums_b.double()
+    if bool(((sa - sb).abs() / (sa + sb) > 1e-3).any()):
+        which = ("do not sum up to the same value." if sa.numel() == 1 else
+                 "have rows that do not sum up to the same values.")
+        raise ValueError(f"The two arrays of marginal weights 'a' and 'b' {which} As a consequence, the balanced OT "
+                         "problem is not feasible. To fix this error, you may either normalize the two marginals or "
+                         "use UNbalanced optimal transport with the 'unbalanced' keyword argument.")
 
 
 def annealing_eps(maxmin_cost, eps, n_iter):
@@ -197,12 +209,7 @@ def solve_sample(X_a, X_b, a=None, b=None, cost="sqeuclidean", debias=False, reg
     a = _check_marginal(a, X_a[:, 0], N, "a")
     b = _check_marginal(b, X_b[:, 0], M, "b")
     if unbalanced is None:
-        sa, sb = float(a.detach().sum()), float(b.detach().sum())
-        if abs(sa - sb) / (sa + sb) > 1e-3:
-            raise ValueError("The two arrays of marginal weights 'a' and 'b' do not sum up to the same value. As a "
-                             "consequence, the balanced OT problem is not feasible. To fix this error, you may either "
-                             "normalize the two marginals or use UNbalanced optimal transport with the 'unbalanced' "
-                             "keyword argument.")
+        _check_masses(a.detach().sum()[None], b.detach().sum()[None])
     if cost != "sqeuclidean":
         raise NotImplementedError()  # as the reference (sample.py:76-88)
     reg = float(reg)
@@ -263,6 +270,24 @@ def solve_sample_batch(*args, **kwargs):
 # ----------------------------------------------------------------------------------------------------
 # results                                       ot/_ot_result.py:164-440, sample.py:444-641
 # ----------------------------------------------------------------------------------------------------
+def _ot_value(a, b, f_ba, g_ab, eps, rho, f_aa=None, g_bb=None):
+    """The transport cost of dual potentials (unbalanced_ot.py:25-185), debiased when f_aa, g_bb are given, summed over
+    the last axis: a scalar for (N,) / (M,) vectors, (B,) for (B, N) / (B, M) ones.  fp64 inside, float32 out."""
+    a, b, f_ba, g_ab = a.double(), b.double(), f_ba.double(), g_ab.double()
+    debias = f_aa is not None
+    if debias:
+        f_aa, g_bb = f_aa.double(), g_bb.double()
+    if rho is None:
+        F, G = (f_ba - f_aa, g_ab - g_bb) if debias else (f_ba, g_ab)
+    elif not debias:
+        F = (rho + eps / 2 * b.sum(-1, keepdim=True)) - (rho + eps / 2) * torch.exp(-f_ba / rho)
+        G = (rho + eps / 2 * a.sum(-1, keepdim=True)) - (rho + eps / 2) * torch.exp(-g_ab / rho)
+    else:
+        F = (rho + eps / 2) * (torch.exp(-f_aa / rho) - torch.exp(-f_ba / rho))
+        G = (rho + eps / 2) * (torch.exp(-g_bb / rho) - torch.exp(-g_ab / rho))
+    return ((a * F).sum(-1) + (b * G).sum(-1)).float()
+
+
 def _fused_operator(s):
     """Whether ``operator @ s`` runs on the fused kernel (``ops.plan_apply_raw``): every CUDA tensor.  The engine has no
     CPU path; a host tensor is evaluated through ``ops.softmin_raw`` alone, where the real operator refuses it, so that
@@ -349,17 +374,8 @@ class OTResultSample:
     # ---- value                                                   unbalanced_ot.py:25-185 ----------
     @cached_property
     def value(self):
-        a, b, f_aa, g_bb, g_ab, f_ba = (None if t is None else t.double() for t in self._live)
-        eps, rho = self._reg, self._unbalanced
-        if rho is None:
-            F, G = (f_ba - f_aa, g_ab - g_bb) if self._debias else (f_ba, g_ab)
-        elif not self._debias:
-            F = (rho + eps / 2 * b.sum()) - (rho + eps / 2) * torch.exp(-f_ba / rho)
-            G = (rho + eps / 2 * a.sum()) - (rho + eps / 2) * torch.exp(-g_ab / rho)
-        else:
-            F = (rho + eps / 2) * (torch.exp(-f_aa / rho) - torch.exp(-f_ba / rho))
-            G = (rho + eps / 2) * (torch.exp(-g_bb / rho) - torch.exp(-g_ab / rho))
-        return ((a * F).sum() + (b * G).sum()).float()
+        a, b, f_aa, g_bb, g_ab, f_ba = self._live
+        return _ot_value(a, b, f_ba, g_ab, self._reg, self._unbalanced, f_aa, g_bb)
 
     # ---- the plan as an operator ---------------------------------------------------------------------
     # With w_ij = softmax_j(h_j - C_ij / reg), h = log_w + g / reg, and sm the softmin of the same h:
@@ -500,3 +516,209 @@ class _PlanApply(torch.autograd.Function):
     def backward(ctx, go):
         transpose, weighted = ctx.meta
         return None, ctx.res._apply(go, not transpose, weighted), None, None
+
+
+# ----------------------------------------------------------------------------------------------------
+# explicit cost matrices                               ot/_implementations/matrix.py:97-660
+# ----------------------------------------------------------------------------------------------------
+class _fp32_matmul:
+    """Full-precision fp32 matmuls (no TF32) inside the block, the caller's setting restored after it."""
+
+    def __enter__(self):
+        self.prev = torch.get_float32_matmul_precision()
+        torch.set_float32_matmul_precision("highest")
+
+    def __exit__(self, *exc):
+        torch.set_float32_matmul_precision(self.prev)
+
+
+def _dense_at_infinity(C, a, b, damp):
+    """eps = +inf: f_i = sum_j b_j C_ij / sum_j b_j and g_j = sum_i a_i C_ij / sum_i a_i as two matvecs on C (no
+    transpose, no C-sized temporary), minus the per-problem offsets 0.5 <a, f>, 0.5 <b, g>, then damped
+    (sinkhorn_ot.py:17-29, matrix.py:72-81)."""
+    with _fp32_matmul():
+        f = (C @ b.unsqueeze(-1)).squeeze(-1) / b.sum(-1, keepdim=True)
+        g = (a.unsqueeze(-2) @ C).squeeze(-2) / a.sum(-1, keepdim=True)
+    f = damp * (f - 0.5 * (a * f).sum(-1, keepdim=True))
+    g = damp * (g - 0.5 * (b * g).sum(-1, keepdim=True))
+    return f.contiguous(), g.contiguous()
+
+
+class _LastPair(torch.autograd.Function):
+    """The last, non-averaged update ``(f, g) = damp * (softmin rows, softmin columns)`` of C, differentiable w.r.t. C
+    through both softmins; log-weights and incoming potentials are constants (sinkhorn_ot.py:419-436).  ``C`` carries
+    the caller's graph, ``Cd`` is its detached contiguous copy the kernels read."""
+
+    @staticmethod
+    def forward(ctx, C, Cd, log_a, log_b, f, g, eps, damp):
+        f_new, g_new, lse2_row, lse2_col = ops.dense_softmin_pair_raw(eps, Cd, log_a, log_b, f, g, beta=damp,
+                                                                      want_lse2=True)
+        ctx.save_for_backward(Cd, log_a, log_b, f, g, lse2_row, lse2_col)
+        ctx.meta = (float(eps), float(damp))
+        return f_new, g_new
+
+    @staticmethod
+    def backward(ctx, go_f, go_g):
+        Cd, log_a, log_b, f, g, lse2_row, lse2_col = ctx.saved_tensors
+        eps, damp = ctx.meta
+        grad_C = ops.dense_softmin_pair_grad(eps, Cd, log_a, log_b, f, g, lse2_row, lse2_col,
+                                             (damp * go_f).contiguous(), (damp * go_g).contiguous())
+        return grad_C, None, None, None, None, None, None, None
+
+
+def solve(C, *, reg, a=None, b=None, unbalanced=None, unbalanced_type="KL", method="auto", max_iter=None, tol=None):
+    """Entropic (un)balanced OT on an explicit (N, M) cost matrix; mirrors ``geomloss.ot.solve`` (matrix.py:348-512).
+
+    C: (N, M), a: (N,), b: (M,) float32 CUDA tensors (a, b non-negative, uniform 1/N, 1/M if None); ``reg`` is the
+    temperature eps, ``unbalanced`` the marginal penalty rho (None: balanced).  Use this for any cost that is not
+    ``|x - y|^p`` on point clouds: build C, then solve.  A non-contiguous C is copied once.  Returns an
+    :class:`OTResultMatrix` without batch axis."""
+    if not torch.is_tensor(C):
+        raise TypeError("C must be a torch CUDA tensor (this engine has no NumPy / CPU path)")
+    if C.dim() != 2:
+        raise ValueError("The 'cost' matrix should be an array with 2 dimensions. "
+                         f"Instead, ot.solve received an array of shape {C.shape}.")
+    N, M = C.shape
+    a = _check_marginal(a, C[:, 0], N, "a")
+    b = _check_marginal(b, C[0, :], M, "b")
+    res = solve_batch(C[None], reg=reg, a=a[None], b=b[None], unbalanced=unbalanced, unbalanced_type=unbalanced_type,
+                      method=method, max_iter=max_iter, tol=tol)
+    res._batched = False
+    return res
+
+
+def solve_batch(C, *, reg, a=None, b=None, unbalanced=None, unbalanced_type="KL", method="auto", max_iter=None,
+                tol=None):
+    """B independent problems of :func:`solve` in one solver, C: (B, N, M), a: (B, N), b: (B, M); mirrors
+    ``geomloss.ot.solve_batch`` (matrix.py:515-660).  The eps ladder starts from max(C) - min(C) over the whole batch.
+
+    Each iteration is ONE pass over C for both potentials (``ops.dense_softmin_pair_raw``): no transposed copy and
+    no (B, N, M) temporary.  ``result.value`` is differentiable w.r.t. C through the last update (both softmins) and
+    w.r.t. a and b through the value formula."""
+    _check_regularization(reg, unbalanced, unbalanced_type, method, tol, max_iter)
+    if not torch.is_tensor(C):
+        raise TypeError("C must be a torch CUDA tensor (this engine has no NumPy / CPU path)")
+    if C.dim() != 3:
+        raise ValueError("The 'cost' matrix should be an array with 3 dimensions (batch, N, M). "
+                         f"Instead, ot.solve received an array of shape {C.shape}.")
+    B, N, M = C.shape
+    a = _check_marginal(a, C[:, :, 0], N, "a")
+    b = _check_marginal(b, C[:, 0, :], M, "b")
+    if unbalanced is None:
+        _check_masses(a.detach().sum(-1), b.detach().sum(-1))
+    for t, name in ((C, "C"), (a, "a"), (b, "b")):
+        if not (t.is_cuda and t.dtype == torch.float32):
+            raise TypeError(f"{name} must be a float32 CUDA tensor (this engine computes in fp32 on the GPU), got "
+                            f"{t.dtype} on {t.device}")
+    reg = float(reg)
+    rho = None if unbalanced is None else float(unbalanced)
+
+    def damp(eps):
+        return 1.0 if rho is None else 1.0 / (1.0 + eps / rho)
+
+    want_grad = torch.is_grad_enabled() and any(t.requires_grad for t in (C, a, b))
+    with torch.no_grad():
+        Cd = C.detach().contiguous()
+        a_d, b_d = a.detach().contiguous(), b.detach().contiguous()
+        eps_list = annealing_eps(float(Cd.amax() - Cd.amin()), reg, int(max_iter))
+        log_a, log_b = log_weights(a_d), log_weights(b_d)
+        lam = damp(eps_list[0])
+        f, g = _dense_at_infinity(Cd, a_d, b_d, lam)
+        for eps in eps_list:
+            lam = damp(eps)
+            f, g, _, _ = ops.dense_softmin_pair_raw(eps, Cd, log_a, log_b, f, g, alpha_old=0.5, beta=0.5 * lam)
+        if not want_grad:  # last, non-averaged update (last_extrapolation=True, sinkhorn_ot.py:419-436)
+            f, g, _, _ = ops.dense_softmin_pair_raw(eps, Cd, log_a, log_b, f, g, beta=lam)
+    if want_grad:
+        f, g = _LastPair.apply(C, Cd, log_a, log_b, f, g, eps, lam)
+    return OTResultMatrix(C=Cd, a=a, b=b, reg=reg, unbalanced=rho, potentials=(f, g))
+
+
+class OTResultMatrix:
+    """Result of :func:`solve` / :func:`solve_batch`; lazily evaluated, cached attributes named like the reference's
+    (matrix.py:97-345): ``value``, ``potential_a``, ``potential_b``, ``marginal_a``, ``marginal_b``, ``density``,
+    ``plan``, ``density_operator``, ``plan_operator``; ``lazy_plan``, ``lazy_density`` are ``None``.  Shapes follow
+    the solver: (N,) / (M,) / (N, M) for :func:`solve`, with a leading batch axis B for :func:`solve_batch`.
+
+    Only ``value`` is attached to the caller's graph; every other attribute is returned detached.  ``density`` and
+    ``plan`` are dense (N, M) tensors, as in the reference, built once and cached; the operators apply them."""
+
+    def __init__(self, *, C, a, b, reg, unbalanced, potentials):
+        self._C, self._a, self._b = C, a.detach(), b.detach()
+        self._reg, self._unbalanced = reg, unbalanced
+        self._live = (a, b) + tuple(potentials)  # possibly attached to the caller's graph: used by `value` only
+        self._f, self._g = (t.detach() for t in potentials)
+        self._batched = True
+
+    def _out(self, t):
+        return t if self._batched else t[0]
+
+    @property
+    def potential_a(self):
+        return self._out(self._f)
+
+    @property
+    def potential_b(self):
+        return self._out(self._g)
+
+    @cached_property
+    def value(self):
+        a, b, f, g = self._live
+        return self._out(_ot_value(a, b, f, g, self._reg, self._unbalanced))
+
+    # (the plan's marginals: a_i sum_j b_j density_ij = a_i exp((f_i - softmin_i) / eps), and the same on columns,
+    # from one pass over C)
+    @cached_property
+    def _marginals(self):
+        eps = self._reg
+        with torch.no_grad():
+            sm_f, sm_g, _, _ = ops.dense_softmin_pair_raw(eps, self._C, log_weights(self._a), log_weights(self._b),
+                                                          self._f, self._g)
+            return self._a * torch.exp((self._f - sm_f) / eps), self._b * torch.exp((self._g - sm_g) / eps)
+
+    @cached_property
+    def marginal_a(self):
+        return self._out(self._marginals[0])
+
+    @cached_property
+    def marginal_b(self):
+        return self._out(self._marginals[1])
+
+    @cached_property
+    def density(self):
+        with torch.no_grad():
+            return self._out(torch.exp((self._f[:, :, None] + self._g[:, None, :] - self._C) / self._reg))
+
+    @cached_property
+    def plan(self):
+        a, b = self._out(self._a), self._out(self._b)
+        return self.density * a[..., :, None] * b[..., None, :]
+
+    def _operator(self, P):
+        def matmat(s):  # (M, K) -> (N, K), or (B, M, K) -> (B, N, K)
+            with _fp32_matmul():
+                return P @ s.to(P.dtype)
+
+        def rmatmat(s):
+            with _fp32_matmul():
+                return P.transpose(-1, -2) @ s.to(P.dtype)
+
+        B, N, M = self._C.shape
+        lead = (B,) if self._batched else ()
+        return LinearOperator(matmat=matmat, rmatmat=rmatmat, input_shape=lead + (M,), output_shape=lead + (N,))
+
+    @cached_property
+    def density_operator(self):
+        return self._operator(self.density)
+
+    @cached_property
+    def plan_operator(self):
+        return self._operator(self.plan)
+
+    lazy_density = None
+    lazy_plan = None
+
+    def cache_clear(self):
+        for k in ("value", "_marginals", "marginal_a", "marginal_b", "density", "plan", "density_operator",
+                  "plan_operator"):
+            self.__dict__.pop(k, None)

@@ -330,6 +330,32 @@ B200OT_API int b200ot_wide_plan_apply(const float* x, const float* y, const floa
                                       int32_t p, float eps, void* scratch, int64_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Explicit cost matrices: both softmins of one symmetric Sinkhorn update from ONE pass over C
+ * replaces softmin_dense on C and on a contiguous copy of C^T (ot/_implementations/matrix.py:29-94, :620-660):
+ *   f_out[b,i] <- alpha_old * f_old[b,i] + beta * (-eps log sum_j exp(log_b[b,j] + inv_eps g_old[b,j] - inv_eps C[b,i,j]))
+ *   g_out[b,j] <- alpha_old * g_old[b,j] + beta * (-eps log sum_i exp(log_a[b,i] + inv_eps f_old[b,i] - inv_eps C[b,i,j]))
+ * C (B,N,M) row-major fp32, any alignment; log_a, f_old (B,N); log_b, g_old (B,M); f_out, g_out must not alias the
+ * inputs.  lse2_row (B,N), lse2_col (B,M) (nullable): the log2-domain log-sum-exps, for the backward entry.
+ * Three launches: the pass over C, then b200ot_softmin_finalize for the rows and for the columns.
+ * EINVAL (before any launch) for null pointers (lse2_* excepted), B, N or M <= 0, eps or inv_eps <= 0; EALIGN for a
+ * scratch not 16-byte aligned; ESCRATCH below b200ot_dense_scratch_bytes(B, N, M), a pure function of the shape.
+ * ------------------------------------------------------------------------------------------- */
+B200OT_API int64_t b200ot_dense_scratch_bytes(int64_t B, int64_t N, int64_t M);
+B200OT_API int b200ot_dense_softmin_pair(const float* C, const float* log_a, const float* log_b, const float* f_old,
+                                         const float* g_old, float inv_eps, float alpha_old, float beta, float* f_out,
+                                         float* g_out, float* lse2_row, float* lse2_col, int64_t B, int64_t N,
+                                         int64_t M, float eps, void* scratch, int64_t scratch_bytes, void* stream);
+/* Gradient of <go_f, f~> + <go_g, g~> w.r.t. C for the pair above (alpha_old = 0, beta = 1; fold a damping factor into
+ * go_*), f and g the potentials the forward read and lse2_* its outputs; one pass, grad_C (B,N,M) overwritten:
+ *   grad_C[b,i,j] = go_f[b,i] 2^(t_ij - lse2_row[b,i]) + go_g[b,j] 2^(u_ij - lse2_col[b,j]),
+ *   t_ij = log2e (log_b[b,j] + inv_eps (g[b,j] - C[b,i,j])),  u_ij = log2e (log_a[b,i] + inv_eps (f[b,i] - C[b,i,j])).
+ * EINVAL (before any launch) for null pointers, B, N or M <= 0, inv_eps <= 0. */
+B200OT_API int b200ot_dense_softmin_pair_bwd(const float* C, const float* log_a, const float* log_b, const float* f,
+                                             const float* g, float inv_eps, const float* lse2_row,
+                                             const float* lse2_col, const float* go_f, const float* go_g,
+                                             float* grad_C, int64_t B, int64_t N, int64_t M, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Block-sparse softmins in the tensor-core dimensions (8 < D <= 64, p = 2 or 2 | B200OT_P_UNCLAMPED): the fine phase
  * of the two-scale Sinkhorn with user cluster labels (sinkhorn_multiscale, sinkhorn_samples.py:547-681), the
  * counterpart of the ranges entries above, which serve D <= B200OT_MAX_D.  A separate family with its own layout:
