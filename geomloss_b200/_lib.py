@@ -98,6 +98,9 @@ _SIGNATURES = {
                                             c_int64, c_int64, c_float, _P, c_int64, _P]),
     "b200ot_dense_softmin_pair_bwd": (c_int32, [_P, _P, _P, _P, _P, c_float, _P, _P, _P, _P, _P, c_int64, c_int64,
                                                 c_int64, _P]),
+    "b200ot_dense_rows_scratch_bytes": (c_int64, [_P, c_int32]),
+    "b200ot_dense_softmin_rows": (c_int32, [_P, c_int32, c_float, c_float, c_float, _P, c_int64, _P]),
+    "b200ot_dense_softmin_rows_bwd": (c_int32, [_P, _P, _P, c_float, _P, _P, _P, c_int64, c_int64, c_int64, _P]),
     "b200ot_blocks_shape": (None, [ctypes.POINTER(c_int32), ctypes.POINTER(c_int32)]),
     "b200ot_blocks_scratch_bytes": (c_int64, [c_int64, c_int64, c_int64, _P, c_int64, _P, c_int32]),
     "b200ot_softmin_fwd_blocks": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, c_float, c_float, _P, _P, c_int64, _P,
@@ -122,6 +125,12 @@ _SIGNATURES = {
                                       c_float, _P]),
     "b200ot_ubench": (c_int32, [c_int32, c_int32, c_int32, _P, ctypes.POINTER(c_int32), _P]),
 }
+
+
+class DenseRows(ctypes.Structure):
+    """``b200ot_dense_rows`` of include/b200ot.h: one problem of a b200ot_dense_softmin_rows group."""
+    _fields_ = [("C", _P), ("log_w", _P), ("pot", _P), ("out_old", _P), ("out", _P), ("lse2", _P), ("B", c_int64),
+                ("n_rows", c_int64), ("n_cols", c_int64)]
 
 
 def exported_symbols():

@@ -241,6 +241,160 @@ __global__ void __launch_bounds__(kDenseBwdCols)
   }
 }
 
+
+// ---- row softmins only: the four Jacobi updates of SamplesLoss("sinkhorn", cost=...) (DESIGN.md section 3.9) ----
+// Each matrix of a group has its own C (B, n_rows, n_cols), column log-weights and column potential; per entry
+//   t_ij = log2e (log_w_j + pot_j / eps - C_ij / eps),   out_i = -eps ln2 LSE2_j t_ij   (finalize).
+// No column direction, so no barrier and no column partials: a warp owns kRowsRPW rows and sweeps its split's columns
+// in steps of 128 (4 consecutive columns per lane, one 16-byte load per row on the aligned path), reusing each column's
+// h across its rows.  The row sums stay in registers with the sum-guarded lazy max and are merged across lanes once.
+// Both load paths visit the same entries in the same order and share the arithmetic, so they return the same bits.
+constexpr int kRowsRPW = 8;                         // rows per warp: 16-byte loads in flight per lane and step
+constexpr int kRowsCTA = kDenseWarps * kRowsRPW;    // 64 rows per CTA
+constexpr int kRowsStep = 4 * 32;                   // columns per warp step
+constexpr int kRowsMinSteps = 4;                    // steps per split at least (512 columns)
+constexpr int kRowsMaxGroup = 4;
+
+struct RowsPlan {
+  int64_t row_blocks, steps;
+  int n_split, steps_per_split;
+};
+
+// Pure function of the shape (no device query), so that scratch sizes are reproducible on any host.
+inline RowsPlan rows_plan(int64_t B, int64_t N, int64_t M) {
+  RowsPlan p;
+  p.row_blocks = ceil_div64(N, kRowsCTA);
+  p.steps = ceil_div64(M, kRowsStep);
+  int64_t want = ceil_div64(kDenseTarget, p.row_blocks * B);
+  const int64_t cap = ceil_div64(p.steps, kRowsMinSteps);
+  want = want < 1 ? 1 : (want > cap ? cap : want);
+  p.steps_per_split = (int)ceil_div64(p.steps, want);
+  p.n_split = (int)ceil_div64(p.steps, p.steps_per_split);  // every split owns at least one step
+  return p;
+}
+
+inline int64_t rows_part_bytes(const RowsPlan& p, int64_t B, int64_t N) {
+  return round_up64((int64_t)p.n_split * B * N * 8, 256);
+}
+
+struct RowsProblem {
+  const float* C;
+  const float* log_w;
+  const float* pot;  // null: 0
+  float2* part;      // part[s (B N) + b N + i], s < n_split
+  int64_t B, N, M, row_blocks, steps, cta_begin;
+  int n_split, steps_per_split, vec;
+};
+struct RowsGroup {
+  RowsProblem p[kRowsMaxGroup];
+  int n;
+};
+
+template <bool VEC>
+__device__ __forceinline__ void dense_rows_reduce(const RowsProblem& d, int64_t blk, float inv_eps) {
+  const int split = (int)(blk % d.n_split);
+  blk /= d.n_split;
+  const int64_t rb = blk % d.row_blocks;
+  const int64_t b = blk / d.row_blocks;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t N = d.N, M = d.M;
+  const int64_t i0 = rb * kRowsCTA + warp * kRowsRPW;
+  if (i0 >= N) return;  // no barrier in this kernel: a warp of padding rows leaves at once
+  const float sc = kLog2e * inv_eps;
+  const float* __restrict__ Cw = d.C + (b * N + i0) * M;
+  const float* __restrict__ lw = d.log_w + b * M;
+  const float* __restrict__ pt = d.pot ? d.pot + b * M : nullptr;
+  float mr[kRowsRPW], sr[kRowsRPW];
+#pragma unroll
+  for (int k = 0; k < kRowsRPW; ++k) {
+    mr[k] = kNegBig;
+    sr[k] = 0.f;
+  }
+  const int64_t s0 = (int64_t)split * d.steps_per_split;
+  const int64_t s_end = min(s0 + d.steps_per_split, d.steps);
+  for (int64_t s = s0; s < s_end; ++s) {
+    const int64_t j0 = s * kRowsStep + 4 * lane;
+    float c[kRowsRPW][4];
+#pragma unroll
+    for (int k = 0; k < kRowsRPW; ++k) {
+      const bool rv = i0 + k < N;
+      if (VEC) {  // M % 4 == 0: the lane's 4 columns are all in range or all out
+        const float4 v = (rv && j0 < M) ? __ldg(reinterpret_cast<const float4*>(Cw + k * M + j0))
+                                        : make_float4(0.f, 0.f, 0.f, 0.f);
+        c[k][0] = v.x, c[k][1] = v.y, c[k][2] = v.z, c[k][3] = v.w;
+      } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) c[k][q] = (rv && j0 + q < M) ? __ldg(Cw + k * M + j0 + q) : 0.f;
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int64_t j = j0 + q;
+      if (j >= M) continue;
+      const float h = kLog2e * (pt ? fmaf(inv_eps, __ldg(pt + j), __ldg(lw + j)) : __ldg(lw + j));
+#pragma unroll
+      for (int k = 0; k < kRowsRPW; ++k) {
+        // one term per entry, the running max raised only when a term exceeds it by 2^64 (kDenseGuard)
+        const float t = fmaf(c[k][q], -sc, h);
+        const float e = ex2_approx(t - mr[k]);
+        if (e > kDenseGuard) {
+          sr[k] = fmaf(sr[k], ex2_approx(mr[k] - t), 1.f);
+          mr[k] = t;
+        } else {
+          sr[k] += e;
+        }
+      }
+    }
+  }
+  // across the 32 lanes, then lane k writes row i0 + k
+#pragma unroll
+  for (int k = 0; k < kRowsRPW; ++k) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+      merge_pair(mr[k], sr[k], __shfl_xor_sync(0xffffffffu, mr[k], o), __shfl_xor_sync(0xffffffffu, sr[k], o));
+    if (lane == k && i0 + k < N) d.part[(int64_t)split * (d.B * N) + b * N + i0 + k] = make_float2(mr[k], sr[k]);
+  }
+}
+
+// The group's CTAs are enumerated problem after problem; the descriptors travel by value.
+__global__ void __launch_bounds__(kDenseWarps * 32) dense_rows_kernel(const __grid_constant__ RowsGroup g, float inv_eps) {
+  const int64_t blk = blockIdx.x;
+  int k = 0;
+#pragma unroll
+  for (int q = 1; q < kRowsMaxGroup; ++q)
+    if (q < g.n && blk >= g.p[q].cta_begin) k = q;
+  const RowsProblem& d = g.p[k];
+  if (d.vec)
+    dense_rows_reduce<true>(d, blk - d.cta_begin, inv_eps);
+  else
+    dense_rows_reduce<false>(d, blk - d.cta_begin, inv_eps);
+}
+
+// grad_C_ij = go_i 2^(t_ij - lse2_i): C read once, grad_C written once; kDenseRPW rows x 256 columns per CTA.
+__global__ void __launch_bounds__(kDenseBwdCols)
+    dense_rows_bwd_kernel(const float* __restrict__ C, const float* __restrict__ log_w, const float* __restrict__ pot,
+                          float inv_eps, const float* __restrict__ lse2, const float* __restrict__ go,
+                          float* __restrict__ grad_C, int64_t N, int64_t M, int64_t row_blocks, int64_t col_blocks) {
+  int64_t blk = blockIdx.x;
+  const int64_t cb = blk % col_blocks;
+  blk /= col_blocks;
+  const int64_t rb = blk % row_blocks;
+  const int64_t b = blk / row_blocks;
+  const int64_t j = cb * kDenseBwdCols + threadIdx.x;
+  if (j >= M) return;
+  const float sc = kLog2e * inv_eps;
+  const float h = kLog2e * (pot ? fmaf(inv_eps, __ldg(pot + b * M + j), __ldg(log_w + b * M + j)) : __ldg(log_w + b * M + j));
+  const int64_t i0 = rb * kDenseRPW;
+#pragma unroll 4
+  for (int k = 0; k < kDenseRPW; ++k) {
+    const int64_t i = i0 + k;
+    if (i >= N) break;
+    const int64_t r = b * N + i;
+    const float c = __ldg(C + r * M + j);
+    grad_C[r * M + j] = __ldg(go + r) * ex2_approx(fmaf(c, -sc, h) - __ldg(lse2 + r));
+  }
+}
+
 }  // namespace b200ot
 
 using namespace b200ot;
@@ -297,6 +451,66 @@ B200OT_API int b200ot_dense_softmin_pair_bwd(const float* C, const float* log_a,
   if (grid > 0x7fffffff) return B200OT_EINVAL;
   dense_pair_bwd_kernel<<<(unsigned)grid, kDenseBwdCols, 0, (cudaStream_t)stream>>>(
       C, log_a, log_b, f, g, inv_eps, lse2_row, lse2_col, go_f, go_g, grad_C, B, N, M, row_blocks, col_blocks);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+
+B200OT_API int64_t b200ot_dense_rows_scratch_bytes(const b200ot_dense_rows* probs, int32_t n) {
+  if (!probs || n < 1 || n > B200OT_DENSE_ROWS_MAX) return 0;
+  int64_t total = 0;
+  for (int k = 0; k < n; ++k) {
+    const b200ot_dense_rows& q = probs[k];
+    if (q.B <= 0 || q.n_rows <= 0 || q.n_cols <= 0) return 0;
+    total += rows_part_bytes(rows_plan(q.B, q.n_rows, q.n_cols), q.B, q.n_rows);
+  }
+  return total;
+}
+
+B200OT_API int b200ot_dense_softmin_rows(const b200ot_dense_rows* probs, int32_t n, float eps, float alpha_old,
+                                         float beta, void* scratch, int64_t scratch_bytes, void* stream) {
+  if (!probs || n < 1 || n > B200OT_DENSE_ROWS_MAX || !scratch || !(eps > 0.f)) return B200OT_EINVAL;
+  RowsGroup g = {};
+  g.n = n;
+  int64_t grid = 0, offset = 0;
+  for (int k = 0; k < n; ++k) {
+    const b200ot_dense_rows& q = probs[k];
+    if (!q.C || !q.log_w || (!q.out && !q.lse2) || q.B <= 0 || q.n_rows <= 0 || q.n_cols <= 0) return B200OT_EINVAL;
+    const RowsPlan pl = rows_plan(q.B, q.n_rows, q.n_cols);
+    RowsProblem& d = g.p[k];
+    d.C = q.C, d.log_w = q.log_w, d.pot = q.pot;
+    d.part = reinterpret_cast<float2*>(reinterpret_cast<char*>(scratch) + offset);
+    d.B = q.B, d.N = q.n_rows, d.M = q.n_cols, d.row_blocks = pl.row_blocks, d.steps = pl.steps, d.cta_begin = grid;
+    d.n_split = pl.n_split, d.steps_per_split = pl.steps_per_split;
+    d.vec = (((uintptr_t)q.C) & 15) == 0 && q.n_cols % 4 == 0;
+    grid += pl.row_blocks * q.B * pl.n_split;
+    offset += rows_part_bytes(pl, q.B, q.n_rows);
+  }
+  if (grid > 0x7fffffff) return B200OT_EINVAL;
+  if (const int rc = scratch_check(scratch, scratch_bytes, offset)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  dense_rows_kernel<<<(unsigned)grid, kDenseWarps * 32, 0, st>>>(g, 1.f / eps);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  for (int k = 0; k < n; ++k) {
+    const b200ot_dense_rows& q = probs[k];
+    const int rc = b200ot_softmin_finalize(reinterpret_cast<const float*>(g.p[k].part), g.p[k].n_split, q.out_old,
+                                           alpha_old, beta, q.out, q.lse2, q.B * q.n_rows, eps, stream);
+    if (rc) return rc;
+  }
+  return B200OT_OK;
+}
+
+B200OT_API int b200ot_dense_softmin_rows_bwd(const float* C, const float* log_w, const float* pot, float inv_eps,
+                                             const float* lse2, const float* go, float* grad_C, int64_t B, int64_t N,
+                                             int64_t M, void* stream) {
+  if (!C || !log_w || !lse2 || !go || !grad_C || B <= 0 || N <= 0 || M <= 0 || !(inv_eps > 0.f))
+    return B200OT_EINVAL;
+  const int64_t row_blocks = ceil_div64(N, kDenseRPW), col_blocks = ceil_div64(M, kDenseBwdCols);
+  const int64_t grid = B * row_blocks * col_blocks;
+  if (grid > 0x7fffffff) return B200OT_EINVAL;
+  dense_rows_bwd_kernel<<<(unsigned)grid, kDenseBwdCols, 0, (cudaStream_t)stream>>>(C, log_w, pot, inv_eps, lse2, go,
+                                                                                     grad_C, N, M, row_blocks,
+                                                                                     col_blocks);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }

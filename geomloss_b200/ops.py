@@ -609,6 +609,50 @@ def dense_softmin_pair_grad(eps, C, log_a, log_b, f, g, lse2_row, lse2_col, go_f
     return grad_C
 
 
+DENSE_ROWS_MAX = 4  # B200OT_DENSE_ROWS_MAX: matrices per dense_softmin_rows_raw call
+
+
+def dense_softmin_rows_raw(eps, problems, *, alpha_old=0.0, beta=1.0, want_lse2=False):
+    """The row softmins of 1 to 4 cost matrices in one partials launch (b200ot_dense_softmin_rows), each averaged /
+    damped like ``softmin_raw``:
+        out <- alpha_old out_old + beta (-eps log sum_j exp(log_w_j + (pot_j - C_ij) / eps)).
+    ``problems``: ``[(C, log_w, pot | None, out_old | None), ...]``, C (N, M) or (B, N, M), log_w and pot (M,) / (B, M),
+    out_old (N,) / (B, N); the matrices may differ in shape.  No autograd.  Returns ``[(out, lse2 | None), ...]``."""
+    if not 1 <= len(problems) <= DENSE_ROWS_MAX:
+        raise ValueError(f"expected 1 to {DENSE_ROWS_MAX} problems, got {len(problems)}")
+    checked = [_dense_inputs(C, ((out_old, "out_old"),), ((log_w, "log_w"), (pot, "pot")))
+               for C, log_w, pot, out_old in problems]
+    dev = checked[0][2][0].device
+    if any(ready[0].device != dev for _, _, ready in checked):
+        raise ValueError(f"every problem must live on one device ({dev})")
+    with nvtx_range("b200ot.dense_rows n={} eps={:.3g}", len(problems), float(eps)):
+        descs, results = (_lib.DenseRows * len(problems))(), []
+        for d, ((B, N, M), (rshape, _), (C, out_old, log_w, pot)) in zip(descs, checked):
+            out = torch.empty(rshape, dtype=torch.float32, device=dev)
+            lse2 = torch.empty_like(out) if want_lse2 else None
+            d.C, d.log_w, d.pot, d.out_old, d.out, d.lse2 = (None if t is None else t.data_ptr()
+                                                             for t in (C, log_w, pot, out_old, out, lse2))
+            d.B, d.n_rows, d.n_cols = B, N, M
+            results.append((out, lse2))
+        scratch = _scratch(_query(dev, "b200ot_dense_rows_scratch_bytes", descs, len(descs)), dev, "dense_rows")
+        _call(dev, "b200ot_dense_softmin_rows", descs, len(descs), float(eps), float(alpha_old), float(beta), scratch,
+              scratch.numel(), launches=1 + len(problems))
+    return results
+
+
+def dense_softmin_rows_grad(eps, C, log_w, pot, lse2, go):
+    """grad_C of ``<go, out~>`` for ``out~, lse2 = dense_softmin_rows_raw(eps, [(C, log_w, pot, None)],
+    want_lse2=True)[0]`` (alpha_old = 0, beta = 1: fold a damping factor into go); one pass over C."""
+    (B, N, M), _, (C, lse2, go, log_w, pot) = _dense_inputs(C, ((lse2, "lse2"), (go, "go")),
+                                                            ((log_w, "log_w"), (pot, "pot")))
+    dev = C.device
+    with nvtx_range("b200ot.dense_rows grad B={} N={} M={} eps={:.3g}", B, N, M, float(eps)):
+        grad_C = torch.empty_like(C)
+        _call(dev, "b200ot_dense_softmin_rows_bwd", C, log_w, pot, 1.0 / float(eps), lse2, go, grad_C, B, N, M,
+              launches=1)
+    return grad_C
+
+
 # which operators serve which clouds: the one place that compares D with MAX_D / MAX_D_TC.  The operators are module
 # globals read at every call, so a replaced operator is the one returned.
 def softmin_operators(D, p=2, batched=False):

@@ -27,6 +27,12 @@ kernel_conv_batched) and the wide ones for 64 < D <= 1024 (ops.softmin_wide, ker
 multi-GPU engines solve the batch element by element.
 Above D = 64 every loss runs on the wide tensor-core operators (K-slab kernels, DESIGN.md section 3.5d), up to
 D = 1024; above that, and for labelled two-scale calls or column-sharded engines above D = 64, NotImplementedError.
+``cost=`` (a callable taking (B,N,D), (B,M,D) clouds and returning the (B,N,M) cost matrix) runs for the Sinkhorn loss
+where the reference runs it, on the "tensorized" backend (chosen, picked by "auto" for N*M <= 5000**2, or reached by the
+batched multiscale fallback), for any p > 0 and any D: the four matrices are formed by the user's function and each
+Jacobi iteration's row softmins are one sm_90a launch (sinkhorn.sinkhorn_cost_matrices).  KeOps formula strings, the
+"online" and "multiscale" backends, labels, column-sharded engines and the kernel losses raise NotImplementedError
+with a cost.
 Inputs must be float32 CUDA tensors: there is no CPU path.
 """
 from __future__ import annotations
@@ -40,7 +46,7 @@ from .kernel_loss import kernel_points, kernel_points_batched
 from .multiscale import kernel_multiscale, sinkhorn_multiscale
 from .ops import MAX_D, MAX_D_TC, MAX_D_WIDE
 from . import kernel_small, sinkhorn_small
-from .sinkhorn import sinkhorn_points, sinkhorn_points_batched
+from .sinkhorn import sinkhorn_cost_matrices, sinkhorn_points, sinkhorn_points_batched
 
 _LOSSES = ("sinkhorn", "hausdorff", "energy", "gaussian", "laplacian")
 
@@ -60,6 +66,10 @@ def _route(loss):
     if loss in ("energy", "gaussian", "laplacian"):
         return lambda *args, **kw: kernel_points(*args, name=loss, **kw)
     raise KeyError(loss)
+
+
+def _cuda_f32(*tensors):
+    return all(t.is_cuda and t.dtype == torch.float32 for t in tensors)
 
 
 _uniform_weights: dict = {}
@@ -119,9 +129,21 @@ class SamplesLoss(Module):
                           "beware of memory overflows!")
             backend = "tensorized"
         if self.cost is not None:
+            if (self.loss == "sinkhorn" and backend == "tensorized" and callable(self.cost) and not self._engine
+                    and self._multiscale_engine is None and _cuda_f32(a, x, b, y)):
+                # the user's cost matrices, row softmins on the GPU (sinkhorn.sinkhorn_cost_matrices)
+                values = sinkhorn_cost_matrices(a, x, b, y, self.cost, p=self.p, blur=self.blur, reach=self.reach,
+                                                diameter=self.diameter, scaling=self.scaling, debias=self.debias,
+                                                potentials=self.potentials)
+                if self.potentials:
+                    return values[0].view(-1, N), values[1].view(-1, M)
+                return values
             raise NotImplementedError(
-                "custom cost functions need a dense (B,N,M) cost matrix or a KeOps formula; the CUDA engine "
-                "only evaluates |x-y|^p/p, p in {1,2}, on the fly")
+                "a custom cost (a callable returning the (B,N,M) cost matrix) runs with loss='sinkhorn' and "
+                "backend='tensorized' (chosen, or picked by 'auto' for "
+                "N*M <= 5000**2) on float32 CUDA clouds, without labels or column-sharded engines: the engine forms "
+                "the user's (B,N,M) cost matrices there; KeOps formulas, the 'online' and 'multiscale' backends "
+                "and the kernel losses evaluate only |x-y|^p/p, p in {1,2}, on the fly")
         routine = _route(self.loss)
         kw = dict(p=self.p, blur=self.blur, reach=self.reach, diameter=self.diameter, scaling=self.scaling,
                   debias=self.debias, potentials=self.potentials, kernel=self.kernel,

@@ -240,3 +240,96 @@ def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=Non
     if potentials:
         return out[0].view(B, N), out[1].view(B, M)
     return out
+
+
+class _LastRows(torch.autograd.Function):
+    """The last, non-averaged update ``lam * softmin(eps, C_k, log_w_k + pot_k / eps)`` of the 2 or 4 cost matrices
+    in one group, differentiable w.r.t. each C_k; log-weights and potentials are constants, as the reference's
+    detached right-hand sides make them (sinkhorn_divergence.py:612-623).  ``rest`` is the k matrices (each carrying
+    the caller's graph, contiguous) followed by their k log-weights and k potentials."""
+
+    @staticmethod
+    def forward(ctx, eps, lam, *rest):
+        k = len(rest) // 3
+        Cs, logs, pots = rest[:k], rest[k:2 * k], rest[2 * k:]
+        res = ops.dense_softmin_rows_raw(eps, [(C, lw, pot, None) for C, lw, pot in zip(Cs, logs, pots)], beta=lam,
+                                         want_lse2=True)
+        ctx.save_for_backward(*Cs, *logs, *pots, *(lse2 for _, lse2 in res))
+        ctx.meta = (k, float(eps), float(lam))
+        return tuple(out for out, _ in res)
+
+    @staticmethod
+    def backward(ctx, *gos):
+        k, eps, lam = ctx.meta
+        saved = ctx.saved_tensors
+        grads = [None] * k
+        for i in range(k):
+            if ctx.needs_input_grad[2 + i] and gos[i] is not None:
+                grads[i] = ops.dense_softmin_rows_grad(eps, saved[i], saved[k + i], saved[2 * k + i], saved[3 * k + i],
+                                                       (lam * gos[i]).contiguous())
+        return (None, None, *grads) + (None,) * (2 * k)
+
+
+def _cost_matrix(cost, u, v, name, rows, cols, like):
+    """``cost(u, v)`` checked like an operator input: (B, rows, cols), of ``like``'s dtype (float32 for the kernels)
+    and on its device; a non-contiguous result (a transposed view, ...) is copied once."""
+    C = cost(u, v)
+    B = u.shape[0]
+    if not torch.is_tensor(C) or tuple(C.shape) != (B, rows, cols):
+        shape = tuple(C.shape) if torch.is_tensor(C) else type(C).__name__
+        raise ValueError(f"cost(x, y) must return the (B, N, M) = {(B, rows, cols)} matrix {name}, got {shape}")
+    if C.dtype != like.dtype or C.device != like.device:
+        raise TypeError(f"cost(x, y) must return a {like.dtype} tensor on {like.device} ({name}), got {C.dtype} on "
+                        f"{C.device}")
+    return C.contiguous()
+
+
+def sinkhorn_cost_matrices(a, x, b, y, cost, p=2, blur=0.05, reach=None, diameter=None, scaling=0.5, debias=True,
+                           potentials=False):
+    """Sinkhorn divergence with a user-supplied cost: the reference's "tensorized" backend with ``cost=``
+    (sinkhorn_samples.py:74-221), for a:(N,) x:(N,D) b:(M,) y:(M,D) or a batch a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D).
+
+    ``cost`` is called exactly as the reference calls it, on (B, n, D) clouds (B = 1 for unbatched input) with detached
+    right-hand sides: C_xy = cost(x, y), C_yx = cost(y, x), then with ``debias`` C_xx = cost(x, x), C_yy = cost(y, y).
+    C_yx need not be C_xy^T.  Every update of the loop is a row softmin of one of these matrices, and all those of one
+    iteration are ONE ``ops.dense_softmin_rows_raw`` call (1 + k launches for k softmins).  The last update carries the
+    gradient to the matrices, and through ``cost`` to x and y; a and b get theirs through the value formula.
+    Returns the (B,) values (a scalar for unbatched input) or the potentials (1, N) / (1, M), (B, N) / (B, M)."""
+    batched = x.dim() == 3
+    if not batched:
+        a, x, b, y = a.unsqueeze(0), x.unsqueeze(0), b.unsqueeze(0), y.unsqueeze(0)
+    B, N, _ = x.shape
+    M = y.shape[1]
+    xd, yd = x.detach(), y.detach()
+    mats = [_cost_matrix(cost, x, yd, "C_xy", N, M, x), _cost_matrix(cost, y, xd, "C_yx", M, N, x)]
+    if debias:
+        mats += [_cost_matrix(cost, x, xd, "C_xx", N, N, x), _cost_matrix(cost, y, yd, "C_yy", M, M, x)]
+    diameter, eps, eps_list, rho = scaling_parameters(x, y, p, blur, reach, diameter, scaling)
+    a_log, b_log = log_weights(a.detach()), log_weights(b.detach())
+    logs = [b_log, a_log, a_log, b_log][:len(mats)]  # the columns of C_xy are y's, of C_yx x's, ...
+    Cd = [C.detach() for C in mats]
+    with torch.no_grad():
+        eps = eps_list[0]
+        lam = damping(eps, rho)
+        pots = [out for out, _ in ops.dense_softmin_rows_raw(eps, [(C, lw, None, None) for C, lw in zip(Cd, logs)],
+                                                              beta=lam)]
+        for eps in eps_list:
+            lam = damping(eps, rho)
+            # (f_ba, g_ab, f_aa, g_bb): C_xy reads g_ab, C_yx reads f_ba, each debias matrix its own potential
+            reads = [pots[1], pots[0]] + pots[2:]
+            pots = [out for out, _ in ops.dense_softmin_rows_raw(
+                eps, [(C, lw, h, old) for C, lw, h, old in zip(Cd, logs, reads, pots)], alpha_old=0.5, beta=0.5 * lam)]
+    # final extrapolation: eps / lam are the last values of the schedule (reference: leaked loop variables)
+    reads = [pots[1], pots[0]] + pots[2:]
+    if torch.is_grad_enabled() and any(C.requires_grad for C in mats):
+        new = _LastRows.apply(eps, lam, *mats, *logs, *reads)
+    else:
+        new = [out for out, _ in ops.dense_softmin_rows_raw(eps, [(C, lw, h, None) for C, lw, h in zip(Cd, logs, reads)],
+                                                             beta=lam)]
+    f_ba, g_ab = new[0].reshape(-1), new[1].reshape(-1)
+    f_aa, g_bb = (new[2].reshape(-1), new[3].reshape(-1)) if debias else (None, None)
+    out = sinkhorn_cost_batched(eps, rho, a.reshape(-1), b.reshape(-1), f_aa, g_bb, g_ab, f_ba, B, debias=debias,
+                                potentials=potentials)
+    if potentials:
+        return out[0].view(B, N), out[1].view(B, M)
+    return out if batched else out[0]

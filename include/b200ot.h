@@ -355,6 +355,34 @@ B200OT_API int b200ot_dense_softmin_pair_bwd(const float* C, const float* log_a,
                                              const float* lse2_col, const float* go_f, const float* go_g,
                                              float* grad_C, int64_t B, int64_t N, int64_t M, void* stream);
 
+/* Row softmins only, for a group of 1 to B200OT_DENSE_ROWS_MAX matrices in ONE partials launch: the Jacobi updates of
+ * the Sinkhorn divergence on user-supplied cost matrices (softmin_tensorized, _legacy/sinkhorn_samples.py:32-71, on
+ * C_xy, C_yx, C_xx, C_yy, which need not be transposes of one another).  Per problem k:
+ *   out[b,i] <- alpha_old * out_old[b,i] + beta * (-eps log sum_j exp(log_w[b,j] + pot[b,j] / eps - C[b,i,j] / eps))
+ * C (B, n_rows, n_cols) row-major fp32, any alignment (16-byte loads when C is 16-byte aligned and n_cols % 4 == 0,
+ * the same bits otherwise); log_w, pot (B, n_cols); out_old, out, lse2 (B, n_rows).  pot null: 0; out_old null:
+ * 0; lse2 (nullable) the log2-domain log-sum-exps for b200ot_dense_softmin_rows_bwd; out may be null when lse2 is
+ * not.  out must not alias the inputs.  1 + n launches: the partials of every problem, then b200ot_softmin_finalize
+ * per problem.  EINVAL (before any launch) for null pointers, n outside [1, B200OT_DENSE_ROWS_MAX], B, n_rows or
+ * n_cols <= 0, eps <= 0; EALIGN for a scratch not 16-byte aligned; ESCRATCH below b200ot_dense_rows_scratch_bytes
+ * (a pure function of the shapes, 0 for a group these entries refuse). */
+#define B200OT_DENSE_ROWS_MAX 4
+typedef struct {
+  const float *C, *log_w, *pot, *out_old;
+  float *out, *lse2;
+  int64_t B, n_rows, n_cols;
+} b200ot_dense_rows;
+B200OT_API int64_t b200ot_dense_rows_scratch_bytes(const b200ot_dense_rows* probs, int32_t n);
+B200OT_API int b200ot_dense_softmin_rows(const b200ot_dense_rows* probs, int32_t n, float eps, float alpha_old,
+                                         float beta, void* scratch, int64_t scratch_bytes, void* stream);
+/* Gradient of <go, out~> w.r.t. C for one problem of the entry above (alpha_old = 0, beta = 1: fold a damping factor
+ * into go), pot the potential the forward read (nullable) and lse2 its output; one pass, grad_C (B,N,M) overwritten:
+ *   grad_C[b,i,j] = go[b,i] 2^(t_ij - lse2[b,i]),   t_ij = log2e (log_w[b,j] + inv_eps (pot[b,j] - C[b,i,j])).
+ * EINVAL (before any launch) for null pointers (pot excepted), B, N or M <= 0, inv_eps <= 0. */
+B200OT_API int b200ot_dense_softmin_rows_bwd(const float* C, const float* log_w, const float* pot, float inv_eps,
+                                             const float* lse2, const float* go, float* grad_C, int64_t B, int64_t N,
+                                             int64_t M, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Block-sparse softmins in the tensor-core dimensions (8 < D <= 64, p = 2 or 2 | B200OT_P_UNCLAMPED): the fine phase
  * of the two-scale Sinkhorn with user cluster labels (sinkhorn_multiscale, sinkhorn_samples.py:547-681), the

@@ -31,7 +31,7 @@ def check(name, got, ref, tol=2e-5):
 
 
 which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "wide", "blocks", "grid", "loss",
-                              "small", "apply", "apply_wide"}
+                              "small", "apply", "apply_wide", "dense"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
     # is refilled a dozen times — the pattern the N = 1e6 runs live in
@@ -294,5 +294,34 @@ if "apply_wide" in which:
         d2 = ((x[:, None, :].double() - y[None, :, :].double()) ** 2).sum(-1)
         check(f"apply_wide_d{d}_k{k}", out, torch.softmax(h.double()[None, :] - d2 / (2 * eps), dim=1) @ v.double(),
               2e-4)
+if "dense" in which:
+    # explicit cost matrices: the pair kernel (ring and scalar paths) and its backward, then a group of row softmins
+    # (one aligned, one odd n_cols, one batch view off the 16-byte grid) and the row backward
+    import math
+
+    def rows_ref(eps, C, lw, pot):
+        return -eps * torch.logsumexp((lw.double() + pot.double() / eps)[..., None, :] - C.double() / eps, dim=-1)
+
+    eps = 0.1
+    for n, m in ((130, 260), (70, 67)):
+        C = torch.rand(2, n, m, generator=g).to(DEV)
+        la, lb = torch.full((2, n), -math.log(n), device=DEV), torch.full((2, m), -math.log(m), device=DEV)
+        f, gg = torch.randn(2, n, generator=g).to(DEV), torch.randn(2, m, generator=g).to(DEV)
+        fo, go, l2r, l2c = ops.dense_softmin_pair_raw(eps, C, la, lb, f, gg, want_lse2=True)
+        check(f"dense_pair_{n}x{m}", fo, rows_ref(eps, C, lb, gg))
+        check(f"dense_pair_cols_{n}x{m}", go, rows_ref(eps, C.transpose(1, 2), la, f))
+        assert torch.isfinite(ops.dense_softmin_pair_grad(eps, C, la, lb, f, gg, l2r, l2c, torch.ones_like(f),
+                                                          torch.ones_like(gg))).all()
+    buf = torch.rand(3 * 40 * 132 + 1, generator=g).to(DEV)
+    probs = []
+    for C in (torch.rand(300, 520, generator=g).to(DEV), torch.rand(2, 90, 77, generator=g).to(DEV),
+              buf[1:].view(3, 40, 132)):
+        m = C.shape[-1]
+        probs.append((C, torch.full(C.shape[:-2] + (m,), -math.log(m), device=DEV),
+                      torch.randn(C.shape[:-2] + (m,), generator=g).to(DEV), None))
+    for k, ((C, lw, pot, _), (out, lse2)) in enumerate(zip(probs, ops.dense_softmin_rows_raw(eps, probs,
+                                                                                              want_lse2=True))):
+        check(f"dense_rows_{k}", out, rows_ref(eps, C, lw, pot))
+        assert torch.isfinite(ops.dense_softmin_rows_grad(eps, C, lw, pot, lse2, torch.ones_like(out))).all()
 torch.cuda.synchronize()
 print("sanitize_smoke: all launches completed")
