@@ -934,7 +934,8 @@ def test_grid_softmin_256_cubed_sampled_lines():
         k = -(d**2) if p == 2 else -d.abs()
         i0 = torch.randint(0, n, (8,), generator=g).to(DEV)
         i1 = torch.randint(0, n, (8,), generator=g).to(DEV)
-        t2 = torch.logsumexp(hh[:, :, None, :] + k[None, None, :, :], dim=-1)
+        # one first-axis slice at a time: the whole (n, n, n, n) fp64 broadcast is 32 GiB, and logsumexp needs two
+        t2 = torch.stack([torch.logsumexp(hh[a][:, None, :] + k[None, :, :], dim=-1) for a in range(n)])
         t1 = torch.logsumexp(t2[:, None, :, :] + k[i1][None, :, :, None], dim=2)
         t0 = torch.logsumexp(t1[None, :, :, :] + k[i0][:, :, None, None], dim=1)
         want = -eps * t0

@@ -24,7 +24,7 @@ stale max and the rebase path runs.
 
 Bars are those the dense CUDA-core operators meet in test_gpu_parity.py (the ranges kernels do the same arithmetic);
 the p = 1, laplacian and energy row gradients add, row by row, the fp32 rounding bound of their pair directions
-(_direction_slack), which pairs a few ulps apart reach at D = 1 in the unclamped convention.  Every check records its error-to-bar ratio; the largest per section is printed when the module ends.
+(fp64_refs.direction_slack), which pairs a few ulps apart reach at D = 1 in the unclamped convention.  Every check records its error-to-bar ratio; the largest per section is printed when the module ends.
 """
 import functools
 import math
@@ -32,6 +32,7 @@ import math
 import pytest
 import torch
 
+from fp64_refs import check, conv64, mid, softmin64
 from oracle import geomloss_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -73,17 +74,7 @@ def _pv(conv):
 
 
 def _check(sec, what, got, ref, bar):
-    """|got - ref| <= bar row by row (``bar``: a number, or one per row), the largest ratio recorded for ``sec``."""
-    err = (got.detach().double().cpu() - ref.double().cpu()).abs()
-    if err.dim() > 1:
-        err = err.amax(dim=1)
-    if err.numel() == 0:
-        return
-    ratio = err / bar
-    r = ratio.max().item()
-    if r > RATIOS.get(sec, ("", -1.0))[1]:
-        RATIOS[sec] = (what, r)
-    assert r <= 1.0, f"{what}: error / bar = {r:.3g} (largest error {err.max().item():.3g})"
+    check(RATIOS, sec, what, got, ref, bar)
 
 
 def _softmin_bar(ref):
@@ -161,98 +152,8 @@ def _problem(P, variant, transposed=False):
 
 
 # ------------------------------------------------------------------------------------------------------
-# fp64 references
+# fp64 references (fp64_refs.py)
 # ------------------------------------------------------------------------------------------------------
-def _cost64(x, y, conv):
-    if conv == "p2":
-        return O.cost_matrix(x, y, 2)
-    if conv == "p1":
-        return O.cost_matrix(x, y, 1)
-    return O.keops_cost(x, y, 1)
-
-
-def _mid(x, y):
-    """ops.default_center in fp64: the middle of the joint bounding box."""
-    both = torch.cat([x, y]).double()
-    return 0.5 * (both.min(0).values + both.max(0).values)
-
-
-def _direction_slack(xb, y, center, clamped):
-    """Per pair, a bound on the error of the unit vector (x_i - y_j) / |x_i - y_j| that the p = 1, laplacian and
-    energy row gradients (rowsum.cuh, explicit differences) compute in fp32.
-
-    The kernels difference PRE-SCALED coordinates, X = s (x - c) and -Y = -s (y - c), each rounded twice (2^-24
-    relative per rounding), so the computed difference is off by up to 2^-23 (|x - c| + |y - c|) in x units, plus
-    2^-24 of itself: below 2^-22 (|x - c| + |y - c|) =: e.  The unit vector of a pair at distance d is then off by
-    up to min(2, 2 e / d).  This is no concern where the cost is smooth or the gradient vanishes — p = 2, the
-    gaussian, and the clamped conventions inside the 1e-8 clamp on |x - y|^2 — but pykeops' unclamped |x - y| keeps a
-    full-weight unit vector at any distance, and a pair a few ulps apart (D = 1: 2209 x 3889 random points in
-    clusters 0.2 wide come within 1e-7 of each other) gets a direction that rounding alone decides.  The same holds,
-    weighted by e / d, for pairs just outside the clamp.  Exactly coincident points (d = 0) give X + (-Y) = 0 exactly
-    in the kernel and a zero gradient on both sides: no slack."""
-    d = O.keops_norm2(xb, y)
-    e = 2.0 ** -22 * ((xb - center).norm(dim=1)[:, None] + (y - center).norm(dim=1)[None, :])
-    slack = torch.clamp(2.0 * e / d, max=2.0)
-    return torch.where(d > (0.999e-4 if clamped else 0.0), slack, torch.zeros_like(slack))
-
-
-def _softmin64(eps, x, y, h, pairs, conv, go=None, center=None, block=256):
-    """fp64 -eps log sum_{j: pairs[i, j]} exp(h_j - C_ij / eps) per row; with ``go`` also the row gradient of
-    <go, softmin> by autograd and, for p = 1, its rounding allowance sum_j |go_i| w_ij slack_ij (_direction_slack;
-    ``center``: the kernel's, None for none).  Rows without a kept pair: +inf and NaN, never compared."""
-    x, y, h = x.double(), y.double(), h.double()
-    N = x.shape[0]
-    c = torch.zeros(x.shape[1], dtype=torch.float64) if center is None else center.double()
-    out = torch.empty(N, dtype=torch.float64)
-    gx = torch.empty_like(x) if go is not None else None
-    allow = torch.zeros(N, dtype=torch.float64)
-    for s in range(0, N, block):
-        xb = x[s:s + block].clone().requires_grad_(go is not None)
-        with torch.set_grad_enabled(go is not None):
-            t = h[None, :] - _cost64(xb, y, conv) / eps
-            if pairs is not None:
-                t = t.masked_fill(~pairs[s:s + block], -math.inf)
-            f = -eps * torch.logsumexp(t, dim=1)
-        out[s:s + block] = f.detach()
-        if go is not None:
-            gb = go[s:s + block].double()
-            (gx[s:s + block],) = torch.autograd.grad((f * gb).sum(), xb)
-            if conv != "p2":
-                wgt = torch.softmax(t.detach(), dim=1).nan_to_num(0.0)
-                slack = _direction_slack(xb.detach(), y, c, clamped=conv == "p1")
-                allow[s:s + block] = gb.abs() * (wgt * slack).sum(1)
-    return out, gx, allow
-
-
-def _kmat64(kind, unclamped, x, y, blur):
-    return (O.keops_kernel_matrix if unclamped else O.kernel_matrix)(kind, x, y, blur)
-
-
-def _conv64(kind, unclamped, x, y, w, blur, pairs, go, center, block=256):
-    """fp64 out = (K(x, y) masked by ``pairs``) @ w, the x, y, w gradients of <go, out> by autograd, and the rounding
-    allowances of the x and y gradients of the laplacian and energy kernels: the sums over i, j of
-    |go_i w_j dk/d|x - y|| slack_ij (_direction_slack)."""
-    xr, yr, wr = (t.double().clone().requires_grad_(True) for t in (x, y, w))
-    c = center.double()
-    out = torch.empty(x.shape[0], dtype=torch.float64)
-    ax, ay = torch.zeros(x.shape[0], dtype=torch.float64), torch.zeros(y.shape[0], dtype=torch.float64)
-    for s in range(0, x.shape[0], block):
-        K = _kmat64(kind, unclamped, xr[s:s + block], yr, blur)
-        if pairs is not None:
-            K = K * pairs[s:s + block].double()
-        ob = K @ wr
-        out[s:s + block] = ob.detach()
-        gb = go[s:s + block].double()
-        (ob * gb).sum().backward()
-        if kind != "gaussian":
-            dk = K.detach().abs() / blur if kind == "laplacian" else K.detach().ne(0).double()  # |dk / d|x - y||
-            pair = gb.abs()[:, None] * dk * wr.detach().abs()[None, :]
-            pair = pair * _direction_slack(xr[s:s + block].detach(), yr.detach(), c, clamped=not unclamped)
-            ax[s:s + block] = pair.sum(1)
-            ay += pair.sum(0)
-    return out, xr.grad, yr.grad, wr.grad, ax, ay
-
-
 @functools.lru_cache(maxsize=None)
 def _ref_softmin(D, conv, eps, shifted=False, self_problem=False, grad=False):
     P = _self_problem(D) if self_problem else _clusters(D)
@@ -260,13 +161,13 @@ def _ref_softmin(D, conv, eps, shifted=False, self_problem=False, grad=False):
     if shifted:  # the fp32 translated clouds, translated back exactly in fp64
         x, y = (x + 50.0).double() - 50.0, (y + 50.0).double() - 50.0
     h = P["h_a"].double() + P["pot"].double() / eps
-    return _softmin64(eps, x, y, h, P["pairs"], conv, go=P["go"] if grad else None)
+    return softmin64(eps, x, y, h, P["pairs"], conv, go=P["go"] if grad else None)
 
 
 @functools.lru_cache(maxsize=None)
 def _ref_conv(D, kind, unclamped, blur, self_problem=False):
     P = _self_problem(D) if self_problem else _clusters(D)
-    return _conv64(kind, unclamped, P["x"], P["y"], P["w"], blur, P["pairs"], P["go"], _mid(P["x"], P["y"]))
+    return conv64(kind, unclamped, P["x"], P["y"], P["w"], blur, P["pairs"], P["go"], mid(P["x"], P["y"]))
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -399,7 +300,7 @@ def test_batched_problems_element_by_element(B, N, M, D):
     for k in range(B):
         what = f"B={B} N={N} M={M} D={D} element {k}"
         for conv in CONVS:
-            ref, gref, _ = _softmin64(eps, x[k], y[k], h[k], None, conv, go=go[k] if conv == "p2" else None)
+            ref, gref, _ = softmin64(eps, x[k], y[k], h[k], None, conv, go=go[k] if conv == "p2" else None)
             _check("D", f"{what} {conv}", got[conv][k, :, 0], ref, _softmin_bar(ref))
             if gref is not None:
                 _check("D", f"{what} row gradient", got["grad"][k], gref, _grad_bar(gref, GRAD_BAR))
@@ -466,14 +367,14 @@ def _dense_case(D, M):
 @functools.lru_cache(maxsize=None)
 def _ref_dense_softmin(D, M, conv, eps):
     P = _dense_case(D, M)
-    return _softmin64(eps, P["x"], P["y"], P["h_a"].double() + P["pot"].double() / eps, None, conv, go=P["go"],
-                      center=_mid(P["x"], P["y"]))
+    return softmin64(eps, P["x"], P["y"], P["h_a"].double() + P["pot"].double() / eps, None, conv, go=P["go"],
+                      center=mid(P["x"], P["y"]))
 
 
 @functools.lru_cache(maxsize=None)
 def _ref_dense_conv(D, M, kind, unclamped, blur):
     P = _dense_case(D, M)
-    return _conv64(kind, unclamped, P["x"], P["y"], P["w"], blur, None, P["go"], _mid(P["x"], P["y"]))
+    return conv64(kind, unclamped, P["x"], P["y"], P["w"], blur, None, P["go"], mid(P["x"], P["y"]))
 
 
 def _shard_softmin(st, eps, P, p, center, W, skip=None):
@@ -611,15 +512,15 @@ def test_one_flipped_block_misses_the_bars(D, variant):
     eps = 0.5
     out, _ = ranges.softmin_ranges_raw(eps, x, y, ha, pot, 1.0 / eps, prob, p=2)
     h = P["h_a"].double() + P["pot"].double() / eps
-    ref = _softmin64(eps, P["x"], P["y"], h, P["pairs"], "p2")[0]
-    bad = _softmin64(eps, P["x"], P["y"], h, wrong, "p2")[0]
+    ref = softmin64(eps, P["x"], P["y"], h, P["pairs"], "p2")[0]
+    bad = softmin64(eps, P["x"], P["y"], h, wrong, "p2")[0]
     bar = _softmin_bar(ref[live])
     _check("F", f"D={D} {variant} softmin, right keep", out[live.to(DEV)], ref[live], bar)
     assert (out[live.to(DEV)].double().cpu() - bad[live]).abs().max().item() >= 10 * bar
     prob_t = _problem(P, variant, transposed=True)
     conv = ranges.kernel_conv_ranges(0, x, y, w, 0.5, prob, prob_t, center=ops.default_center(x, y))
     ref = _ref_conv(D, "gaussian", False, 0.5)[0]
-    bad = _conv64("gaussian", False, P["x"], P["y"], P["w"], 0.5, wrong, P["go"], _mid(P["x"], P["y"]))[0]
+    bad = conv64("gaussian", False, P["x"], P["y"], P["w"], 0.5, wrong, P["go"], mid(P["x"], P["y"]))[0]
     bar = _conv_bar(ref[live], P["w"])
     _check("F", f"D={D} {variant} gaussian, right keep", conv[live.to(DEV)], ref[live], bar)
     assert (conv[live.to(DEV)].double().cpu() - bad[live]).abs().max().item() >= 10 * bar
