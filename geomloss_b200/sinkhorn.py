@@ -69,91 +69,91 @@ def softmin_many(sm, calls):
     return [sm(*args, **kw) for args, kw in calls]
 
 
+def potential_reads(pots):
+    """The potential each slot (f_ba, g_ab, f_aa, g_bb) reads: C_xy reads g_ab, C_yx f_ba, the debias ones their own."""
+    return [pots[1], pots[0]] + list(pots[2:])
+
+
+def descend(step, eps_list, rho, pots=None):
+    """The no-grad part of the reference's loop (sinkhorn_divergence.py:461-493) over the 2 (no debias) or 4 slots
+    (f_ba, g_ab, f_aa, g_bb): without starting ``pots``, the initialisation at ``eps_list[0]``; then one averaged
+    Jacobi step per temperature of ``eps_list``, every slot reading the OLD potentials.  ``step(eps, reads, olds,
+    alpha_old, beta)`` returns the slots' ``alpha_old * olds[k] + beta * softmin(eps, slot k, reads[k])``, ``reads``
+    and ``olds`` None at the initialisation.  The extrapolations and the last, gradient-carrying step stay with the
+    drivers: each runs its own operator there."""
+    with torch.no_grad():
+        if pots is None:
+            pots = step(eps_list[0], None, None, 0.0, damping(eps_list[0], rho))
+        for eps in eps_list:
+            pots = step(eps, potential_reads(pots), pots, 0.5, 0.5 * damping(eps, rho))
+    return pots
+
+
+def slot_calls(slots, eps, reads, olds, alpha_old, beta, **kw):
+    """The calls ``[(args, kwargs), ...]`` of one ``descend`` step of a point-cloud softmin (``ops.softmin_raw``'s
+    signature): slot k is (rows, columns, log-weights of the columns, operands after ``h_scale_b``)."""
+    n = len(slots)
+    inv = 0.0 if reads is None else 1.0 / eps
+    return [((eps, rows, cols, log_w, h, inv, *more), dict(out_old=old, alpha_old=alpha_old, beta=beta, **kw))
+            for (rows, cols, log_w, *more), h, old in zip(slots, reads or [None] * n, olds or [None] * n)]
+
+
 def sinkhorn_loop_points(a_log, b_log, x, y, eps_list, rho, *, p=2, debias=True, center=None, softmin_raw=None,
                          softmin_grad=None, problems=None):
     """Symmetric Sinkhorn iterations with eps-scaling on one pair of clouds.   sinkhorn_divergence.py:258-628
 
-    The iterations run without autograd on detached clouds.  All four updates of an iteration read the
-    OLD potentials (Jacobi), then  f <- 1/2 f + 1/2 lam softmin(...)  — one fused launch each.
+    The iterations (``descend``) run without autograd on detached clouds, each one fused launch group per update.
     The last update is not averaged, takes ``x`` / ``y`` with autograd and detached right-hand sides,
     and therefore carries the whole gradient (envelope theorem).  Returns (f_aa, g_bb, g_ab, f_ba).
 
     ``softmin_raw`` / ``softmin_grad`` default to the single-GPU kernels; the column-sharded
-    multi-GPU engine (distributed.py) injects its own pair with the same signatures.
-    ``problems`` (batched inputs): ranges-mode descriptors {"xy", "yx", "xx", "yy"} of the block-diagonal problems
+    multi-GPU engine (distributed.py) injects its own pair with the same signatures, and gets the updates of one
+    iteration at once (``softmin_many``).
+    ``problems`` (batched inputs): ranges-mode descriptors of the block-diagonal problems (f_ba, g_ab[, f_aa, g_bb])
     obtained by stacking the B batch elements along the point axis — the whole batch then runs in ONE launch group
     per softmin, like the reference's batched LazyTensor reduction (sinkhorn_samples.py:229-290).
     """
+    # the (f_ba, g_ab, f_aa, g_bb) slots: rows, columns, log-weights of the columns (, ranges problem)
+    slots = [(x, y, b_log), (y, x, a_log), (x, x, a_log), (y, y, b_log)][:4 if debias else 2]
     if problems is None:
-        sm = softmin_raw or ops.softmin_raw
-        smg = softmin_grad or ops.softmin
+        sm, smg = softmin_raw or ops.softmin_raw, softmin_grad or ops.softmin
     else:
         from . import ranges
 
-        def _prob(rows, cols):
-            key = ("x" if rows is x or rows is xd else "y") + ("x" if cols is x or cols is xd else "y")
-            # (x is y: every key reads "xx", and the four problems have the same shape)
-            return problems[key] if key in problems else problems["xy"]
+        sm, smg = ranges.softmin_ranges_raw, ranges.softmin_ranges
+        slots = [slot + (prob,) for slot, prob in zip(slots, problems)]
+    detached = [(rows.detach(), cols.detach(), *rest) for rows, cols, *rest in slots]
 
-        def sm(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
-            return ranges.softmin_ranges_raw(eps, rows, cols, h_a, h_b, h_scale_b, _prob(rows, cols), **kw)
+    def step(*args):
+        return [out for out, _ in softmin_many(sm, slot_calls(detached, *args, p=p, center=center))]
 
-        def smg(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
-            return ranges.softmin_ranges(eps, rows, cols, h_a, h_b, h_scale_b, _prob(rows, cols), **kw)
-
-    xd, yd = x.detach(), y.detach()
-    with torch.no_grad():
-        eps = eps_list[0]
-        lam = damping(eps, rho)
-        g_ab = sm(eps, yd, xd, a_log, p=p, center=center, beta=lam)[0]
-        f_ba = sm(eps, xd, yd, b_log, p=p, center=center, beta=lam)[0]
-        if debias:
-            f_aa = sm(eps, xd, xd, a_log, p=p, center=center, beta=lam)[0]
-            g_bb = sm(eps, yd, yd, b_log, p=p, center=center, beta=lam)[0]
-        for eps in eps_list:
-            lam = damping(eps, rho)
-            inv = 1.0 / eps
-            ukw = dict(p=p, center=center, alpha_old=0.5, beta=0.5 * lam)
-            calls = [((eps, xd, yd, b_log, g_ab, inv), dict(out_old=f_ba, **ukw)),
-                     ((eps, yd, xd, a_log, f_ba, inv), dict(out_old=g_ab, **ukw))]
-            if debias:
-                calls += [((eps, xd, xd, a_log, f_aa, inv), dict(out_old=f_aa, **ukw)),
-                          ((eps, yd, yd, b_log, g_bb, inv), dict(out_old=g_bb, **ukw))]
-            res = softmin_many(sm, calls)  # all four read the OLD potentials (Jacobi): independent
-            f_ba, g_ab = res[0][0], res[1][0]
-            if debias:
-                f_aa, g_bb = res[2][0], res[3][0]
+    pots = descend(step, eps_list, rho)
     # final extrapolation: eps / lam are the last values of the schedule (reference: leaked loop variables)
-    inv = 1.0 / eps
-    new_f_ba = smg(eps, x, yd, b_log, g_ab, inv, p=p, center=center, scale_out=lam)
-    new_g_ab = smg(eps, y, xd, a_log, f_ba, inv, p=p, center=center, scale_out=lam)
-    if debias:
-        new_f_aa = smg(eps, x, xd, a_log, f_aa, inv, p=p, center=center, scale_out=lam)
-        new_g_bb = smg(eps, y, yd, b_log, g_bb, inv, p=p, center=center, scale_out=lam)
-        return new_f_aa, new_g_bb, new_g_ab, new_f_ba
-    return None, None, new_g_ab, new_f_ba
-
-
-def _dot(w, f):
-    """<w, f> as an elementwise product + sum (a plain reduction kernel: no cuBLAS on the value path)."""
-    return (w * f).sum()
+    eps = eps_list[-1]
+    lam, inv = damping(eps, rho), 1.0 / eps
+    new = [smg(eps, rows, cols.detach(), log_w, h, inv, *more, p=p, center=center, scale_out=lam)
+           for (rows, cols, log_w, *more), h in zip(slots, potential_reads(pots))]
+    f_ba, g_ab, f_aa, g_bb = new + [None] * (4 - len(new))
+    return f_aa, g_bb, g_ab, f_ba
 
 
 def sinkhorn_cost(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, debias=True, potentials=False):
-    """Value of the divergence (or the dual potentials) from the four potentials, unbatched vectors.
+    """Value of the divergence (or the dual potentials) from the four potentials, reduced over the last axis: (N,)
+    vectors give a scalar, B problems as (B, n) rows give (B,) (scal(batch=True), utils.py:13-18).
     sinkhorn_divergence.py:171-250.  The unbalanced weight is (rho + eps/2) in both passes — the
-    reference's UnbalancedWeight.backward is dead code (SURVEY.md appendix A-11)."""
+    reference's UnbalancedWeight.backward is dead code (SURVEY.md appendix A-11).  Elementwise products and sums
+    (plain reduction kernels: no cuBLAS on the value path)."""
     if potentials:
         return (f_ba - f_aa, g_ab - g_bb) if debias else (f_ba, g_ab)
     if rho is None:
+        f, g = (f_ba - f_aa, g_ab - g_bb) if debias else (f_ba, g_ab)
+    else:
+        w = rho + eps / 2
         if debias:
-            return _dot(a, f_ba - f_aa) + _dot(b, g_ab - g_bb)
-        return _dot(a, f_ba) + _dot(b, g_ab)
-    w = rho + eps / 2
-    if debias:
-        return _dot(a, w * ((-f_aa / rho).exp() - (-f_ba / rho).exp())) + _dot(
-            b, w * ((-g_bb / rho).exp() - (-g_ab / rho).exp()))
-    return _dot(a, w * (1 - (-f_ba / rho).exp())) + _dot(b, w * (1 - (-g_ab / rho).exp()))
+            f, g = w * ((-f_aa / rho).exp() - (-f_ba / rho).exp()), w * ((-g_bb / rho).exp() - (-g_ab / rho).exp())
+        else:
+            f, g = w * (1 - (-f_ba / rho).exp()), w * (1 - (-g_ab / rho).exp())
+    return (a * f).sum(-1) + (b * g).sum(-1)
 
 
 def sinkhorn_points(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scaling=0.5, debias=True,
@@ -176,26 +176,6 @@ def sinkhorn_points(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scali
     return sinkhorn_cost(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, debias=debias, potentials=potentials)
 
 
-def _bsum(w, f, B):
-    return (w * f).view(B, -1).sum(1)
-
-
-def sinkhorn_cost_batched(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, B, debias=True, potentials=False):
-    """sinkhorn_cost on B problems stacked along the point axis: one value per batch element (scal(batch=True),
-    utils.py:13-18)."""
-    if potentials:
-        return (f_ba - f_aa, g_ab - g_bb) if debias else (f_ba, g_ab)
-    if rho is None:
-        if debias:
-            return _bsum(a, f_ba - f_aa, B) + _bsum(b, g_ab - g_bb, B)
-        return _bsum(a, f_ba, B) + _bsum(b, g_ab, B)
-    w = rho + eps / 2
-    if debias:
-        return _bsum(a, w * ((-f_aa / rho).exp() - (-f_ba / rho).exp()), B) + _bsum(
-            b, w * ((-g_bb / rho).exp() - (-g_ab / rho).exp()), B)
-    return _bsum(a, w * (1 - (-f_ba / rho).exp()), B) + _bsum(b, w * (1 - (-g_ab / rho).exp()), B)
-
-
 def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scaling=0.5, debias=True,
                             potentials=False, keops=False, **_ignored):
     """Batched Sinkhorn divergence a:(B,N) x:(B,N,D) b:(B,M) y:(B,M,D): every softmin of the loop is ONE launch group
@@ -210,36 +190,22 @@ def sinkhorn_points_batched(a, x, b, y, p=2, blur=0.05, reach=None, diameter=Non
     B, N, D = x.shape
     M = y.shape[1]
     diameter, eps, eps_list, rho = scaling_parameters(x, y, p, blur, reach, diameter, scaling)
-    xf, yf, af, bf = x.reshape(B * N, D), y.reshape(B * M, D), a.reshape(B * N), b.reshape(B * M)
+    xf, yf = x.reshape(B * N, D), y.reshape(B * M, D)
     center = ops.default_center(xf.detach(), yf.detach())
-    dev = x.device
     pk = (p | ops.P_UNCLAMPED) if keops else p
-    loop = dict(p=pk, debias=debias, center=center)
+    a_log, b_log = log_weights(a.detach()), log_weights(b.detach())
     batched_ops = ops.softmin_operators(D, p, batched=True)
-    if batched_ops is not None:
+    if batched_ops is not None:  # the operators take the (B, n, D) clouds and (B, n) potentials
         raw, grad = batched_ops
-
-        # the loop runs on the flattened clouds and potentials; the operators see the (B, n, D) views
-        def sm(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
-            out, lse2 = raw(eps, rows.view(B, -1, D), cols.view(B, -1, D), h_a, h_b, h_scale_b, **kw)
-            return out.view(-1), None if lse2 is None else lse2.view(-1)
-
-        def smg(eps, rows, cols, h_a, h_b=None, h_scale_b=0.0, **kw):
-            return grad(eps, rows.view(B, -1, D), cols.view(B, -1, D), h_a, h_b, h_scale_b, **kw).view(-1)
-
-        loop.update(softmin_raw=sm, softmin_grad=smg)
-    else:
-        problems = {"xy": ranges.batch_problem(B, N, M, dev), "yx": ranges.batch_problem(B, M, N, dev)}
-        if debias:
-            problems["xx"] = ranges.batch_problem(B, N, N, dev)
-            problems["yy"] = ranges.batch_problem(B, M, M, dev)
-        loop.update(problems=problems)
-    f_aa, g_bb, g_ab, f_ba = sinkhorn_loop_points(log_weights(af.detach()), log_weights(bf.detach()), xf, yf,
-                                                  eps_list, rho, **loop)
-    out = sinkhorn_cost_batched(eps, rho, af, bf, f_aa, g_bb, g_ab, f_ba, B, debias=debias, potentials=potentials)
-    if potentials:
-        return out[0].view(B, N), out[1].view(B, M)
-    return out
+        inputs = (a_log, b_log, xf.view(B, N, D), yf.view(B, M, D))
+        loop = dict(softmin_raw=raw, softmin_grad=grad)
+    else:  # the B problems stacked along the point axis: one block-diagonal ranges problem per pair of clouds
+        sizes = [(N, M), (M, N), (N, N), (M, M)][:4 if debias else 2]
+        inputs = (a_log.reshape(B * N), b_log.reshape(B * M), xf, yf)
+        loop = dict(problems=[ranges.batch_problem(B, r, c, x.device) for r, c in sizes])
+    pots = sinkhorn_loop_points(*inputs, eps_list, rho, p=pk, debias=debias, center=center, **loop)
+    f_aa, g_bb, g_ab, f_ba = (None if t is None else t.view(B, -1) for t in pots)
+    return sinkhorn_cost(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, debias=debias, potentials=potentials)
 
 
 class _LastRows(torch.autograd.Function):
@@ -308,28 +274,21 @@ def sinkhorn_cost_matrices(a, x, b, y, cost, p=2, blur=0.05, reach=None, diamete
     a_log, b_log = log_weights(a.detach()), log_weights(b.detach())
     logs = [b_log, a_log, a_log, b_log][:len(mats)]  # the columns of C_xy are y's, of C_yx x's, ...
     Cd = [C.detach() for C in mats]
-    with torch.no_grad():
-        eps = eps_list[0]
-        lam = damping(eps, rho)
-        pots = [out for out, _ in ops.dense_softmin_rows_raw(eps, [(C, lw, None, None) for C, lw in zip(Cd, logs)],
-                                                              beta=lam)]
-        for eps in eps_list:
-            lam = damping(eps, rho)
-            # (f_ba, g_ab, f_aa, g_bb): C_xy reads g_ab, C_yx reads f_ba, each debias matrix its own potential
-            reads = [pots[1], pots[0]] + pots[2:]
-            pots = [out for out, _ in ops.dense_softmin_rows_raw(
-                eps, [(C, lw, h, old) for C, lw, h, old in zip(Cd, logs, reads, pots)], alpha_old=0.5, beta=0.5 * lam)]
+
+    def step(eps, reads, olds, alpha_old, beta):
+        none = [None] * len(Cd)
+        problems = list(zip(Cd, logs, reads or none, olds or none))
+        return [out for out, _ in ops.dense_softmin_rows_raw(eps, problems, alpha_old=alpha_old, beta=beta)]
+
+    pots = descend(step, eps_list, rho)
     # final extrapolation: eps / lam are the last values of the schedule (reference: leaked loop variables)
-    reads = [pots[1], pots[0]] + pots[2:]
+    eps = eps_list[-1]
+    lam = damping(eps, rho)
+    reads = potential_reads(pots)
     if torch.is_grad_enabled() and any(C.requires_grad for C in mats):
-        new = _LastRows.apply(eps, lam, *mats, *logs, *reads)
+        new = list(_LastRows.apply(eps, lam, *mats, *logs, *reads))
     else:
-        new = [out for out, _ in ops.dense_softmin_rows_raw(eps, [(C, lw, h, None) for C, lw, h in zip(Cd, logs, reads)],
-                                                             beta=lam)]
-    f_ba, g_ab = new[0].reshape(-1), new[1].reshape(-1)
-    f_aa, g_bb = (new[2].reshape(-1), new[3].reshape(-1)) if debias else (None, None)
-    out = sinkhorn_cost_batched(eps, rho, a.reshape(-1), b.reshape(-1), f_aa, g_bb, g_ab, f_ba, B, debias=debias,
-                                potentials=potentials)
-    if potentials:
-        return out[0].view(B, N), out[1].view(B, M)
-    return out if batched else out[0]
+        new = step(eps, reads, None, 0.0, lam)
+    f_ba, g_ab, f_aa, g_bb = new + [None] * (4 - len(new))
+    out = sinkhorn_cost(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, debias=debias, potentials=potentials)
+    return out if batched or potentials else out[0]

@@ -19,7 +19,7 @@ import torch
 from torch.nn.functional import avg_pool2d, avg_pool3d, interpolate
 
 from . import ops
-from .sinkhorn import damping, epsilon_schedule
+from .sinkhorn import damping, descend, epsilon_schedule, potential_reads, sinkhorn_cost
 
 
 def _dimension(t):
@@ -105,64 +105,31 @@ def sinkhorn_divergence(a, b, p=2, blur=None, reach=None, axes=None, scaling=0.5
         print("Jumps: ", jumps)
     assert len(jumps) == len(a_s) - 1, "There's a bug in the multicale pre-processing..."
 
-    sm = softmin_grid
-    last_extrapolation = True
-    with torch.no_grad():
-        k = 0
-        eps = eps_list[0]
-        lam = damping(eps, rho)
-        a_log, b_log = a_logs[0], b_logs[0]
-        g_ab = sm(eps, p, a_log, beta=lam)
-        f_ba = sm(eps, p, b_log, beta=lam)
-        if debias:
-            f_aa = sm(eps, p, a_log, beta=lam)
-            g_bb = sm(eps, p, b_log, beta=lam)
-        for i, eps in enumerate(eps_list):
-            lam = damping(eps, rho)
-            inv = 1.0 / eps
-            ft_ba = sm(eps, p, b_log, g_ab, inv, out_old=f_ba, alpha_old=0.5, beta=0.5 * lam)
-            gt_ab = sm(eps, p, a_log, f_ba, inv, out_old=g_ab, alpha_old=0.5, beta=0.5 * lam)
-            if debias:
-                ft_aa = sm(eps, p, a_log, f_aa, inv, out_old=f_aa, alpha_old=0.5, beta=0.5 * lam)
-                gt_bb = sm(eps, p, b_log, g_bb, inv, out_old=g_bb, alpha_old=0.5, beta=0.5 * lam)
-                f_aa, g_bb = ft_aa, gt_bb
-            f_ba, g_ab = ft_ba, gt_ab
-            if i in jumps:
-                if i == len(eps_list) - 1:
-                    last_extrapolation = False  # the up-sampling below is the last step (:520-526)
-                f_ba, g_ab = upsample(f_ba), upsample(g_ab)
-                if debias:
-                    f_aa, g_bb = upsample(f_aa), upsample(g_bb)
-                k += 1
-                a_log, b_log = a_logs[k], b_logs[k]
-        if last_extrapolation:
-            inv = 1.0 / eps
-            new_f_ba = sm(eps, p, b_log, g_ab, inv, beta=lam)
-            new_g_ab = sm(eps, p, a_log, f_ba, inv, beta=lam)
-            f_ba, g_ab = new_f_ba, new_g_ab
-            if debias:
-                f_aa = sm(eps, p, a_log, f_aa, inv, beta=lam)
-                g_bb = sm(eps, p, b_log, g_bb, inv, beta=lam)
+    def level_step(k):
+        """``descend``'s step on pyramid level k, its slots (f_ba, g_ab, f_aa, g_bb) the log-weights of the columns."""
+        logs = [b_logs[k], a_logs[k], a_logs[k], b_logs[k]][:4 if debias else 2]
+        none = [None] * len(logs)
 
-    return _image_cost(eps_final, rho, a, b, f_aa if debias else None, g_bb if debias else None, g_ab, f_ba,
-                       debias, potentials)
+        def step(eps, reads, olds, alpha_old, beta):
+            inv = 0.0 if reads is None else 1.0 / eps
+            return [softmin_grid(eps, p, log_w, h, inv, out_old=old, alpha_old=alpha_old, beta=beta)
+                    for log_w, h, old in zip(logs, reads or none, olds or none)]
+        return step
 
+    # one descent per level on the temperatures up to its jump, the potentials up-sampled between levels
+    bounds = [0] + [i + 1 for i in jumps] + [len(eps_list)]
+    pots = None
+    for k in range(len(a_s)):
+        pots = descend(level_step(k), eps_list[bounds[k]:bounds[k + 1]], rho, pots)
+        if k + 1 < len(a_s):
+            pots = [upsample(t) for t in pots]
+    if len(eps_list) - 1 not in jumps:  # else the up-sampling was the last step (:520-526)
+        eps = eps_list[-1]
+        with torch.no_grad():
+            pots = level_step(len(a_s) - 1)(eps, potential_reads(pots), None, 0.0, damping(eps, rho))
 
-def _bdot(a, f):
-    n = a.shape[0]
-    return (a.reshape(n, -1) * f.reshape(n, -1)).sum(1)
-
-
-def _image_cost(eps, rho, a, b, f_aa, g_bb, g_ab, f_ba, debias, potentials):
-    """sinkhorn_cost with batch=True on grids (sinkhorn_divergence.py:171-250)."""
-    if potentials:
-        return (f_ba - f_aa, g_ab - g_bb) if debias else (f_ba, g_ab)
-    if rho is None:
-        if debias:
-            return _bdot(a, f_ba - f_aa) + _bdot(b, g_ab - g_bb)
-        return _bdot(a, f_ba) + _bdot(b, g_ab)
-    w = rho + eps / 2
-    if debias:
-        return _bdot(a, w * ((-f_aa / rho).exp() - (-f_ba / rho).exp())) + _bdot(
-            b, w * ((-g_bb / rho).exp() - (-g_ab / rho).exp()))
-    return _bdot(a, w * (1 - (-f_ba / rho).exp())) + _bdot(b, w * (1 - (-g_ab / rho).exp()))
+    B = a.shape[0]
+    f_ba, g_ab, f_aa, g_bb = [t.reshape(B, -1) for t in pots] + [None] * (4 - len(pots))
+    out = sinkhorn_cost(eps_final, rho, a.reshape(B, -1), b.reshape(B, -1), f_aa, g_bb, g_ab, f_ba, debias=debias,
+                        potentials=potentials)
+    return tuple(t.view(a.shape) for t in out) if potentials else out

@@ -15,7 +15,7 @@ import ctypes
 import torch
 
 from . import ops
-from .sinkhorn import damping, extent_diameter, scaling_parameters, sinkhorn_cost_batched
+from .sinkhorn import damping, extent_diameter, scaling_parameters, sinkhorn_cost
 
 # largest cloud served by the one-launch-per-iteration kernels; beyond, the tiled TMA kernels win
 SMALL_MAX = 6000
@@ -148,8 +148,7 @@ def sinkhorn_small(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scalin
         raise KeyError(p)
     x, y = ops._f32c(x, "x"), ops._f32c(y, "y")
     a, b = ops._f32c(a, "a"), ops._f32c(b, "b")
-    B, N, D = x.shape
-    M = y.shape[1]
+    D = x.shape[-1]
     # the batch's bounding box, in one launch: its mid-point is the origin of the kernels' coordinates (whatever the
     # diameter), its diagonal the default diameter (one over the flattened batch, as the reference measures it)
     lh = ops.cloud_extent(x.view(-1, D), y.view(-1, D))
@@ -165,14 +164,5 @@ def sinkhorn_small(a, x, b, y, p=2, blur=0.05, reach=None, diameter=None, scalin
     if not potentials:
         return _FinalValue.apply(x, y, a, b, f_ba, g_ab, f_aa, g_bb, eps, lam, pk, debias, rho, eps_final, lh)
     outs = _FinalStep.apply(x, y, ad, bd, f_ba, g_ab, f_aa, g_bb, eps, lam, pk, debias, lh)
-    if debias:
-        n_f_ba, n_g_ab, n_f_aa, n_g_bb = outs
-    else:
-        (n_f_ba, n_g_ab), n_f_aa, n_g_bb = outs, None, None
-    out = sinkhorn_cost_batched(eps_final, rho, a.reshape(-1), b.reshape(-1),
-                                None if n_f_aa is None else n_f_aa.reshape(-1),
-                                None if n_g_bb is None else n_g_bb.reshape(-1), n_g_ab.reshape(-1),
-                                n_f_ba.reshape(-1), B, debias=debias, potentials=potentials)
-    if potentials:
-        return out[0].view(B, N), out[1].view(B, M)
-    return out
+    n_f_ba, n_g_ab, n_f_aa, n_g_bb = outs if debias else outs + (None, None)
+    return sinkhorn_cost(eps_final, rho, a, b, n_f_aa, n_g_bb, n_g_ab, n_f_ba, debias=debias, potentials=True)

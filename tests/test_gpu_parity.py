@@ -305,13 +305,13 @@ def test_cloud_extent_vs_torch(shape):
 
 @pytest.mark.parametrize("rho", [None, 0.7])
 @pytest.mark.parametrize("debias", [True, False])
-def test_sinkhorn_cost_small_kernel_vs_torch(rho, debias):
+def test_sinkhorn_cost_small_kernel_vs_host_formula(rho, debias):
     """b200ot_sinkhorn_cost_small: values, d value / d potential and d value / d weight against autograd of the host
-    formula (sinkhorn.sinkhorn_cost_batched = sinkhorn_divergence.py:165-255)."""
+    formula (sinkhorn.sinkhorn_cost = sinkhorn_divergence.py:165-255)."""
     import ctypes
 
     from geomloss_b200 import _lib, ops
-    from geomloss_b200.sinkhorn import sinkhorn_cost_batched
+    from geomloss_b200.sinkhorn import sinkhorn_cost
 
     B, N, M, eps = 3, 257, 301, 0.01
     g = torch.Generator().manual_seed(3)
@@ -319,9 +319,7 @@ def test_sinkhorn_cost_small_kernel_vs_torch(rho, debias):
     b = torch.rand(B, M, generator=g).to(DEV).requires_grad_(True)
     pots = [(torch.randn(B, n, generator=g) * 0.3).to(DEV).requires_grad_(True) for n in (N, M, N, M)]
     f_ba, g_ab, f_aa, g_bb = pots
-    ref = sinkhorn_cost_batched(eps, rho, a.reshape(-1), b.reshape(-1), f_aa.reshape(-1) if debias else None,
-                                g_bb.reshape(-1) if debias else None, g_ab.reshape(-1), f_ba.reshape(-1), B,
-                                debias=debias)
+    ref = sinkhorn_cost(eps, rho, a, b, f_aa if debias else None, g_bb if debias else None, g_ab, f_ba, debias=debias)
     go = torch.tensor([1.0, -2.0, 0.5], device=DEV)
     used = [a, b, f_ba, g_ab] + ([f_aa, g_bb] if debias else [])
     grads = torch.autograd.grad(ref, used, go)
