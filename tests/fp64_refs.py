@@ -1,9 +1,9 @@
 """fp64 references of the CUDA-core reduction operators (softmin values and row gradients, kernel products and their x,
-y, w gradients), with the fp32 rounding allowances of the explicit-difference row gradients, and the error-to-bar check
-the GPU test modules share.
+y, w gradients, the separable grid softmin and its closed-form backward), with the fp32 rounding allowances of the
+explicit-difference row gradients and of the grid backward, and the error-to-bar check the GPU test modules share.
 
-Each reference runs on ``device`` (the CPU by default; "cuda:0" for the large clouds, where the CPU needs minutes) in
-row blocks of ``block`` rows, and returns its results on that device.
+Each reference runs on ``device`` (the CPU by default; "cuda:0" for the large clouds and grids, where the CPU needs
+minutes) in blocks of rows or lines, and returns its results on that device.
 """
 import math
 
@@ -144,3 +144,76 @@ def conv64(kind, unclamped, x, y, w, blur, pairs, go, center, block=256, device=
             ax[s:s + block] = pair.sum(1)
             ay += pair.sum(0)
     return out, xr.grad, yr.grad, wr.grad, ax, ay
+
+
+def grid_cost64(N, eps, p, device="cpu"):
+    """(N, N) fp64 -|x_i - x_j|^p / (p eps) on the pixel grid x = arange(N) / N: one axis of the grid softmin."""
+    x = torch.arange(N, dtype=torch.float64, device=device) / N
+    d = x[:, None] - x[None, :]
+    return -d.abs() / eps if p == 1 else -(d * d) / (2 * eps)
+
+
+def grid_softmin64(eps, p, h, dim, rows=None, device="cpu", budget=2**25):
+    """fp64 -eps * (one log-sum-exp per grid axis) of h (..., N, .., N), whose last ``dim`` axes are the grid, on the
+    pixel grid x = arange(N) / N: the last axis first, then the others, as b200ot_softmin_grid and
+    oracle.softmin_grid_dense order them.
+
+    ``rows``: per grid axis, the output indices to compute along it (None: all).  The axes are reduced in that order,
+    each for its own sampled indices only, so 8 indices per axis of an N^3 volume cost about 8 N^3 terms.  Each axis is
+    reduced in blocks of lines of about ``budget`` terms, and h is converted to fp64 one block at a time: neither an
+    (N, N, N) temporary of a 1024^2 image nor an fp64 copy of a 1024^3 volume is formed.  Returns on ``device``."""
+    N = h.shape[-1]
+    k = grid_cost64(N, eps, p, device)
+    t = h.detach().to(device)
+    for axis in reversed(range(dim)):
+        ax = t.dim() - dim + axis
+        kr = k if rows is None or rows[axis] is None else k[torch.as_tensor(rows[axis], device=device)]
+        src = t.movedim(ax, -1)
+        lines = src.reshape(-1, N)
+        out = torch.empty(lines.shape[0], kr.shape[0], dtype=torch.float64, device=device)
+        step = max(1, budget // (kr.shape[0] * N))
+        for s in range(0, lines.shape[0], step):
+            out[s:s + step] = torch.logsumexp(lines[s:s + step, None, :].double() + kr[None], dim=-1)
+        t = out.reshape(src.shape[:-1] + (kr.shape[0],)).movedim(-1, ax)
+    return -eps * t
+
+
+# Roundings of 2^-24 in a part eps exp(h - conv / eps) of the closed-form grid backward beyond its exponent: the
+# exponential, the product by eps and the accumulation into the gradient.
+GRID_BWD_ROUNDINGS = 4
+
+
+def grid_softmin_grad64(eps, p, h, go, value_bar, device="cpu"):
+    """fp64 gradient of <go, softmin_grid(eps, p, h)> w.r.t. h (h: (B, C, N, N[, N])) by autograd through
+    oracle.softmin_grid_dense, and the allowance of the closed-form backward of barycenter_images._GridSoftmin.
+
+    That backward forms the gradient as  sum over s = +1, -1 of  -s eps exp(h - conv_s / eps), with
+    conv_s = softmin_grid(eps, p, log((s go)^+) + out / eps), from two more fp32 grid softmins.  If every grid softmin
+    meets the value bar, |error| <= value_bar max(1, |value|) over its batch element: conv_s is off by up to its own
+    bar delta_s, plus the bar delta_out of ``out``, which enters its input divided by eps and so moves it by at most
+    delta_out.  The part is then off by a factor exp(+-(delta_s + delta_out) / eps), and by the fp32 rounding of its
+    exponent, 2^-23 (|h| + |conv_s| / eps) in absolute terms, and GRID_BWD_ROUNDINGS more roundings of 2^-24.  Summed
+    over the two parts, per pixel.  Returns (gradient, allowance) on ``device``."""
+    from oracle import geomloss_oracle as O
+
+    hr = h.detach().to(device, torch.float64).requires_grad_(True)
+    go = go.detach().to(device, torch.float64)
+    out = O.softmin_grid_dense(eps, p, hr)
+    (grad,) = torch.autograd.grad(out, hr, go)
+    out, hr = out.detach(), hr.detach()
+
+    def element_bar(t):
+        fin = torch.where(torch.isfinite(t), t.abs(), torch.zeros_like(t))
+        return value_bar * fin.flatten(2).amax(dim=2).clamp_min(1.0).reshape(t.shape[:2] + (1,) * (t.dim() - 2))
+
+    dim = h.dim() - 2
+    d_out = element_bar(out)
+    allow = torch.zeros_like(hr)
+    for s in (1.0, -1.0):
+        part = (s * go).clamp_min(0.0)
+        lw = torch.where(part > 0, part.log(), torch.full_like(part, -math.inf))
+        conv = grid_softmin64(eps, p, lw + out / eps, dim, device=device)
+        expo = hr - conv / eps
+        rel = torch.expm1((element_bar(conv) + d_out) / eps + 2.0**-23 * (hr.abs() + conv.abs() / eps))
+        allow += torch.where(torch.isfinite(expo), eps * expo.exp() * (rel + GRID_BWD_ROUNDINGS * 2.0**-24), 0.0)
+    return grad, allow

@@ -4,6 +4,8 @@ The fixtures in tests/golden/ were produced by tests/golden/make_golden.py, whic
 jeanfeydy/geomloss @ 00e493f from /root/reference/src.  The oracle runs the same dense torch
 arithmetic, so fp32 agreement is expected to a few ulps; tolerances are stated per test.
 """
+import math
+
 import numpy as np
 import pytest
 import torch
@@ -146,6 +148,40 @@ def test_grid_softmin_is_the_full_grid_softmin(d, n):
             ref = O.softmin_dense(eps, C[None], h.reshape(1, -1))[0]
             got = O.softmin_grid_dense(eps, p, h).reshape(-1)
             assert (got - ref).abs().max().item() < 1e-12
+
+
+def grid64_vs_oracle(device):
+    """The largest relative difference between fp64_refs.grid_softmin64 (full and sampled, small line blocks) and
+    oracle.softmin_grid_dense, at sides and grids of every dimension where the oracle's dense broadcast is cheap."""
+    from fp64_refs import grid_softmin64
+
+    g = torch.Generator().manual_seed(4)
+    worst = 0.0
+    for dim, n in ((1, 1), (1, 9), (2, 1), (2, 7), (2, 17), (3, 5), (3, 12)):
+        h = (torch.randn(2, 3, *([n] * dim), generator=g, dtype=torch.float64) * 3.0).to(device)
+        h.view(6, -1)[1, ::3] = -10000.0
+        h.view(6, -1)[2, :] = -math.inf
+        h.view(6, -1)[3, 1:] = -math.inf
+        rows = [torch.randint(0, n, (3,), generator=g) for _ in range(dim)]
+        for p in (1, 2):
+            for eps in (2.0, 0.1, (0.5 / n) ** p):
+                ref = O.softmin_grid_dense(eps, p, h)
+                sub = ref
+                for axis, r in enumerate(rows):
+                    sub = sub.index_select(2 + axis, r.to(device))
+                for got, want in ((grid_softmin64(eps, p, h, dim, device=device, budget=64), ref),
+                                  (grid_softmin64(eps, p, h, dim, rows=rows, device=device, budget=64), sub)):
+                    assert got.device == want.device and got.shape == want.shape
+                    fin = torch.isfinite(want)
+                    assert torch.equal(got[~fin], want[~fin]) and bool(torch.isfinite(got[fin]).all())
+                    err = (got[fin] - want[fin]).abs().max().item() / max(1.0, want[fin].abs().max().item())
+                    worst = max(worst, err)
+    return worst
+
+
+def test_fp64_grid_reference_is_the_grid_oracle():
+    """CPU half of the cross-check of the grid softmin's fp64 reference (test_gpu_grid.py runs it on the GPU)."""
+    assert grid64_vs_oracle("cpu") <= 1e-11
 
 
 def test_grid_pyramid_and_schedule():

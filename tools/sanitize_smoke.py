@@ -4,8 +4,9 @@
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
     B200OT_FORCE_SPLITS=1 compute-sanitizer --tool racecheck python tools/sanitize_smoke.py ring tc
 
-Shapes are the smallest that select each code path (big / small tile shapes, ranges mode, tensor-core kernels, 2-D and
-3-D grid passes with both tile widths); results are checked against torch so a silent corruption also fails."""
+Shapes are the smallest that select each code path (big / small tile shapes, ranges mode, tensor-core kernels, 2-D grid
+passes with both tile widths, 3-D grid passes with the 32-line tile); results are checked against torch so a silent
+corruption also fails."""
 import sys
 
 import torch
