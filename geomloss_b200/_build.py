@@ -13,8 +13,8 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB_PATH = os.path.join(PKG, "libb200ot.so")
-SOURCES = ["b200ot_core.cu", "b200ot_softmin.cu", "b200ot_softmin_bwd.cu", "b200ot_kernel_conv.cu", "b200ot_grid.cu",
-           "b200ot_small.cu", "b200ot_wide.cu", "b200ot_plan_apply.cu", "b200ot_dense.cu"]
+SOURCES = ["b200ot_core.cu", "b200ot_softmin.cu", "b200ot_softmin_bwd.cu", "b200ot_kernel_conv.cu", "b200ot_tc.cu",
+           "b200ot_grid.cu", "b200ot_small.cu", "b200ot_wide.cu", "b200ot_plan_apply.cu", "b200ot_dense.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",

@@ -3,64 +3,20 @@
 //   gaussian  k = exp(-|x/s - y/s|^2 / 2)                    (kernel_samples.py:62-68)
 //   laplacian k = exp(-sqrt(max(|x/s - y/s|^2, 1e-8)))       (kernel_samples.py:71-77, utils.py:56-61)
 //   energy    k = -sqrt(max(|x - y|^2, 1e-8))                (kernel_samples.py:80-82)
-// evaluated on the fly (never as an N x M matrix) by rowsum_partial_kernel.
+// evaluated on the fly (never as an N x M matrix) by rowsum_partial_kernel, or on the tensor cores (b200ot_tc.cu) above
+// D = 8 and wherever tc_routed sends the gaussian.
 #include "b200ot.h"
+#include "conv_kind.cuh"
 #include "host_util.cuh"
 #include "pack.cuh"
 #include "plan.cuh"
 #include "rowsum.cuh"
 #include "rowsum_launch.cuh"
-#include "tcapply.cuh"
-#include "tcbwd.cuh"
-#include "tcconv.cuh"
-#include "tcwide.cuh"
-
-#include <stdio.h>
-#include <stdlib.h>
+#include "tcconv.cuh"  // tc_energy_coord_scale, which the finalize kernels undo for the tensor-core energy kernel
 
 #include <algorithm>
-#include <vector>
 
 namespace b200ot {
-
-struct ConvScales {
-  float scale;   // coordinate scale
-  float clampq;  // clamp on the scaled squared distance
-  int direct;
-  int extra;
-};
-
-// `kind` may carry B200OT_KERNEL_UNCLAMPED (laplacian / energy with pykeops' unclamped sqrt)
-static int kind_base(int kind) { return kind & 0xff; }
-static bool valid_kind(int kind) {
-  return kind_base(kind) >= 0 && kind_base(kind) <= 2 && (kind & ~(0xff | B200OT_KERNEL_UNCLAMPED)) == 0;
-}
-
-// blur is the length scale of the gaussian and laplacian kernels; the energy kernel has none
-static bool blur_ok(int kind, float blur) { return kind_base(kind) == B200OT_KERNEL_ENERGY || blur > 0.f; }
-
-static ConvScales conv_scales(int kind_flags, float blur) {
-  ConvScales c;
-  const int kind = kind_base(kind_flags);
-  const float clamp = cost_clamp(kind_flags);  // B200OT_KERNEL_UNCLAMPED == B200OT_P_UNCLAMPED
-  if (kind == B200OT_KERNEL_GAUSSIAN) {
-    c.scale = sqrtf(kLog2e) / blur;  // 2^(-|X-Y|^2/2) = exp(-|x-y|^2 / (2 blur^2))
-    c.clampq = 0.f;
-    c.direct = 0;
-    c.extra = 2;
-  } else if (kind == B200OT_KERNEL_LAPLACIAN) {
-    c.scale = kLog2e / blur;  // 2^(-|X-Y|) = exp(-|x-y| / blur)
-    c.clampq = kLog2e * kLog2e * clamp;
-    c.direct = 1;
-    c.extra = 1;
-  } else {
-    c.scale = 1.f;
-    c.clampq = clamp;
-    c.direct = 1;
-    c.extra = 1;
-  }
-  return c;
-}
 
 // coord_absmax (tensor-core energy kernel): the sums are in coordinates scaled by tc_energy_coord_scale, undone here
 __global__ void conv_fwd_finalize_kernel(const float* __restrict__ part, int n_split, float sign,
@@ -116,31 +72,21 @@ __global__ void conv_bwd_finalize_kernel(const float* __restrict__ part, int n_s
   }
 }
 
-// max_j |w_j| into *out (zero-initialised by the caller); bit order of non-negative floats = integer order.
-// gridDim.y > 1: one maximum per batch element of n weights, out[blockIdx.y]
-__global__ void absmax_kernel(const float* __restrict__ w, int64_t n, float* __restrict__ out) {
-  w += (int64_t)blockIdx.y * n;
-  out += blockIdx.y;
-  float m = 0.f;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    m = fmaxf(m, fabsf(w[i]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0 && m > 0.f && !(m != m)) atomicMax(reinterpret_cast<unsigned int*>(out), __float_as_uint(m));
+int conv_fwd_finalize(const float* part, int n_part, int kind, float* out, int64_t N, const float* coord_absmax,
+                      cudaStream_t st) {
+  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
+      part, n_part, kind_base(kind) == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, N, coord_absmax);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
 }
 
-// max_k |pts[i, k] - center[k]| over the rows of a (na x D) and b (nb x D) into *out (zero-initialised by the caller)
-__global__ void coord_absmax_kernel(const float* __restrict__ a, int64_t na, const float* __restrict__ b, int64_t nb,
-                                    int D, const float* __restrict__ center, float* __restrict__ out) {
-  float m = 0.f;
-  const int64_t ta = na * D, tot = ta + nb * D;
-  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < tot; e += (int64_t)gridDim.x * blockDim.x) {
-    const float v = e < ta ? a[e] : b[e - ta];
-    m = fmaxf(m, fabsf(v - (center ? center[e % D] : 0.f)));
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0 && m > 0.f && !(m != m)) atomicMax(reinterpret_cast<unsigned int*>(out), __float_as_uint(m));
+int conv_bwd_finalize(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
+                      float* grad_x, int64_t N, int D, int kind, float scale, float coef, const float* w_absmax,
+                      float* value_out, const float* coord_absmax, int64_t n_per, cudaStream_t st) {
+  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
+      part, n_part, x, center, grad_out, grad_x, N, D, kind, scale, coef, w_absmax, value_out, coord_absmax, n_per);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
 }
 
 static int conv_pack(const float* y, const float* w, const float* center, int64_t M, int D, const ConvScales& cs,
@@ -177,505 +123,6 @@ static float conv_bwd_coef(int kind_flags, const ConvScales& cs, float blur) {
   return -1.0f;
 }
 
-
-// ---------------------------------------------------------------------------------------------------
-// tensor-core path (gaussian, and laplacian / energy for 8 < D <= 64): see tcconv.cuh
-// ---------------------------------------------------------------------------------------------------
-// A launch group: `ctas` x n_split x slices CTAs over a_tiles row images and b_tiles column images, then the partials
-// and a misc block in the scratch
-struct TcPlan {
-  int kp, nstage, n_split, tiles_per_split, slices;
-  int rtpe, ctpe;  // row / column tiles per batch element (0 for a block-sparse problem)
-  int64_t a_tiles, b_tiles, ctas, smem;
-  int64_t off_b, off_part, off_misc, total;
-};
-
-// Which path serves an operator.  Above B200OT_MAX_D the tensor-core kernels are the only ones.  At or below it both
-// exist: the CUDA-core kernels are FMA-pipe bound from D = 5 up while the tensor-core kernels run the zero-padded
-// dk = 16 problem at the same rate whatever D.  Measured on an H100 80GB HBM3 (SXM, 400 W power limit) at N = M = 4e5
-// (tools/ab_tc_route.py part A; CUDA-core -> tensor-core, 1e12 pairs/s):
-//   softmin forward   D = 5: 2.38 -> 1.96   D = 6: 2.02 -> 1.95   D = 7: 1.85 -> 1.94   D = 8: 1.54 -> 1.87
-//   gaussian forward  D = 4: 2.42 -> 2.39   D = 5: 1.77 -> 2.42   D = 6: 1.60 -> 2.45   D = 8: 1.31 -> 2.37
-//   row gradients     D = 6: 1.33 / 1.22 -> 1.69 / 1.52 (softmin / gaussian); D = 8: 1.08 / 0.97 -> 1.63 / 1.49
-// (at N = M = 1e5 and 3e4 the softmin forward already breaks even at D = 6, the others switch where they do at 4e5).  The
-// forward operators switch at D = 7 (softmin) and D = 5 (gaussian).  The row gradients stay on the CUDA cores for every
-// D <= 8 although the tensor cores are faster from D = 6: the fp16 image of P that GEMM 2 consumes costs accuracy at
-// small blur in low dimension (relative difference between the two paths' gradients at eps = 1e-4 / blur = .05 in the
-// same run: up to 3e-3 at D = 4, 4e-4 at D = 6..8, against ~1e-5 for the forward operators).  Problems below 8e8 pairs
-// keep the CUDA-core kernels.  $B200OT_TC_MIN_D ("d" or "softmin_fwd,softmin_bwd,conv_fwd,conv_bwd")
-// and $B200OT_TC_MIN_PAIRS override the defaults for A/B timing and for the parity tests of both routes — read on every
-// call, never set by the bench.
-static const int kTcMinDimDefault[4] = {7, 9, 5, 9};
-static const double kTcMinPairsDefault = 8.0e8;
-
-bool tc_routed(int op, int D, int64_t N, int64_t M) {
-  if (!tc_capable_dim(D)) return false;
-  if (D > B200OT_MAX_D) return true;
-  int min_dim[4] = {kTcMinDimDefault[0], kTcMinDimDefault[1], kTcMinDimDefault[2], kTcMinDimDefault[3]};
-  double min_pairs = kTcMinPairsDefault;
-  if (const char* e = getenv("B200OT_TC_MIN_D")) {
-    int v[4];
-    const int n = sscanf(e, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]);
-    if (n == 1) {
-      for (int k = 0; k < 4; ++k) min_dim[k] = v[0];
-    } else if (n == 4) {
-      for (int k = 0; k < 4; ++k) min_dim[k] = v[k];
-    }
-  }
-  if (const char* e = getenv("B200OT_TC_MIN_PAIRS")) {
-    const double v = atof(e);
-    if (v >= 0.0) min_pairs = v;
-  }
-  return D >= min_dim[op] && (double)N * (double)M >= min_pairs;
-}
-
-bool tc_any_routed(int D, int64_t N, int64_t M) {
-  for (int op = 0; op < 4; ++op)
-    if (tc_routed(op, D, N, M)) return true;
-  return false;
-}
-
-// The plan of a launch group: `ctas` row CTAs, each reading up to `tiles` (>= 1) column tiles.  The split count is
-// chosen for the whole grid and cuts those tiles.  Behind the images: the partials of `rows` rows ((m, s) pairs forward, D+1
-// sums per row backward, D+2 for the p = 1 softmin: `head` sums ahead of the D), then a misc block of misc_bytes.
-// Above D = 64 the K-slab ring of tcwide.cuh, whose row gradients run `slices` CTAs per row tile and split.
-static TcPlan make_tc_plan(int D, bool bwd, int64_t a_tiles, int64_t b_tiles, int64_t ctas, int64_t tiles, int64_t rows,
-                           int64_t misc_bytes, int head = 1, int slices = 1) {
-  TcPlan p;
-  p.kp = tc_kp(D);
-  p.slices = slices;
-  p.rtpe = p.ctpe = 0;
-  p.a_tiles = a_tiles;
-  p.b_tiles = b_tiles;
-  p.ctas = ctas;
-  const int64_t b_bytes = tc_b_img_bytes(p.kp, kTcBN);
-  if (D > 64) {
-    // row tail, column tails and slab ring (tcwide.cuh): as many stages as fit, whatever D
-    int ns = kTcMaxStage;
-    while (ns > 0 && tc_wide_smem(ns) > 227 * 1024) --ns;
-    p.nstage = ns;
-    p.smem = tc_wide_smem(ns);
-  } else {
-    const int64_t bar_bytes = 256;  // mbarriers behind the column ring
-    // the CTA's row image stays in shared memory; the rest of the 227 KB a block may use holds the column ring
-    const int64_t avail = 227 * 1024 - bar_bytes - tc_a_span(p.kp);
-    int64_t ns = avail / b_bytes;
-    p.nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
-    p.smem = tc_a_span(p.kp) + p.nstage * b_bytes + bar_bytes;
-  }
-  int64_t want = ceil_div64((int64_t)num_sms() * 4, ctas * slices);
-  const int forced = forced_splits();  // test hook (plan.cuh)
-  if (forced > 0) want = forced;
-  if (want < 1) want = 1;
-  if (want > 64) want = 64;
-  if (want > tiles) want = tiles;
-  p.tiles_per_split = (int)ceil_div64(tiles, want);
-  p.n_split = (int)ceil_div64(tiles, p.tiles_per_split);
-  p.off_b = round_up64(a_tiles * tc_a_img_bytes(p.kp), 256);
-  p.off_part = p.off_b + round_up64(b_tiles * b_bytes, 256);
-  p.off_misc = p.off_part + round_up64((int64_t)p.n_split * (bwd ? rows * (D + head) : kTcParts * rows * 2) * 4, 256);
-  p.total = p.off_misc + round_up64(misc_bytes, 256);
-  return p;
-}
-
-// B problems of N rows x M columns side by side (B = 1: one problem), each element padded to whole tiles on its own
-// (tc_pack_kernel).  The splits cut each element's ctpe column tiles, so a CTA never reads another element's columns.
-// Above D = 64 the row gradients run one slice per K slab.  Misc block: [0] the energy coordinate maximum, [1 + b]
-// max|w| of element b.
-static TcPlan make_tc_plan(int64_t N, int64_t M, int D, bool bwd, int64_t B = 1, int head = 1) {
-  const int rtpe = (int)ceil_div64(N, kTcM), ctpe = (int)ceil_div64(M, kTcBN);
-  TcPlan p = make_tc_plan(D, bwd, B * rtpe, B * ctpe, B * rtpe, ctpe, B * N, (B + 1) * 4, head,
-                          bwd && D > 64 ? tc_wide_slabs(D) : 1);
-  p.rtpe = rtpe;
-  p.ctpe = ctpe;
-  return p;
-}
-
-int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B, int head) {
-  // forward and row-gradient launches split the columns differently: size for the larger of the two
-  return std::max(make_tc_plan(N, M, D, false, B).total, make_tc_plan(N, M, D, true, B, head).total);
-}
-
-// The plan of one block-sparse problem: a CTA per segment, images of n_row_slots / n_col_slots points, segments cut
-// into splits from the longest one.  Misc block: the segment descriptors, then the pieces.
-static int64_t tc_blocks_seg_bytes(int64_t n_seg) { return round_up64(n_seg * 16, 256); }
-static TcPlan make_tc_blocks_plan(int64_t N, int D, bool bwd, const TcBlocks& b) {
-  return make_tc_plan(D, bwd, b.n_row_slots / kTcM, b.n_col_slots / kTcBN, b.n_seg, std::max(b.max_tiles, 1), N,
-                      tc_blocks_seg_bytes(b.n_seg) + std::max<int64_t>(b.n_pieces, 1) * 8);
-}
-
-int64_t tc_blocks_scratch_bytes(int64_t N, int D, const TcBlocks& b) {
-  return std::max(make_tc_blocks_plan(N, D, false, b).total, make_tc_blocks_plan(N, D, true, b).total);
-}
-
-// What the images of a launch group hold (tc_pack_kernel): the row cloud x and the column cloud y, centred at `center`
-// and multiplied by `scale`; B elements of N rows / M columns, or N / M block-sparse slots gathered through row_src /
-// col_src.  Besides the coordinates: the column weights w, the softmin's column terms h_a + h_scale_b h_b and the
-// softmin row gradient's row term lse2.  l1_c = log2e / eps > 0: the p = 1 softmin's layout (tc_pack_kernel's l1).
-struct TcOperands {
-  const float *x, *y, *center;
-  float scale;
-  int64_t N, M;
-  int D;
-  int64_t B = 1;
-  const float *w = nullptr, *h_a = nullptr, *h_b = nullptr;
-  float h_scale_b = 0.f;
-  const float* lse2 = nullptr;
-  const int *row_src = nullptr, *col_src = nullptr;
-  float l1_c = 0.f;
-};
-
-// Packs both images of plan p.  Asked for through a non-null out pointer, it first computes into the misc block:
-//   * w_absmax (row gradients): P = w_j e_ij feeds an fp16 GEMM, so the weights are normalised to max|w| = kTcPScale
-//     (undone by the finalize kernel), one maximum per batch element, so that a heavy element cannot push a light
-//     one's P into fp16's subnormal range;
-//   * coord_absmax (energy): the largest centred coordinate of both clouds (of every batch element: one scale for the
-//     whole batch, a power of two that the finalize undoes exactly), from which every kernel of the pass derives the
-//     same power-of-two coordinate scale (tc_energy_coord_scale).
-static int tc_pack(const TcPlan& p, unsigned char* base, const TcOperands& o, cudaStream_t st,
-                   const float** w_absmax = nullptr, const float** coord_absmax = nullptr) {
-  float* misc = reinterpret_cast<float*>(base + p.off_misc);
-  const float* cmax = nullptr;
-  if (coord_absmax) {
-    B200OT_CUDA_TRY(cudaMemsetAsync(misc, 0, sizeof(float), st));
-    const int64_t n = o.B * o.N, m = o.B * o.M;
-    coord_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64((n + m) * o.D, 256), 1024), 256, 0, st>>>(
-        o.x, n, o.y, m, o.D, o.center, misc);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    cmax = *coord_absmax = misc;
-  }
-  const float* wmax = nullptr;
-  if (w_absmax) {
-    if (o.w != nullptr) {
-      B200OT_CUDA_TRY(cudaMemsetAsync(misc + 1, 0, o.B * sizeof(float), st));
-      const dim3 g((unsigned)std::min<int64_t>(ceil_div64(o.M, 256), 1024), (unsigned)o.B);
-      absmax_kernel<<<g, 256, 0, st>>>(o.w, o.M, misc + 1);
-      B200OT_CUDA_TRY(cudaGetLastError());
-      wmax = misc + 1;
-    }
-    *w_absmax = wmax;
-  }
-  const int threads = 128;
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.a_tiles * kTcM, threads), threads, 0, st>>>(
-      o.x, nullptr, nullptr, nullptr, 0.f, o.l1_c, o.center, o.scale, o.N, o.D, p.kp, kTcM, 0, base, o.lse2, nullptr, cmax,
-      o.B, o.row_src, o.l1_c > 0.f);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  tc_pack_kernel<<<(unsigned)ceil_div64(p.b_tiles * kTcBN, threads), threads, 0, st>>>(
-      o.y, o.w, o.h_a, o.h_b, o.h_scale_b, kLog2e, o.center, o.scale, o.M, o.D, p.kp, kTcBN, 1, base + p.off_b, nullptr,
-      wmax, cmax, o.B, o.col_src, o.l1_c > 0.f);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
-// tc_reduce_kernel<FWD> (forward) or tc_bwd_kernel<BWD> at the padded dimension of D (row gradients)
-template <int FWD, int BWD, bool BATCH, bool BLOCKS = false>
-static TcKernel tc_kernel_of(bool bwd, int D) {
-  if (!bwd) return tc_reduce_kernel<FWD, BATCH, BLOCKS>;
-  switch (tc_dk(D)) {
-    case 16: return tc_bwd_kernel<BWD, 16, BATCH, BLOCKS>;
-    case 32: return tc_bwd_kernel<BWD, 32, BATCH, BLOCKS>;
-    case 48: return tc_bwd_kernel<BWD, 48, BATCH, BLOCKS>;
-    default: return tc_bwd_kernel<BWD, 64, BATCH, BLOCKS>;
-  }
-}
-
-// The kernel of `mode` (the MODE of tc_reduce_kernel forward, of tc_bwd_kernel for the row gradients: 0 / 2 gaussian
-// conv, 1 / 3 softmin p = 2, 4 laplacian, 5 energy, 6 / 7 softmin p = 1) for D and the layout; null for a pair that
-// has none.  Above D = 64 the K-slab kernels, whatever the layout.
-static TcKernel tc_kernel(int mode, bool bwd, int D, TcLayout layout) {
-  if (D > 64) return tc_wide_kernel(mode, bwd);
-  const bool one = layout == TcLayout::kOne, batch = layout == TcLayout::kBatch;
-  switch (mode) {
-    case 0:
-    case 2: return one ? tc_kernel_of<0, 2, false>(bwd, D) : batch ? tc_kernel_of<0, 2, true>(bwd, D) : nullptr;
-    case 1:
-    case 3:
-      return one     ? tc_kernel_of<1, 3, false>(bwd, D)
-             : batch ? tc_kernel_of<1, 3, true>(bwd, D)
-                     : tc_kernel_of<1, 3, false, true>(bwd, D);
-    case 4: return one ? tc_kernel_of<4, 4, false>(bwd, D) : batch ? tc_kernel_of<4, 4, true>(bwd, D) : nullptr;
-    case 5: return one ? tc_kernel_of<5, 5, false>(bwd, D) : batch ? tc_kernel_of<5, 5, true>(bwd, D) : nullptr;
-    default: return batch ? tc_kernel_of<6, 7, true>(bwd, D) : nullptr;
-  }
-}
-
-// One tensor-core pass of `mode` (tc_kernel) over B elements of o.N rows / o.M columns, or over the block-sparse
-// problem `blocks` of o.N rows: plan, images, kernel and launch.  The row gradients normalise the weights (when the
-// operator has any) and the energy's coordinates (modes 5, 6, 7) take a power-of-two scale from their maximum
-// (tc_pack); the finalize undoes both.
-static int tc_pass(int mode, bool bwd, TcLayout layout, TcOperands o, float clampq, const TcBlocks* blocks,
-                   void* scratch, cudaStream_t st, TcPass* r) {
-  const TcPlan p = blocks ? make_tc_blocks_plan(o.N, o.D, bwd, *blocks)
-                          : make_tc_plan(o.N, o.M, o.D, bwd, o.B, mode == 7 ? 2 : 1);
-  const TcKernel kern = tc_kernel(mode, bwd, o.D, layout);
-  if (p.nstage < 1 || kern == nullptr) return B200OT_EINVAL;
-  // K_xx / K_yy and the p = 1 xx / yy: the diagonal exponent is exact (tcconv.cuh)
-  const int self_mode = (mode != 1 && mode != 3 && o.x == o.y && o.N == o.M) ? 1 : 0;
-  const int64_t rows = o.B * o.N, n_local = blocks ? 0 : o.N;
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  const int4* seg = nullptr;
-  const int2* pieces = nullptr;
-  if (blocks) {
-    // the host descriptors travel in the misc block
-    int4* d_seg = reinterpret_cast<int4*>(base + p.off_misc);
-    int2* d_pieces = reinterpret_cast<int2*>(base + p.off_misc + tc_blocks_seg_bytes(blocks->n_seg));
-    B200OT_CUDA_TRY(cudaMemcpyAsync(d_seg, blocks->seg, blocks->n_seg * 16, cudaMemcpyHostToDevice, st));
-    if (blocks->n_pieces > 0)
-      B200OT_CUDA_TRY(cudaMemcpyAsync(d_pieces, blocks->pieces, blocks->n_pieces * 8, cudaMemcpyHostToDevice, st));
-    seg = d_seg;
-    pieces = d_pieces;
-    o.N = blocks->n_row_slots;
-    o.M = blocks->n_col_slots;
-    o.row_src = blocks->row_src;
-    o.col_src = blocks->col_src;
-  }
-  *r = TcPass{};
-  int rc = tc_pack(p, base, o, st, bwd ? &r->w_absmax : nullptr, mode >= 5 ? &r->coord_absmax : nullptr);
-  if (rc) return rc;
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-  const dim3 grid((unsigned)p.ctas, (unsigned)p.n_split, (unsigned)p.slices);
-  kern<<<grid, kTcThreads, (size_t)p.smem, st>>>(base, base + p.off_b, reinterpret_cast<float*>(base + p.off_part),
-                                                 rows, p.kp, p.ctpe, p.tiles_per_split, p.nstage, o.D, self_mode,
-                                                 clampq, r->coord_absmax, p.rtpe, n_local, seg, pieces, o.row_src);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  r->part = reinterpret_cast<float*>(base + p.off_part);
-  // row gradients: G of a CTA is complete over its column split (both column halves feed one GEMM)
-  r->n_part = bwd ? p.n_split : p.n_split * kTcParts;
-  return B200OT_OK;
-}
-
-// The softmin, p = 2 (MODE 1 / 3) or p = 1 (MODE 6 / 7, on the energy's coordinates with the clamp of p)
-int softmin_pass_tc(bool bwd, TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, void* scratch,
-                    cudaStream_t st, TcPass* r) {
-  const bool l1 = p_exponent(s.p) == 1;
-  TcOperands o{s.x, s.y, s.center, l1 ? 1.f : softmin_coord_scale(2, s.eps), s.N, s.M, s.D, s.B, nullptr, s.h_a, s.h_b,
-               s.h_scale_b, s.lse2};
-  if (l1) o.l1_c = kLog2e / s.eps;
-  return tc_pass(l1 ? (bwd ? 7 : 6) : (bwd ? 3 : 1), bwd, layout, o, l1 ? cost_clamp(s.p) : 0.f, blocks, scratch, st,
-                 r);
-}
-
-int softmin_fwd_tc(TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, const float* out_old, float alpha_old,
-                   float beta, float* out, float* lse2_out, void* scratch, void* stream) {
-  TcPass r;
-  const int rc = softmin_pass_tc(false, layout, s, blocks, scratch, (cudaStream_t)stream, &r);
-  if (rc) return rc;
-  return b200ot_softmin_finalize(r.part, r.n_part, out_old, alpha_old, beta, out, lse2_out, s.B * s.N, s.eps, stream);
-}
-
-// p = 1 on the tensor cores: part (n_split, N, D+2) with [0] = sum P, [1] = sum Q, [2+k] = sum Q Y_k (tcbwd.cuh, MODE 7)
-// -> grad_x = go (X_i sum Q - sum Q Y) / sum P, X = scale (x - center) with the pass's coordinate scale
-__global__ void softmin_l1_bwd_finalize_kernel(const float* __restrict__ part, int n_split,
-                                               const float* __restrict__ x, const float* __restrict__ center,
-                                               const float* __restrict__ grad_out, float* __restrict__ grad_x,
-                                               int64_t N, int D, const float* __restrict__ coord_absmax) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  const int na = D + 2;
-  const float scale = tc_energy_coord_scale(*coord_absmax);
-  float sp = 0.f, sq = 0.f;
-  for (int s = 0; s < n_split; ++s) {
-    sp += part[((int64_t)s * N + i) * na];
-    sq += part[((int64_t)s * N + i) * na + 1];
-  }
-  const float go = sp > 0.f ? grad_out[i] / sp : 0.f;
-  for (int k = 0; k < D; ++k) {
-    float a = 0.f;
-    for (int s = 0; s < n_split; ++s) a += part[((int64_t)s * N + i) * na + 2 + k];
-    const float X = scale * (x[i * D + k] - (center ? center[k] : 0.f));
-    grad_x[i * D + k] = go * (X * sq - a);
-  }
-}
-
-int softmin_bwd_x_tc(TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, const float* grad_out, float* grad_x,
-                     void* scratch, cudaStream_t st) {
-  TcPass r;
-  const int rc = softmin_pass_tc(true, layout, s, blocks, scratch, st, &r);
-  if (rc) return rc;
-  // P carries kTcPScale (p = 2) or 2^k_i (p = 1), which cancel: both finalizes divide by each row's sum of P
-  const int64_t rows = s.B * s.N;
-  if (p_exponent(s.p) == 2)
-    return softmin_bwd_finalize_tc(r.part, r.n_part, s.x, s.center, grad_out, grad_x, rows, s.D, s.eps, st);
-  softmin_l1_bwd_finalize_kernel<<<(unsigned)ceil_div64(rows, 256), 256, 0, st>>>(r.part, r.n_part, s.x, s.center,
-                                                                                  grad_out, grad_x, rows, s.D,
-                                                                                  r.coord_absmax);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
-// The kernel convolution of B elements of N rows / M columns on the tensor cores: out (forward) or grad_x (bwd) and,
-// with value_out, the forward values from the same pass (gaussian only).  Every row-gradient kernel leaves the
-// gaussian's sums: grad = coef (sum_j P Y_j - X_i sum_j P) with coef = 1 / (scale blur^2) for the gaussian; the
-// laplacian and energy P = w k'(d) / d carries 2^-kTcNormPLog2 (tcbwd.cuh), so coef = 2^kTcNormPLog2 / blur (laplacian,
-// X = x log2e / blur) or 2^kTcNormPLog2 (energy).  Arguments already validated.
-static int conv_tc(bool bwd, TcLayout layout, int kind, const float* x, const float* y, const float* w,
-                   const float* center, const float* grad_out, float* res, float* value_out, int64_t B, int64_t N,
-                   int64_t M, int D, float blur, void* scratch, cudaStream_t st) {
-  const int kb = kind_base(kind);
-  // gaussian: 2^(-|X-Y|^2/2) with X = x sqrt(log2e) / blur; laplacian / energy: conv_scales' coordinates and clamp
-  const ConvScales cs = conv_scales(kind, blur);
-  const int mode = kb == B200OT_KERNEL_GAUSSIAN ? (bwd ? 2 : 0) : (kb == B200OT_KERNEL_LAPLACIAN ? 4 : 5);
-  TcPass r;
-  const int rc = tc_pass(mode, bwd, layout, {x, y, center, cs.scale, N, M, D, B, w}, cs.clampq, nullptr, scratch, st, &r);
-  if (rc) return rc;
-  const unsigned blocks = (unsigned)ceil_div64(B * N, 256);
-  if (!bwd) {
-    conv_fwd_finalize_kernel<<<blocks, 256, 0, st>>>(r.part, r.n_part, kb == B200OT_KERNEL_ENERGY ? -1.f : 1.f, res,
-                                                    B * N, r.coord_absmax);
-  } else {
-    const float coef = kb == B200OT_KERNEL_GAUSSIAN
-                           ? 1.0f / (cs.scale * blur * blur)
-                           : (float)(1 << kTcNormPLog2) * (kb == B200OT_KERNEL_LAPLACIAN ? 1.0f / blur : 1.0f);
-    // n_per = N: the finalize undoes each element's weight scale
-    conv_bwd_finalize_kernel<<<blocks, 256, 0, st>>>(r.part, r.n_part, x, center, grad_out, res, B * N, D,
-                                                    B200OT_KERNEL_GAUSSIAN, cs.scale, coef, r.w_absmax, value_out,
-                                                    r.coord_absmax, N);
-  }
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
-// The plan applied to a value matrix (tcapply.cuh): the images and splits of the softmin row gradient's plan, one CTA
-// per row tile and split whatever D (no D slices above 64: GEMM 2 reads the value image, not a column slab), and
-// behind the images the partials (n_split, N, 1 + min(K, 64)), one slab's value image and the K column maxima of V.
-// V wider than 64 columns runs in slabs of 64 (the last one padded to a multiple of 16), each a pass of its own over
-// the pairs through the same images, partials and value image.  A ring stage holds, up to D = 64, a column tile and
-// the slab's value image: at dk = 64 and 64 value columns 36.5 + 32 KB, two stages next to the 36 KB row image.  Above
-// D = 64 it is a K slab of tcwide.cuh (64 KB) with a value slot of its own next to the column tail: at 64 value
-// columns 14 KB (row tail, column tails, barriers) + 2 x (64 + 32) KB = 206 KB, where a third stage would take 302.
-struct TcApplyPlan {
-  TcPlan p;
-  bool wide;
-  int64_t off_v, off_vmax, total;
-};
-static int tc_apply_dkv(int K, int k0) { return tc_dk(std::min(64, K - k0)); }
-static void tc_apply_stages(bool wide, int kp, int dkv, int* nstage, int64_t* smem) {
-  const int64_t v_bytes = tc_value_img_bytes(dkv);
-  if (wide) {
-    int ns = kTcMaxStage;
-    while (ns > 0 && tc_wide_smem(ns) + ns * v_bytes > 227 * 1024) --ns;
-    *nstage = ns;
-    *smem = tc_wide_smem(ns) + ns * v_bytes;
-    return;
-  }
-  const int64_t bar_bytes = 256, b_bytes = tc_b_img_bytes(kp, kTcBN);
-  const int64_t ns = (227 * 1024 - bar_bytes - tc_a_span(kp)) / (b_bytes + v_bytes);
-  *nstage = (int)(ns > kTcMaxStage ? kTcMaxStage : ns);
-  *smem = tc_a_span(kp) + *nstage * (b_bytes + v_bytes) + bar_bytes;
-}
-static TcApplyPlan make_tc_apply_plan(int64_t N, int64_t M, int D, int K) {
-  TcApplyPlan a;
-  const int64_t rtpe = ceil_div64(N, kTcM), ctpe = ceil_div64(M, kTcBN);
-  a.p = make_tc_plan(D, true, rtpe, ctpe, rtpe, ctpe, N, 2 * 4);
-  a.p.rtpe = (int)rtpe;
-  a.p.ctpe = (int)ctpe;
-  a.wide = D > 64;
-  a.off_v = a.p.off_part + round_up64((int64_t)a.p.n_split * N * (1 + std::min(K, 64)) * 4, 256);
-  a.off_vmax = a.off_v + round_up64(a.p.b_tiles * tc_value_img_bytes(tc_apply_dkv(K, 0)), 256);
-  a.total = a.off_vmax + round_up64((int64_t)K * 4, 256);
-  return a;
-}
-
-int64_t plan_apply_tc_scratch_bytes(int64_t N, int64_t M, int D, int K) { return make_tc_apply_plan(N, M, D, K).total; }
-
-template <int DKV>
-static int tc_apply_launch(const TcApplyPlan& a, unsigned char* base, int64_t N, int kv, cudaStream_t st) {
-  int nstage;
-  int64_t smem;
-  tc_apply_stages(a.wide, a.p.kp, DKV, &nstage, &smem);
-  if (nstage < 2) return B200OT_EINVAL;
-  const auto kern = a.wide ? tc_wide_apply_kernel<DKV> : tc_apply_kernel<DKV>;
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const dim3 grid((unsigned)a.p.ctas, (unsigned)a.p.n_split);
-  kern<<<grid, kTcThreads, (size_t)smem, st>>>(base, base + a.p.off_b, base + a.off_v,
-                                               reinterpret_cast<float*>(base + a.p.off_part), N, a.p.kp, a.p.ctpe,
-                                               a.p.tiles_per_split, nstage, kv);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
-}
-
-// out (N, K) = row_factor_i sum_j softmax_j(...) V_jk on the tensor-core path.  Arguments already validated.
-int plan_apply_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
-                  const float* center, const float* lse2, const float* v, const float* row_factor, float* out,
-                  int64_t N, int64_t M, int D, int K, float eps, void* scratch, cudaStream_t st) {
-  const TcApplyPlan a = make_tc_apply_plan(N, M, D, K);
-  unsigned char* base = reinterpret_cast<unsigned char*>(scratch);
-  int rc = tc_pack(a.p, base, {x, y, center, softmin_coord_scale(2, eps), N, M, D, 1, nullptr, h_a, h_b, h_scale_b, lse2},
-                   st);
-  if (rc) return rc;
-  float* vmax = reinterpret_cast<float*>(base + a.off_vmax);
-  B200OT_CUDA_TRY(cudaMemsetAsync(vmax, 0, (size_t)K * sizeof(float), st));
-  col_absmax_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(M, 8), 1024), dim3(32, 8), 0, st>>>(v, M, K, vmax);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  float* part = reinterpret_cast<float*>(base + a.p.off_part);
-  for (int k0 = 0; k0 < K; k0 += 64) {
-    const int kv = std::min(64, K - k0), dkv = tc_apply_dkv(K, k0);
-    const int64_t ncols = a.p.b_tiles * kTcBN;
-    tc_pack_values_kernel<<<(unsigned)ceil_div64(ncols, 128), 128, 0, st>>>(v, vmax, M, K, k0, dkv, ncols,
-                                                                           base + a.off_v);
-    B200OT_CUDA_TRY(cudaGetLastError());
-    rc = dkv == 16   ? tc_apply_launch<16>(a, base, N, kv, st)
-         : dkv == 32 ? tc_apply_launch<32>(a, base, N, kv, st)
-         : dkv == 48 ? tc_apply_launch<48>(a, base, N, kv, st)
-                     : tc_apply_launch<64>(a, base, N, kv, st);
-    if (rc) return rc;
-    rc = plan_apply_finalize(part, a.p.n_split, 1 + kv, kv, k0, K, vmax, row_factor, out, N, st);
-    if (rc) return rc;
-  }
-  return B200OT_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Block-sparse softmins (the fine phase of the two-scale Sinkhorn above D = 8): every row cluster and every column
-// cluster is padded to whole 128-point tiles on its own, slot -> point through row_src / col_src (-1: padding).  One
-// segment per row tile; the host descriptors are validated here and copied into the scratch behind the partials
-// (tc_pass).
-// ---------------------------------------------------------------------------------------------------
-static_assert(kTcBlocksTile == kTcM && kTcBlocksTile == kTcBN, "segments are one row tile, pieces whole column tiles");
-
-int blocks_check(int64_t N, int D, int p, float eps, const void* scratch, TcBlocks& b) {
-  const b200ot_segment* seg = b.seg;
-  const b200ot_piece* pieces = b.pieces;
-  const int64_t n_row_slots = b.n_row_slots, n_col_slots = b.n_col_slots, n_seg = b.n_seg;
-  if (!seg || !pieces || N <= 0 || n_seg <= 0 || n_seg > 0x7fffffff || !tc_blocks_dims(D) || !valid_p(p) ||
-      p_exponent(p) != 2 || !(eps > 0.f))
-    return B200OT_EINVAL;
-  if ((((uintptr_t)seg) & 15) || (((uintptr_t)pieces) & 7) || (((uintptr_t)scratch) & 15)) return B200OT_EALIGN;
-  if (n_row_slots <= 0 || n_col_slots <= 0 || n_row_slots % kTcM || n_col_slots % kTcBN ||
-      n_row_slots / kTcM != n_seg || n_col_slots / kTcBN > 0x7fffffff)
-    return B200OT_EINVAL;
-  int64_t np = 0;
-  for (int64_t s = 0; s < n_seg; ++s) {
-    const b200ot_segment& g = seg[s];
-    if (g.row_start < 0 || g.row_start % kTcM || g.row_start >= n_row_slots || g.row_count < 1 ||
-        g.row_count > kTcM || g.piece_begin < 0 || g.piece_end < g.piece_begin)
-      return B200OT_EINVAL;
-    np = std::max<int64_t>(np, g.piece_end);
-  }
-  // column tiles before piece q, so that a segment's tile count is one difference
-  std::vector<int64_t> before(np + 1, 0);
-  for (int64_t q = 0; q < np; ++q) {
-    const b200ot_piece& c = pieces[q];
-    if (c.col_start < 0 || c.col_start % kTcBN || c.col_count <= 0 || c.col_count % kTcBN ||
-        (int64_t)c.col_start + c.col_count > n_col_slots)
-      return B200OT_EINVAL;
-    before[q + 1] = before[q] + c.col_count / kTcBN;
-  }
-  // every row tile belongs to exactly one segment: each live row is written once per split
-  std::vector<char> seen(n_seg, 0);
-  int64_t mt = 0;
-  for (int64_t s = 0; s < n_seg; ++s) {
-    const int64_t t = seg[s].row_start / kTcM;
-    if (seen[t]) return B200OT_EINVAL;
-    seen[t] = 1;
-    mt = std::max(mt, before[seg[s].piece_end] - before[seg[s].piece_begin]);
-  }
-  if (mt > 0x7fffffff) return B200OT_EINVAL;
-  b.max_tiles = (int)mt;
-  b.n_pieces = np;
-  return B200OT_OK;
-}
-
 }  // namespace b200ot
 
 using namespace b200ot;
@@ -684,23 +131,19 @@ extern "C" {
 
 B200OT_API int64_t b200ot_kernel_conv_scratch_bytes(int64_t N, int64_t M, int32_t D) {
   if (N <= 0 || M <= 0 || D <= 0) return 0;
-  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D, 1, 1) : 0;
+  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D) : 0;
   const ReducePlan pl = make_plan(N, M, D);
   const int64_t cols = b200ot_packed_cols_floats(M, D, 2) * 4;
   const int64_t part = (int64_t)pl.n_split * N * 4 * (D + 1);
   const int64_t simt = round_up64(cols, 256) + round_up64(part, 256);
   // (one size for every operator of the shape: the caller does not say which one it is about to run)
-  return tc_any_routed(D, N, M) ? std::max(simt, tc_scratch_bytes(N, M, D, 1, 1)) : simt;
+  return tc_any_routed(D, N, M) ? std::max(simt, tc_scratch_bytes(N, M, D)) : simt;
 }
 
 B200OT_API int b200ot_kernel_conv_finalize(const float* part, int32_t n_part, float* out, int64_t N, int32_t kind,
                                            void* stream) {
   if (!part || !out || n_part <= 0 || N <= 0 || !valid_kind(kind)) return B200OT_EINVAL;
-  const int threads = 256;
-  conv_fwd_finalize_kernel<<<(unsigned)ceil_div64(N, threads), threads, 0, (cudaStream_t)stream>>>(
-      part, n_part, kind_base(kind) == B200OT_KERNEL_ENERGY ? -1.f : 1.f, out, N);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
+  return conv_fwd_finalize(part, n_part, kind, out, N, nullptr, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_kernel_conv_bwd_finalize(const float* part, int32_t n_part, const float* x, const float* center,
@@ -710,12 +153,8 @@ B200OT_API int b200ot_kernel_conv_bwd_finalize(const float* part, int32_t n_part
     return B200OT_EINVAL;
   if (!blur_ok(kind, blur)) return B200OT_EINVAL;
   const ConvScales cs = conv_scales(kind, blur);
-  const int threads = 256;
-  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, threads), threads, 0, (cudaStream_t)stream>>>(
-      part, n_part, x, center, grad_out, grad_x, N, D, kind_base(kind), cs.scale, conv_bwd_coef(kind, cs, blur),
-      (const float*)nullptr);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
+  return conv_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, kind_base(kind), cs.scale,
+                           conv_bwd_coef(kind, cs, blur), nullptr, nullptr, nullptr, 0, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_kernel_conv_pack_gather(const float* y, const float* w, const float* center,
@@ -746,29 +185,24 @@ B200OT_API int b200ot_kernel_conv_partial_ranges(const float* x, const float* ce
                       reinterpret_cast<const int2*>(pieces));
 }
 
-// The kernel convolution of one problem, or (`batched`, 8 < D <= 64) of B problems of N rows / M columns side by side.
-// The two differ only in the shapes they accept and in their routing.
-static int conv_fwd_impl(const float* x, const float* y, const float* w, const float* center, float* out, int64_t B,
-                         int64_t N, int64_t M, int32_t D, int32_t kind, float blur, void* scratch,
-                         int64_t scratch_bytes, void* stream, bool batched) {
-  // laplacian / energy: the tensor cores serve 8 < D <= 64 only (no measured cross-over below)
-  const bool tc = batched || ((kind_base(kind) == B200OT_KERNEL_GAUSSIAN) ? tc_routed(kTcConvFwd, D, N, M)
-                                                                          : (D > B200OT_MAX_D && tc_capable_dim(D)));
-  const bool shape = batched ? tc_batched_dims(B, N, M, D) : (N > 0 && M > 0 && (supported_simt_dim(D) || tc));
-  if (!x || !y || !w || !out || !scratch || !shape || !valid_kind(kind)) return B200OT_EINVAL;
+// The kernel convolution of one problem.  Laplacian / energy: the tensor cores serve 8 < D <= 64 only (no measured
+// cross-over below).
+B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
+                                      float* out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                                      void* scratch, int64_t scratch_bytes, void* stream) {
+  const bool tc = (kind_base(kind) == B200OT_KERNEL_GAUSSIAN) ? tc_routed(kTcConvFwd, D, N, M)
+                                                              : (D > B200OT_MAX_D && tc_capable_dim(D));
+  if (!x || !y || !w || !out || !scratch || N <= 0 || M <= 0 || !(supported_simt_dim(D) || tc) || !valid_kind(kind))
+    return B200OT_EINVAL;
   if (!blur_ok(kind, blur)) return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, batched ? b200ot_batched_scratch_bytes(B, N, M, D)
-                                                                   : b200ot_kernel_conv_scratch_bytes(N, M, D)))
-    return rc;
-  if (tc)
-    return conv_tc(false, batched ? TcLayout::kBatch : TcLayout::kOne, kind, x, y, w, center, nullptr, out, nullptr, B,
-                   N, M, D, blur, scratch, (cudaStream_t)stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_kernel_conv_scratch_bytes(N, M, D))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tc) return tc_kernel_conv(false, kind, x, y, w, center, nullptr, out, nullptr, N, M, D, blur, scratch, st);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
                                          round_up64(b200ot_packed_cols_floats(M, D, 2) * 4, 256));
-  cudaStream_t st = (cudaStream_t)stream;
   int rc = conv_pack(y, w, center, M, D, cs, cols, st);
   if (rc) return rc;
   rc = conv_partial(kind, false, pl, st, x, center, cs, cols, part, N, D);
@@ -776,45 +210,30 @@ static int conv_fwd_impl(const float* x, const float* y, const float* w, const f
   return b200ot_kernel_conv_finalize(part, pl.n_split, out, N, kind, stream);
 }
 
-B200OT_API int b200ot_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
-                                      float* out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
-                                      void* scratch, int64_t scratch_bytes, void* stream) {
-  return conv_fwd_impl(x, y, w, center, out, 1, N, M, D, kind, blur, scratch, scratch_bytes, stream, false);
-}
-
-// Row gradients (and, with value_out, the forward values from the same pass: gaussian only), of one problem or
-// (`batched`) of B problems, as conv_fwd_impl.
+// Row gradients (and, with value_out, the forward values from the same pass: gaussian only), as b200ot_kernel_conv_fwd.
 static int conv_bwd_x_impl(const float* x, const float* y, const float* w, const float* center, const float* grad_out,
-                           float* grad_x, float* value_out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
-                           float blur, void* scratch, int64_t scratch_bytes, void* stream, bool batched) {
+                           float* grad_x, float* value_out, int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
+                           void* scratch, int64_t scratch_bytes, void* stream) {
   const bool gauss = kind_base(kind) == B200OT_KERNEL_GAUSSIAN;
-  const bool tc =
-      batched || (gauss ? tc_routed(kTcConvBwd, D, N, M) : (D > B200OT_MAX_D && tc_capable_dim(D)));
-  const bool shape = batched ? tc_batched_dims(B, N, M, D) : (N > 0 && M > 0 && (supported_simt_dim(D) || tc));
-  if (!x || !y || !w || !grad_x || !scratch || !shape || !valid_kind(kind) || (value_out && !gauss))
+  const bool tc = gauss ? tc_routed(kTcConvBwd, D, N, M) : (D > B200OT_MAX_D && tc_capable_dim(D));
+  if (!x || !y || !w || !grad_x || !scratch || N <= 0 || M <= 0 || !(supported_simt_dim(D) || tc) || !valid_kind(kind) ||
+      (value_out && !gauss))
     return B200OT_EINVAL;
   if (!blur_ok(kind, blur)) return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, batched ? b200ot_batched_scratch_bytes(B, N, M, D)
-                                                                   : b200ot_kernel_conv_scratch_bytes(N, M, D)))
-    return rc;
-  if (tc)
-    return conv_tc(true, batched ? TcLayout::kBatch : TcLayout::kOne, kind, x, y, w, center, grad_out, grad_x,
-                   value_out, B, N, M, D, blur, scratch, (cudaStream_t)stream);
+  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_kernel_conv_scratch_bytes(N, M, D))) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (tc) return tc_kernel_conv(true, kind, x, y, w, center, grad_out, grad_x, value_out, N, M, D, blur, scratch, st);
   const ReducePlan pl = make_plan(N, M, D);
   const ConvScales cs = conv_scales(kind, blur);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
                                          round_up64(b200ot_packed_cols_floats(M, D, 2) * 4, 256));
-  cudaStream_t st = (cudaStream_t)stream;
   int rc = conv_pack(y, w, center, M, D, cs, cols, st);
   if (rc) return rc;
   rc = conv_partial(kind, true, pl, st, x, center, cs, cols, part, N, D);
   if (rc) return rc;
-  conv_bwd_finalize_kernel<<<(unsigned)ceil_div64(N, 256), 256, 0, st>>>(
-      part, pl.n_split, x, center, grad_out, grad_x, N, D, kind_base(kind), cs.scale, conv_bwd_coef(kind, cs, blur),
-      (const float*)nullptr, value_out);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
+  return conv_bwd_finalize(part, pl.n_split, x, center, grad_out, grad_x, N, D, kind_base(kind), cs.scale,
+                           conv_bwd_coef(kind, cs, blur), nullptr, value_out, nullptr, 0, st);
 }
 
 B200OT_API int b200ot_kernel_conv_bwd_x(const float* x, const float* y, const float* w, const float* center,
@@ -822,8 +241,8 @@ B200OT_API int b200ot_kernel_conv_bwd_x(const float* x, const float* y, const fl
                                         int32_t kind, float blur, void* scratch, int64_t scratch_bytes,
                                         void* stream) {
   if (!grad_out) return B200OT_EINVAL;
-  return conv_bwd_x_impl(x, y, w, center, grad_out, grad_x, nullptr, 1, N, M, D, kind, blur, scratch, scratch_bytes,
-                         stream, false);
+  return conv_bwd_x_impl(x, y, w, center, grad_out, grad_x, nullptr, N, M, D, kind, blur, scratch, scratch_bytes,
+                         stream);
 }
 
 B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, const float* w, const float* center,
@@ -831,89 +250,7 @@ B200OT_API int b200ot_kernel_conv_fwd_bwd_x(const float* x, const float* y, cons
                                             int32_t kind, float blur, void* scratch, int64_t scratch_bytes,
                                             void* stream) {
   if (!out) return B200OT_EINVAL;
-  return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, 1, N, M, D, kind, blur, scratch, scratch_bytes,
-                         stream, false);
-}
-
-// ---- batches of B problems in the tensor-core dimensions (tc_reduce_kernel / tc_bwd_kernel with BATCH) ----
-B200OT_API int64_t b200ot_batched_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
-  return tc_batched_dims(B, N, M, D) ? tc_scratch_bytes(N, M, D, B, 1) : 0;
-}
-
-B200OT_API int b200ot_kernel_conv_fwd_batched(const float* x, const float* y, const float* w, const float* center,
-                                              float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
-                                              float blur, void* scratch, int64_t scratch_bytes, void* stream) {
-  return conv_fwd_impl(x, y, w, center, out, B, N, M, D, kind, blur, scratch, scratch_bytes, stream, true);
-}
-
-B200OT_API int b200ot_kernel_conv_bwd_x_batched(const float* x, const float* y, const float* w, const float* center,
-                                                const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
-                                                int32_t D, int32_t kind, float blur, void* scratch,
-                                                int64_t scratch_bytes, void* stream) {
-  if (!grad_out) return B200OT_EINVAL;
-  return conv_bwd_x_impl(x, y, w, center, grad_out, grad_x, nullptr, B, N, M, D, kind, blur, scratch, scratch_bytes,
-                         stream, true);
-}
-
-B200OT_API int b200ot_kernel_conv_fwd_bwd_x_batched(const float* x, const float* y, const float* w,
-                                                    const float* center, float* out, float* grad_unit, int64_t B,
-                                                    int64_t N, int64_t M, int32_t D, int32_t kind, float blur,
-                                                    void* scratch, int64_t scratch_bytes, void* stream) {
-  if (!out) return B200OT_EINVAL;
-  return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, B, N, M, D, kind, blur, scratch, scratch_bytes,
-                         stream, true);
-}
-
-// ---- above D = 64: the K-slab tensor-core kernels (tcwide.cuh), B >= 1 elements ----
-B200OT_API int64_t b200ot_wide_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
-  return tc_wide_dims(B, N, M, D) ? tc_scratch_bytes(N, M, D, B, 2) : 0;
-}
-
-B200OT_API int b200ot_wide_softmin_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
-                                       float h_scale_b, const float* center, const float* out_old, float alpha_old,
-                                       float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
-                                       int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                       void* stream) {
-  if (!x || !y || !h_a || !scratch || !tc_wide_dims(B, N, M, D) || !valid_p(p) || !(eps > 0.f) || (!out && !lse2_out))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
-  return softmin_fwd_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps}, nullptr,
-                        out_old, alpha_old, beta, out, lse2_out, scratch, stream);
-}
-
-B200OT_API int b200ot_wide_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
-                                         float h_scale_b, const float* center, const float* lse2,
-                                         const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
-                                         int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                         void* stream) {
-  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_wide_dims(B, N, M, D) || !valid_p(p) ||
-      !(eps > 0.f))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
-  return softmin_bwd_x_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps}, nullptr,
-                          grad_out, grad_x, scratch, (cudaStream_t)stream);
-}
-
-B200OT_API int b200ot_wide_kernel_conv_fwd(const float* x, const float* y, const float* w, const float* center,
-                                           float* out, int64_t B, int64_t N, int64_t M, int32_t D, int32_t kind,
-                                           float blur, void* scratch, int64_t scratch_bytes, void* stream) {
-  if (!x || !y || !w || !out || !scratch || !tc_wide_dims(B, N, M, D) || !valid_kind(kind) || !blur_ok(kind, blur))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
-  return conv_tc(false, TcLayout::kBatch, kind, x, y, w, center, nullptr, out, nullptr, B, N, M, D, blur, scratch,
-                 (cudaStream_t)stream);
-}
-
-B200OT_API int b200ot_wide_kernel_conv_bwd_x(const float* x, const float* y, const float* w, const float* center,
-                                             const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
-                                             int32_t D, int32_t kind, float blur, void* scratch,
-                                             int64_t scratch_bytes, void* stream) {
-  if (!x || !y || !w || !grad_out || !grad_x || !scratch || !tc_wide_dims(B, N, M, D) || !valid_kind(kind) ||
-      !blur_ok(kind, blur))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_scratch_bytes(B, N, M, D))) return rc;
-  return conv_tc(true, TcLayout::kBatch, kind, x, y, w, center, grad_out, grad_x, nullptr, B, N, M, D, blur, scratch,
-                 (cudaStream_t)stream);
+  return conv_bwd_x_impl(x, y, w, center, nullptr, grad_unit, out, N, M, D, kind, blur, scratch, scratch_bytes, stream);
 }
 
 }  // extern "C"

@@ -122,9 +122,6 @@ static int plan_apply_simt(const float* x, const float* y, const float* h_a, con
 static bool plan_apply_dims(int64_t N, int64_t M, int D, int64_t K) {
   return N > 0 && M > 0 && tc_capable_dim(D) && K >= 1 && K <= 0x7fffffff;
 }
-static bool plan_apply_wide_dims(int64_t N, int64_t M, int D, int64_t K) {
-  return tc_wide_dims(1, N, M, D) && K >= 1 && K <= 0x7fffffff;
-}
 
 }  // namespace b200ot
 
@@ -134,7 +131,7 @@ extern "C" {
 
 B200OT_API int64_t b200ot_plan_apply_scratch_bytes(int64_t N, int64_t M, int32_t D, int64_t K) {
   if (!plan_apply_dims(N, M, D, K)) return 0;
-  if (tc_routed(kTcSoftminBwd, D, N, M)) return plan_apply_tc_scratch_bytes(N, M, D, (int)K);
+  if (tc_routed(kTcSoftminBwd, D, N, M)) return tc_plan_apply_scratch_bytes(N, M, D, (int)K);
   return make_simt_apply_plan(N, M, D, (int)K).total;
 }
 
@@ -149,26 +146,9 @@ B200OT_API int b200ot_plan_apply(const float* x, const float* y, const float* h_
   if (scratch_bytes < b200ot_plan_apply_scratch_bytes(N, M, D, K)) return B200OT_ESCRATCH;
   cudaStream_t st = (cudaStream_t)stream;
   if (tc_routed(kTcSoftminBwd, D, N, M))
-    return plan_apply_tc(x, y, h_a, h_b, h_scale_b, center, lse2, v, row_factor, out, N, M, D, (int)K, eps, scratch, st);
+    return tc_plan_apply(x, y, h_a, h_b, h_scale_b, center, lse2, v, row_factor, out, N, M, D, (int)K, eps, scratch, st);
   return plan_apply_simt(x, y, h_a, h_b, h_scale_b, center, lse2, v, row_factor, out, N, M, D, (int)K, eps, scratch,
                          st);
-}
-
-// ---- above D = 64: the K-slab tensor-core kernel (tcapply.cuh, tc_wide_apply_kernel), one problem ----
-B200OT_API int64_t b200ot_wide_plan_apply_scratch_bytes(int64_t N, int64_t M, int32_t D, int64_t K) {
-  return plan_apply_wide_dims(N, M, D, K) ? plan_apply_tc_scratch_bytes(N, M, D, (int)K) : 0;
-}
-
-B200OT_API int b200ot_wide_plan_apply(const float* x, const float* y, const float* h_a, const float* h_b,
-                                      float h_scale_b, const float* center, const float* lse2, const float* v,
-                                      const float* row_factor, float* out, int64_t N, int64_t M, int32_t D, int64_t K,
-                                      int32_t p, float eps, void* scratch, int64_t scratch_bytes, void* stream) {
-  if (!x || !y || !h_a || !lse2 || !v || !out || !scratch || !plan_apply_wide_dims(N, M, D, K) || !valid_p(p) ||
-      p_exponent(p) != 2 || !(eps > 0.f))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_wide_plan_apply_scratch_bytes(N, M, D, K))) return rc;
-  return plan_apply_tc(x, y, h_a, h_b, h_scale_b, center, lse2, v, row_factor, out, N, M, D, (int)K, eps, scratch,
-                       (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -197,14 +197,14 @@ B200OT_API int32_t b200ot_softmin_num_splits(int64_t N, int64_t M, int32_t D) {
 
 B200OT_API int64_t b200ot_softmin_scratch_bytes(int64_t N, int64_t M, int32_t D) {
   if (N <= 0 || M <= 0 || D <= 0) return 0;
-  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D, 1, 1) : 0;
+  if (D > B200OT_MAX_D) return tc_capable_dim(D) ? tc_scratch_bytes(N, M, D) : 0;
   const ReducePlan pl = make_plan(N, M, D);
   const int64_t cols = b200ot_packed_cols_floats(M, D, 1) * 4;
   // forward partials are (m, s) pairs; the backward pass keeps D+1 sums per (split, row)
   const int64_t part = (int64_t)pl.n_split * N * 4 * (D + 1 > 2 ? D + 1 : 2);
   const int64_t simt = round_up64(cols, 256) + round_up64(part, 256);
   if (!tc_any_routed(D, N, M)) return simt;
-  const int64_t tc = tc_scratch_bytes(N, M, D, 1, 1);
+  const int64_t tc = tc_scratch_bytes(N, M, D);
   return simt > tc ? simt : tc;
 }
 
@@ -293,8 +293,8 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
     return B200OT_EINVAL;
   if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_scratch_bytes(N, M, D))) return rc;
   if (tc)
-    return softmin_fwd_tc(TcLayout::kOne, {x, y, h_a, h_b, h_scale_b, center, nullptr, 1, N, M, D, p, eps}, nullptr,
-                          out_old, alpha_old, beta, out, lse2_out, scratch, stream);
+    return tc_softmin_fwd(x, y, h_a, h_b, h_scale_b, center, out_old, alpha_old, beta, out, lse2_out, N, M, D, p, eps,
+                          scratch, stream);
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
@@ -305,64 +305,6 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
   rc = softmin_partial_impl(x, center, cols, part, pl, N, D, p, eps, st);
   if (rc) return rc;
   return b200ot_softmin_finalize(part, pl.n_split, out_old, alpha_old, beta, out, lse2_out, N, eps, stream);
-}
-
-B200OT_API int b200ot_softmin_fwd_batched(const float* x, const float* y, const float* h_a, const float* h_b,
-                                          float h_scale_b, const float* center, const float* out_old, float alpha_old,
-                                          float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
-                                          int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                          void* stream) {
-  // p = 2 only: the p = 1 softmin has no tensor-core kernel
-  if (!x || !y || !h_a || !scratch || !tc_batched_dims(B, N, M, D) || !valid_p(p) || p_exponent(p) != 2 ||
-      !(eps > 0.f) || (!out && !lse2_out))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_batched_scratch_bytes(B, N, M, D))) return rc;
-  return softmin_fwd_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps}, nullptr,
-                        out_old, alpha_old, beta, out, lse2_out, scratch, stream);
-}
-
-// ---- the p = 1 softmin in the tensor-core dimensions (tc_reduce_kernel<6> / tc_bwd_kernel<7>, batched flavour) ----
-B200OT_API int64_t b200ot_softmin_l1_scratch_bytes(int64_t B, int64_t N, int64_t M, int32_t D) {
-  return tc_l1_args(B, N, M, D, 1) ? tc_scratch_bytes(N, M, D, B, 2) : 0;
-}
-
-B200OT_API int b200ot_softmin_l1_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
-                                     float h_scale_b, const float* center, const float* out_old, float alpha_old,
-                                     float beta, float* out, float* lse2_out, int64_t B, int64_t N, int64_t M,
-                                     int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                     void* stream) {
-  if (!x || !y || !h_a || !scratch || !tc_l1_args(B, N, M, D, p) || !(eps > 0.f) || (!out && !lse2_out))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_l1_scratch_bytes(B, N, M, D))) return rc;
-  return softmin_fwd_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, nullptr, B, N, M, D, p, eps}, nullptr,
-                        out_old, alpha_old, beta, out, lse2_out, scratch, stream);
-}
-
-B200OT_API void b200ot_blocks_shape(int32_t* rows_per_segment, int32_t* col_align) {
-  if (rows_per_segment) *rows_per_segment = kTcBlocksTile;
-  if (col_align) *col_align = kTcBlocksTile;
-}
-
-B200OT_API int64_t b200ot_blocks_scratch_bytes(int64_t N, int64_t n_row_slots, int64_t n_col_slots,
-                                               const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
-                                               int32_t D) {
-  TcBlocks b{nullptr, nullptr, n_row_slots, n_col_slots, seg, n_seg, pieces};
-  return blocks_check(N, D, 2, 1.f, nullptr, b) ? 0 : tc_blocks_scratch_bytes(N, D, b);
-}
-
-B200OT_API int b200ot_softmin_fwd_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
-                                         float h_scale_b, const float* center, const float* out_old, float alpha_old,
-                                         float beta, float* out, float* lse2_out, int64_t N, const int32_t* row_src,
-                                         int64_t n_row_slots, const int32_t* col_src, int64_t n_col_slots,
-                                         const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
-                                         int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                         void* stream) {
-  if (!x || !y || !h_a || !row_src || !col_src || !scratch || (!out && !lse2_out)) return B200OT_EINVAL;
-  TcBlocks b{row_src, col_src, n_row_slots, n_col_slots, seg, n_seg, pieces};
-  if (const int rc = blocks_check(N, D, p, eps, scratch, b)) return rc;
-  if (scratch_bytes < tc_blocks_scratch_bytes(N, D, b)) return B200OT_ESCRATCH;
-  return softmin_fwd_tc(TcLayout::kBlocks, {x, y, h_a, h_b, h_scale_b, center, nullptr, 1, N, 0, D, p, eps}, &b, out_old,
-                        alpha_old, beta, out, lse2_out, scratch, stream);
 }
 
 }  // extern "C"

@@ -128,12 +128,12 @@ B200OT_API int b200ot_softmin_bwd_finalize(const float* part, int32_t n_part, co
   return B200OT_OK;
 }
 
-// Runs pack + partial reduction of the row-gradient pass and leaves r->n_part sets of (N, D+1) sums in scratch, each
-// `*scale_out` times the softmax-weighted sums (kTcPScale on the tensor-core path, common.cuh; 1 otherwise).
+// Runs pack + partial reduction of the row-gradient pass and leaves *n_part sets of (N, D+1) sums in scratch at *part,
+// each `*scale_out` times the softmax-weighted sums (kTcPScale on the tensor-core path, common.cuh; 1 otherwise).
 static int softmin_bwd_partials(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
                                 const float* center, const float* lse2, int64_t N, int64_t M, int32_t D, int32_t p,
-                                float eps, void* scratch, int64_t scratch_bytes, void* stream, TcPass* r,
-                                float* scale_out) {
+                                float eps, void* scratch, int64_t scratch_bytes, void* stream, float** part,
+                                int* n_part, float* scale_out) {
   const bool tc = p_exponent(p) == 2 && tc_routed(kTcSoftminBwd, D, N, M);
   if (!x || !y || !h_a || !lse2 || !scratch || N <= 0 || M <= 0 || (!supported_simt_dim(D) && !tc) || !valid_p(p) ||
       !(eps > 0.f))
@@ -141,18 +141,16 @@ static int softmin_bwd_partials(const float* x, const float* y, const float* h_a
   if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_scratch_bytes(N, M, D))) return rc;
   *scale_out = tc ? kTcPScale : 1.f;
   if (tc)
-    return softmin_pass_tc(true, TcLayout::kOne, {x, y, h_a, h_b, h_scale_b, center, lse2, 1, N, M, D, p, eps}, nullptr,
-                           scratch, (cudaStream_t)stream, r);
+    return tc_softmin_bwd_sums(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch, (cudaStream_t)stream,
+                               part, n_part);
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
-  float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
-                                         round_up64(b200ot_packed_cols_floats(M, D, 1) * 4, 256));
+  *part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
+                                   round_up64(b200ot_packed_cols_floats(M, D, 1) * 4, 256));
+  *n_part = pl.n_split;
   int rc = softmin_pack_impl(y, h_a, h_b, h_scale_b, center, M, D, p, eps, cols, (cudaStream_t)stream, nullptr);
   if (rc) return rc;
-  rc = b200ot_softmin_bwd_partial(x, center, cols, lse2, part, pl.n_split, N, M, D, p, eps, stream);
-  r->part = part;
-  r->n_part = pl.n_split;
-  return rc;
+  return b200ot_softmin_bwd_partial(x, center, cols, lse2, *part, pl.n_split, N, M, D, p, eps, stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_sums(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -160,13 +158,14 @@ B200OT_API int b200ot_softmin_bwd_sums(const float* x, const float* y, const flo
                                        int64_t N, int64_t M, int32_t D, int32_t p, float eps, void* scratch,
                                        int64_t scratch_bytes, void* stream) {
   if (!sums) return B200OT_EINVAL;
-  TcPass r;
+  float* part = nullptr;
+  int n_part = 0;
   float p_scale = 1.f;
   const int rc = softmin_bwd_partials(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch,
-                                      scratch_bytes, stream, &r, &p_scale);
+                                      scratch_bytes, stream, &part, &n_part, &p_scale);
   if (rc) return rc;
   // raw sums leave the library (the multi-GPU engine adds them over the column shards): undo the P scale here
-  return rowsum_merge(r.part, r.n_part, D + 1, sums, N, 1.f / p_scale, (cudaStream_t)stream);
+  return rowsum_merge(part, n_part, D + 1, sums, N, 1.f / p_scale, (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -174,51 +173,13 @@ B200OT_API int b200ot_softmin_bwd_x(const float* x, const float* y, const float*
                                     float* grad_x, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
                                     void* scratch, int64_t scratch_bytes, void* stream) {
   if (!grad_out || !grad_x) return B200OT_EINVAL;
-  TcPass r;
+  float* part = nullptr;
+  int n_part = 0;
   float p_scale = 1.f;  // cancels: the finalize divides by the row sum of P
   const int rc = softmin_bwd_partials(x, y, h_a, h_b, h_scale_b, center, lse2, N, M, D, p, eps, scratch,
-                                      scratch_bytes, stream, &r, &p_scale);
+                                      scratch_bytes, stream, &part, &n_part, &p_scale);
   if (rc) return rc;
-  return b200ot_softmin_bwd_finalize(r.part, r.n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
-}
-
-B200OT_API int b200ot_softmin_bwd_x_batched(const float* x, const float* y, const float* h_a, const float* h_b,
-                                            float h_scale_b, const float* center, const float* lse2,
-                                            const float* grad_out, float* grad_x, int64_t B, int64_t N, int64_t M,
-                                            int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                            void* stream) {
-  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_batched_dims(B, N, M, D) || !valid_p(p) ||
-      p_exponent(p) != 2 || !(eps > 0.f))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_batched_scratch_bytes(B, N, M, D))) return rc;
-  return softmin_bwd_x_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps}, nullptr,
-                          grad_out, grad_x, scratch, (cudaStream_t)stream);
-}
-
-B200OT_API int b200ot_softmin_l1_bwd_x(const float* x, const float* y, const float* h_a, const float* h_b,
-                                       float h_scale_b, const float* center, const float* lse2, const float* grad_out,
-                                       float* grad_x, int64_t B, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
-                                       void* scratch, int64_t scratch_bytes, void* stream) {
-  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !scratch || !tc_l1_args(B, N, M, D, p) || !(eps > 0.f))
-    return B200OT_EINVAL;
-  if (const int rc = scratch_check(scratch, scratch_bytes, b200ot_softmin_l1_scratch_bytes(B, N, M, D))) return rc;
-  return softmin_bwd_x_tc(TcLayout::kBatch, {x, y, h_a, h_b, h_scale_b, center, lse2, B, N, M, D, p, eps}, nullptr,
-                          grad_out, grad_x, scratch, (cudaStream_t)stream);
-}
-
-B200OT_API int b200ot_softmin_bwd_x_blocks(const float* x, const float* y, const float* h_a, const float* h_b,
-                                           float h_scale_b, const float* center, const float* lse2,
-                                           const float* grad_out, float* grad_x, int64_t N, const int32_t* row_src,
-                                           int64_t n_row_slots, const int32_t* col_src, int64_t n_col_slots,
-                                           const b200ot_segment* seg, int64_t n_seg, const b200ot_piece* pieces,
-                                           int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
-                                           void* stream) {
-  if (!x || !y || !h_a || !lse2 || !grad_out || !grad_x || !row_src || !col_src || !scratch) return B200OT_EINVAL;
-  TcBlocks b{row_src, col_src, n_row_slots, n_col_slots, seg, n_seg, pieces};
-  if (const int rc = blocks_check(N, D, p, eps, scratch, b)) return rc;
-  if (scratch_bytes < tc_blocks_scratch_bytes(N, D, b)) return B200OT_ESCRATCH;
-  return softmin_bwd_x_tc(TcLayout::kBlocks, {x, y, h_a, h_b, h_scale_b, center, lse2, 1, N, 0, D, p, eps}, &b,
-                          grad_out, grad_x, scratch, (cudaStream_t)stream);
+  return b200ot_softmin_bwd_finalize(part, n_part, x, center, grad_out, grad_x, N, D, p, eps, stream);
 }
 
 }  // extern "C"

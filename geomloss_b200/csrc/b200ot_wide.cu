@@ -1,5 +1,6 @@
-// b200ot — instantiations of the tensor-core kernels above D = 64 (tcwide.cuh).  The host side (plans, packs,
-// finalize kernels, the b200ot_wide_* entries) is that of the other tensor-core operators, in b200ot_kernel_conv.cu.
+// b200ot — instantiations of the tensor-core kernels above D = 64 (tcwide.cuh), in a translation unit of their own so
+// that they compile in parallel with b200ot_tc.cu.  The host side (plans, packs, finalizes, the b200ot_wide_* entries)
+// is that of the other tensor-core operators, in b200ot_tc.cu.
 #include "b200ot.h"
 #include "host_util.cuh"
 #include "tcwide.cuh"

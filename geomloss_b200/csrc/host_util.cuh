@@ -40,99 +40,57 @@ inline float softmin_coord_scale(int p, float eps) {
 int softmin_pack_impl(const float* y, const float* h_a, const float* h_b, float h_scale_b, const float* center,
                       int64_t M, int D, int p, float eps, float* cols_out, cudaStream_t st, const int* src);
 
-// Tensor-core (wgmma) path, defined in b200ot_kernel_conv.cu.  The kernels serve any 1 <= D <= 64 (coordinates are
-// zero-padded to a multiple of 16); above B200OT_MAX_D they are the only path, at or below it `tc_routed` decides per
-// operator from the measured cross-over (see there).
+// ---- the tensor-core (wgmma) path, b200ot_tc.cu ----
+// The kernels serve any 1 <= D <= 64 (coordinates are zero-padded to a multiple of 16); above B200OT_MAX_D they are the
+// only path, at or below it `tc_routed` decides per operator from the measured cross-over (see there).
 enum TcOp { kTcSoftminFwd = 0, kTcSoftminBwd = 1, kTcConvFwd = 2, kTcConvBwd = 3 };
 inline bool tc_capable_dim(int D) { return D >= 1 && D <= 64; }
 bool tc_routed(int op, int D, int64_t N, int64_t M);
 bool tc_any_routed(int D, int64_t N, int64_t M);  // some operator of this shape takes the tensor-core path (scratch sizing)
-// Scratch of B problems of N rows x M columns (B = 1: one problem), any D the tensor cores serve: the larger of the
-// forward plan and the row-gradient plan, whose rows keep D + head sums (head = 2: the p = 1 softmin)
-int64_t tc_scratch_bytes(int64_t N, int64_t M, int D, int64_t B, int head);
-// Shapes of the batched entry points: 8 < D <= 64 only (smaller dimensions batch through the ranges entry points)
-inline bool tc_batched_dims(int64_t B, int64_t N, int64_t M, int D) {
-  return B >= 1 && N > 0 && M > 0 && D > B200OT_MAX_D && tc_capable_dim(D);
-}
-// The p = 1 softmin on the tensor cores (b200ot_softmin_l1_*): B >= 1 elements, 8 < D <= 64, p = 1 | UNCLAMPED
-inline bool tc_l1_args(int64_t B, int64_t N, int64_t M, int D, int p) {
-  return tc_batched_dims(B, N, M, D) && valid_p(p) && p_exponent(p) == 1;
-}
-// Above D = 64 (b200ot_wide_*, tcwide.cuh): B >= 1 elements, 64 < D <= B200OT_MAX_D_WIDE
-inline bool tc_wide_dims(int64_t B, int64_t N, int64_t M, int D) {
-  return B >= 1 && N > 0 && M > 0 && D > 64 && D <= B200OT_MAX_D_WIDE;
-}
-// The parameter list of tc_reduce_kernel / tc_bwd_kernel and of the wide kernels
+// Scratch of one problem of N rows x M columns, any D the tensor cores serve: enough for the softmin and kernel
+// convolution passes, forward and row gradients
+int64_t tc_scratch_bytes(int64_t N, int64_t M, int D);
+int64_t tc_plan_apply_scratch_bytes(int64_t N, int64_t M, int D, int K);
+// One problem on the tensor cores, the arguments validated by the caller.  The softmin forward leaves out / lse2_out as
+// b200ot_softmin_finalize; the row-gradient sums leave *n_part sets of (N, D + 1) sums inside the scratch at *part,
+// times kTcPScale (common.cuh); the kernel convolution leaves out (forward) or grad_x (bwd) in res and, with value_out,
+// the forward values from the same pass (gaussian only); the plan apply leaves out (N, K) as b200ot_plan_apply.
+int tc_softmin_fwd(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                   const float* center, const float* out_old, float alpha_old, float beta, float* out, float* lse2_out,
+                   int64_t N, int64_t M, int D, int p, float eps, void* scratch, void* stream);
+int tc_softmin_bwd_sums(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                        const float* center, const float* lse2, int64_t N, int64_t M, int D, int p, float eps,
+                        void* scratch, cudaStream_t st, float** part, int* n_part);
+int tc_kernel_conv(bool bwd, int kind, const float* x, const float* y, const float* w, const float* center,
+                   const float* grad_out, float* res, float* value_out, int64_t N, int64_t M, int D, float blur,
+                   void* scratch, cudaStream_t st);
+int tc_plan_apply(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                  const float* center, const float* lse2, const float* v, const float* row_factor, float* out,
+                  int64_t N, int64_t M, int D, int K, float eps, void* scratch, cudaStream_t st);
+// The parameter list of tc_reduce_kernel / tc_bwd_kernel and of the wide kernels, and the wide kernel of a
+// tc_reduce_kernel (bwd = false) or tc_bwd_kernel MODE, null for a mode it does not serve: instantiated in
+// b200ot_wide.cu, a translation unit of its own so that it compiles next to b200ot_tc.cu
 using TcKernel = void (*)(const unsigned char*, const unsigned char*, float*, int64_t, int, int, int, int, int, int,
                           float, const float*, int, int64_t, const int4*, const int2*, const int*);
-// the wide kernel of a tc_reduce_kernel (bwd = false) or tc_bwd_kernel MODE, null for a mode it does not serve
-// (b200ot_wide.cu)
 TcKernel tc_wide_kernel(int mode, bool bwd);
 
-// How the rows and columns of a tensor-core pass are laid out: one problem, a batch of B problems side by side (x
-// (B,N,D), y (B,M,D), element b of the rows reduced over element b of the columns only), or one block-sparse problem.
-// The p = 1 softmin runs the batch kernels only, B = 1 included.
-enum class TcLayout { kOne, kBatch, kBlocks };
-
-// A block-sparse problem (8 < D <= 64, p = 2; b200ot_*_blocks): every row cluster and every column cluster is padded
-// to whole kTcBlocksTile-point tiles on its own, slot -> point through row_src / col_src (-1: padding), one segment per
-// row tile.  blocks_check fills max_tiles (the longest segment in column tiles) and n_pieces (the pieces the segments
-// reference).
-inline bool tc_blocks_dims(int D) { return D > B200OT_MAX_D && tc_capable_dim(D); }
-constexpr int kTcBlocksTile = 128;  // segment height and column alignment: the kernels' tile (kTcM = kTcBN, tcconv.cuh)
-struct TcBlocks {
-  const int *row_src, *col_src;
-  int64_t n_row_slots, n_col_slots;
-  const b200ot_segment* seg;
-  int64_t n_seg;
-  const b200ot_piece* pieces;
-  int64_t n_pieces = 0;
-  int max_tiles = 0;
-};
-// The checks every b200ot_*_blocks entry makes before any launch, in this order: EINVAL for a null descriptor array,
-// N <= 0, n_seg <= 0, D outside (8, 64], p other than 2 (| B200OT_P_UNCLAMPED) or eps <= 0; EALIGN for misaligned
-// descriptor arrays or scratch; EINVAL for descriptors off the tile grid.
-int blocks_check(int64_t N, int D, int p, float eps, const void* scratch, TcBlocks& b);
-int64_t tc_blocks_scratch_bytes(int64_t N, int D, const TcBlocks& b);
-
-// A softmin on the tensor cores: B elements of N rows / M columns (TcLayout::kBlocks: B = 1, N rows, the slots in the
-// TcBlocks).  p may carry B200OT_P_UNCLAMPED; lse2: the forward's, for the row gradients.
-struct TcSoftmin {
-  const float *x, *y, *h_a, *h_b;
-  float h_scale_b;
-  const float *center, *lse2;
-  int64_t B, N, M;
-  int D, p;
-  float eps;
-};
-// What a pass leaves for its finalize: n_part sets of partials inside the scratch ((m, s) pairs forward, D + head sums
-// per row for the row gradients), and the maxima the finalize undoes (null when the pass has none)
-struct TcPass {
-  float* part = nullptr;
-  int n_part = 0;
-  const float* w_absmax = nullptr;
-  const float* coord_absmax = nullptr;
-};
-int softmin_pass_tc(bool bwd, TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, void* scratch,
-                    cudaStream_t st, TcPass* r);
-// out / lse2_out of the B N rows, as b200ot_softmin_finalize
-int softmin_fwd_tc(TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, const float* out_old, float alpha_old,
-                   float beta, float* out, float* lse2_out, void* scratch, void* stream);
-int softmin_bwd_x_tc(TcLayout layout, const TcSoftmin& s, const TcBlocks* blocks, const float* grad_out, float* grad_x,
-                     void* scratch, cudaStream_t st);
+// ---- finalize launches that both paths share, defined with their operator ----
+// out = sign(kind) sum of the n_part (N) partials, the energy's coordinate scale undone when coord_absmax is given
+// (b200ot_kernel_conv.cu: conv_fwd_finalize_kernel)
+int conv_fwd_finalize(const float* part, int n_part, int kind, float* out, int64_t N, const float* coord_absmax,
+                      cudaStream_t st);
+// grad_x (and value_out) from the row-gradient sums of a kernel convolution (b200ot_kernel_conv.cu:
+// conv_bwd_finalize_kernel)
+int conv_bwd_finalize(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
+                      float* grad_x, int64_t N, int D, int kind, float scale, float coef, const float* w_absmax,
+                      float* value_out, const float* coord_absmax, int64_t n_per, cudaStream_t st);
 // grad_x of the N rows from the p = 2 softmin's tensor-core row-gradient sums, (n_part, N, D + 1), any D
 // (b200ot_softmin_bwd.cu)
 int softmin_bwd_finalize_tc(const float* part, int n_part, const float* x, const float* center, const float* grad_out,
                             float* grad_x, int64_t N, int D, float eps, cudaStream_t st);
-
-// The plan applied to a value matrix v (M, K) (b200ot_plan_apply): the tensor-core pass (b200ot_kernel_conv.cu,
-// tcapply.cuh) and the finalize both paths share (b200ot_plan_apply.cu).
-int64_t plan_apply_tc_scratch_bytes(int64_t N, int64_t M, int D, int K);
-int plan_apply_tc(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
-                  const float* center, const float* lse2, const float* v, const float* row_factor, float* out,
-                  int64_t N, int64_t M, int D, int K, float eps, void* scratch, cudaStream_t st);
 // out[i, k0 + k] = row_factor_i (sum_s part[s, i, 1 + k]) / (sum_s part[s, i, 0]) / s_k for k < kv, part (n_part, N,
 // nacc); s_k = tc_energy_coord_scale(vmax[k0 + k]) when vmax is given, row_factor_i = 1 when it is null
+// (b200ot_plan_apply.cu)
 int plan_apply_finalize(const float* part, int n_part, int nacc, int kv, int k0, int K, const float* vmax,
                         const float* row_factor, float* out, int64_t N, cudaStream_t st);
 

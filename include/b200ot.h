@@ -209,7 +209,7 @@ B200OT_API int b200ot_softmin_bwd_finalize(const float* part, int32_t n_part, co
 /* b200ot_kernel_conv_fwd and _bwd_x additionally accept 8 < D <= 64 for every kind: that range runs on the tensor
  * cores (wgmma, fp16x2 split operands, exponent accumulated in registers; laplacian / energy take d from it, see
  * DESIGN.md section 3.3d).  For D <= B200OT_MAX_D the gaussian kernel takes the faster of the two paths per operator
- * and problem size (csrc/b200ot_kernel_conv.cu: tc_routed); laplacian / energy stay on the CUDA cores.  Results agree
+ * and problem size (csrc/b200ot_tc.cu: tc_routed); laplacian / energy stay on the CUDA cores.  Results agree
  * to the tolerances of DESIGN.md section 4 either way. */
 B200OT_API int64_t b200ot_kernel_conv_scratch_bytes(int64_t N, int64_t M, int32_t D);
 

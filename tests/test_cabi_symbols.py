@@ -76,7 +76,7 @@ def test_argument_validation_needs_no_gpu(L):
 
 def test_routing_below_nine_dimensions_shows_in_the_scratch_size(L, monkeypatch):
     """D <= 8: large forward problems take the tensor-core path from D = 7 (softmin) / D = 5 (gaussian)
-    (csrc/b200ot_kernel_conv.cu: tc_routed); the size queries then cover both paths.  $B200OT_TC_MIN_D /
+    (csrc/b200ot_tc.cu: tc_routed); the size queries then cover both paths.  $B200OT_TC_MIN_D /
     $B200OT_TC_MIN_PAIRS are read on every call.  (Observed on a small shape with the size threshold lifted: there the
     tensor-core images are the larger of the two needs.)"""
     def sizes():

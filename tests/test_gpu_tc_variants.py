@@ -1,4 +1,4 @@
-"""GPU parity of the tensor-core kernels' routing knobs (csrc/b200ot_kernel_conv.cu: tc_routed), of the row-gradient
+"""GPU parity of the tensor-core kernels' routing knobs (csrc/b200ot_tc.cu: tc_routed), of the row-gradient
 kernel at every padded dimension (csrc/tcbwd.cuh) and of the one-pass value + row-gradient entry
 (b200ot_kernel_conv_fwd_bwd_x).  Every route — not only the shipped default — is held to the same bars against the
 fp64 oracle as the default kernels in test_gpu_parity.py, so that a default can be flipped from a measurement

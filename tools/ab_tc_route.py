@@ -2,7 +2,7 @@
 (the knobs are environment variables the C entry points read on every call):
 
   part A  CUDA-core vs tensor-core path for D <= 8 (B200OT_TC_MIN_D / B200OT_TC_MIN_PAIRS), per operator and size —
-          the cross-over that csrc/b200ot_kernel_conv.cu::kTcMinDimDefault encodes;
+          the cross-over that csrc/b200ot_tc.cu::kTcMinDimDefault encodes;
   part C  value + unit gradient in one pass (b200ot_kernel_conv_fwd_bwd_x) against the two separate reductions;
   part D  BASELINE configs[2] (gaussian MMD, N = M = 1e6, D = 64, forward + gradient), two-pass and one-pass.
 
