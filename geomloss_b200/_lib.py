@@ -28,6 +28,10 @@ _SIGNATURES = {
     "b200ot_softmin_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32]),
     "b200ot_softmin_fwd": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, c_float, c_float, _P, _P, c_int64, c_int64,
                                      c_int32, c_int32, c_float, _P, c_int64, _P]),
+    "b200ot_softmin_pair_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32]),
+    "b200ot_softmin_fwd_pair": (c_int32, [_P, _P, _P, _P, c_float, _P, c_float, c_float, _P, _P, _P, _P, c_float, _P,
+                                          c_float, c_float, _P, _P, _P, c_int64, c_int64, c_int32, c_int32, c_float,
+                                          _P, c_int64, _P]),
     "b200ot_softmin_bwd_x": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32,
                                        c_float, _P, c_int64, _P]),
     "b200ot_plan_apply_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32, c_int64]),

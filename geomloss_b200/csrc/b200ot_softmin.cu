@@ -7,6 +7,11 @@
 #include "pack.cuh"
 #include "plan.cuh"
 #include "softmin.cuh"
+#include "softmin_pair.cuh"
+
+#include <string.h>
+
+#include <algorithm>
 
 namespace b200ot {
 
@@ -46,13 +51,24 @@ __global__ void softmin_merge_kernel(const float2* __restrict__ part, int n_part
   out[i] = ms.s > 0.0 ? make_float2(ms.m + (float)e, (float)frac) : make_float2(ms.m, 0.f);
 }
 
+// kFinPlain: the epilogue of every softmin.  kFinChecked: also sets *flag when a merged sum is not finite or leaves
+// [min_sum, 2^100] — the range in which the plan-scale sums of a paired softmin are exact (softmin_pair.cuh).
+// kFinGated: returns at once unless *flag is set (the recomputation of such a softmin on the unpaired path).
+enum { kFinPlain = 0, kFinChecked = 1, kFinGated = 2 };
+template <int MODE>
 __global__ void softmin_finalize_kernel(const float2* __restrict__ part, int n_part,
                                         const float* __restrict__ out_old, float alpha_old, float beta,
                                         float* __restrict__ out, float* __restrict__ lse2_out, int64_t N,
-                                        float neg_eps_ln2) {
+                                        float neg_eps_ln2, int* __restrict__ flag, double min_sum) {
+  if constexpr (MODE == kFinGated) {
+    if (*flag == 0) return;
+  }
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   const MergedMS ms = merge_ms(part, n_part, N, i);
+  if constexpr (MODE == kFinChecked) {
+    if (!(ms.s >= min_sum && ms.s <= 0x1p100)) *flag = 1;
+  }
   const double lse2 = (double)ms.m + log2(ms.s);
   if (lse2_out) lse2_out[i] = (float)lse2;
   if (out) {
@@ -123,10 +139,11 @@ static int launch_partial(const float* x, const float* center, float scale, floa
   static_assert(C::ROWS_PER_CTA == CR::ROWS_PER_CTA && C::TJ == CR::TJ, "dense and ranges instantiations share one ReducePlan");
   if (seg != nullptr)
     return launch_reduce<CR>(softmin_partial_kernel<CR, true>, pl, st, x, center, scale, clampq, cols,
-                             reinterpret_cast<float2*>(part), N, pl.ntiles, pl.tiles_per_split, 0, seg, pieces);
+                             reinterpret_cast<float2*>(part), N, pl.ntiles, pl.tiles_per_split, 0, seg, pieces,
+                             (const int*)nullptr);
   return launch_reduce<C>(softmin_partial_kernel<C, false>, pl, st, x, center, scale, clampq, cols,
                           reinterpret_cast<float2*>(part), N, pl.ntiles, pl.tiles_per_split, pl.last_pairs, seg,
-                          pieces);
+                          pieces, (const int*)nullptr);
 }
 
 template <int D>
@@ -146,14 +163,15 @@ static int partial_for_d(int p, const float* x, const float* center, float scale
 
 // `p` may carry B200OT_P_UNCLAMPED; M = number of column slots (gather mode: src maps slots to columns)
 int softmin_pack_impl(const float* y, const float* h_a, const float* h_b, float h_scale_b, const float* center,
-                      int64_t M, int D, int p, float eps, float* cols_out, cudaStream_t st, const int* src) {
+                      int64_t M, int D, int p, float eps, float* cols_out, cudaStream_t st, const int* src,
+                      const int* gate) {
   const int pe = p_exponent(p);
   const int nf2 = colfmt_nf2(D, 1);
   const int64_t mpad = round_up64(M, kPackPad);
   const int threads = 256;
   pack_cols_kernel<<<(unsigned)ceil_div64(mpad, threads), threads, 0, st>>>(
       y, h_a, h_b, h_scale_b, kLog2e, nullptr, center, softmin_coord_scale(pe, eps), pe == 1 ? 1 : 0, D, nf2, M,
-      mpad, cols_out, src);
+      mpad, cols_out, src, gate);
   B200OT_CUDA_TRY(cudaGetLastError());
   return B200OT_OK;
 }
@@ -176,6 +194,145 @@ static int softmin_partial_impl(const float* x, const float* center, const float
     case 8: return partial_for_d<8>(pe, x, center, scale, clampq, cols, part, pl, N, st, seg, pieces);
     default: return B200OT_EINVAL;
   }
+}
+
+// -------------------------------------------------------------------------------------------------
+// paired softmins (softmin_pair.cuh): D = 3, p = 2, the dense big plan
+// -------------------------------------------------------------------------------------------------
+// the epilogue arguments of one softmin (b200ot_softmin_finalize)
+struct SoftminOut {
+  const float* out_old;
+  float alpha_old, beta;
+  float* out;
+  float* lse2;
+};
+
+template <int MODE>
+static int finalize_launch(const float2* part, int n_part, const SoftminOut& o, int64_t N, float eps, int* flag,
+                           double min_sum, cudaStream_t st) {
+  const int threads = 256;
+  softmin_finalize_kernel<MODE><<<(unsigned)ceil_div64(N, threads), threads, 0, st>>>(
+      part, n_part, o.out_old, o.alpha_old, o.beta, o.out, o.lse2, N, -eps * kLn2, flag, min_sum);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// 8 rows per thread; the paired kernel fits 4 CTAs/SM in 96 registers, the symmetric one (its column and row-only
+// blocks in one body) needs 3 to stay free of spills
+using PairC = PairCfg<8, 128, 4>;
+using SymC = PairCfg<8, 128, 3>;
+
+// $B200OT_PAIR=0 (read on every call): every softmin takes the unpaired path, for A/B runs and tests
+static bool pair_on() {
+  const char* e = getenv("B200OT_PAIR");
+  return !(e && strcmp(e, "0") == 0);
+}
+
+// The shapes the paired kernels serve: what the unpaired path would run on softmin_partial_kernel's big plan
+static bool pair_shape(int64_t N, int64_t M, int D, int p) {
+  return D == 3 && p_exponent(p) == 2 && !make_plan(N, M, D).small && !tc_routed(kTcSoftminFwd, D, N, M) &&
+         !tc_routed(kTcSoftminFwd, D, M, N);
+}
+
+// Blocks of whole tiles along an axis of n points: as few tiles per block as keep the partial slots at 64 or fewer.
+// Test hook $B200OT_PAIR_TILES: at least that many tiles per block (1: many blocks at small sizes).
+static int pair_blocks(int64_t n) {
+  const int nt = (int)ceil_div64(n, PairC::TJ);
+  int tpb = (int)ceil_div64(nt, 64);
+  const char* e = getenv("B200OT_PAIR_TILES");
+  const int forced = e ? atoi(e) : 0;
+  if (forced > tpb) tpb = forced;
+  return (int)ceil_div64(nt, tpb);
+}
+
+// The unpaired path's scratch (b200ot_softmin_fwd at a shape the paired kernels serve)
+static int64_t unpaired_bytes(int64_t N, int64_t M) {
+  return round_up64(b200ot_packed_cols_floats(M, 3, 1) * 4, 256) +
+         round_up64((int64_t)make_plan(N, M, 3).n_split * N * 16, 256);
+}
+static int64_t packed_bytes(int64_t n) { return round_up64(b200ot_packed_cols_floats(n, 3, 1) * 4, 256); }
+// Scratch: the two range flags, then the region the paired pass uses and the recomputation reuses
+constexpr int64_t kPairFlagBytes = 256;
+static int64_t pair_bytes(int64_t N, int64_t M) {
+  const int64_t paired = packed_bytes(M) + packed_bytes(N) + round_up64((int64_t)pair_blocks(M) * N * 8, 256) +
+                         round_up64((int64_t)pair_blocks(N) * M * 8, 256);
+  return kPairFlagBytes + std::max(paired, std::max(unpaired_bytes(N, M), unpaired_bytes(M, N)));
+}
+static int64_t sym_bytes(int64_t N) {
+  const int64_t paired = packed_bytes(N) + round_up64((int64_t)pair_blocks(N) * N * 8, 256);
+  return kPairFlagBytes + std::max(paired, unpaired_bytes(N, N));
+}
+
+static bool overlaps(const void* a, int64_t na, const void* b, int64_t nb) {
+  if (!a || !b) return false;
+  const char *pa = (const char*)a, *pb = (const char*)b;
+  return pa < pb + nb * 4 && pb < pa + na * 4;
+}
+// an output of a softmin of N rows (columns: M points, column potential h_a, h_b) overlaps one of its inputs
+static bool out_aliases(const SoftminOut& o, int64_t N, const void* const* ins, const int64_t* lens, int nin) {
+  for (int k = 0; k < nin; ++k)
+    if (overlaps(o.out, N, ins[k], lens[k]) || overlaps(o.lse2, N, ins[k], lens[k])) return true;
+  return false;
+}
+
+// Today's pack -> partial -> finalize of one softmin (rows x, columns y), every launch returning at once unless *gate
+// is set: bit for bit what b200ot_softmin_fwd computes on the unpaired path
+static int softmin_fwd_gated(const float* x, const float* y, const float* h_a, const float* h_b, float h_scale_b,
+                             const float* center, int64_t N, int64_t M, float eps, const SoftminOut& o, void* region,
+                             int* gate, cudaStream_t st) {
+  using C = Variants<3, 2, false>::Big;
+  const ReducePlan pl = make_plan(N, M, 3);
+  float* cols = reinterpret_cast<float*>(region);
+  float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(region) + packed_bytes(M));
+  int rc = softmin_pack_impl(y, h_a, h_b, h_scale_b, center, M, 3, 2, eps, cols, st, nullptr, gate);
+  if (rc) return rc;
+  const float scale = softmin_coord_scale(2, eps);
+  rc = launch_reduce<C>(softmin_partial_kernel<C, false, true>, pl, st, x, center, scale, scale * scale * cost_clamp(2),
+                        (const float*)cols, reinterpret_cast<float2*>(part), N, pl.ntiles, pl.tiles_per_split,
+                        pl.last_pairs, (const int4*)nullptr, (const int2*)nullptr, (const int*)gate);
+  if (rc) return rc;
+  return finalize_launch<kFinGated>(reinterpret_cast<const float2*>(part), pl.n_split, o, N, eps, gate, 0.0, st);
+}
+
+// Softmin A (rows x, columns y, column potential hy) and, unless sym, softmin B (rows y, columns x, column potential
+// hx) from one pass; sym: x is y, hx is hy, one softmin.  Then the range check of every sum, and the gated
+// recomputation of a softmin that failed it.  Arguments validated by the caller; scratch >= pair_bytes / sym_bytes.
+static int pair_fwd(bool sym, const float* x, const float* y, const float* hy_a, const float* hy_b, float hy_s,
+                    const float* hx_a, const float* hx_b, float hx_s, const float* center, int64_t N, int64_t M,
+                    float eps, const SoftminOut& oa, const SoftminOut& ob, void* scratch, cudaStream_t st) {
+  int* flags = reinterpret_cast<int*>(scratch);
+  char* region = reinterpret_cast<char*>(scratch) + kPairFlagBytes;
+  const int nbr = pair_blocks(N), nbc = pair_blocks(M);
+  float* cols = reinterpret_cast<float*>(region);
+  float* rows = sym ? cols : reinterpret_cast<float*>(region + packed_bytes(M));
+  float2* part_a = reinterpret_cast<float2*>(region + packed_bytes(M) + (sym ? 0 : packed_bytes(N)));
+  float2* part_b = sym ? part_a : reinterpret_cast<float2*>(reinterpret_cast<char*>(part_a) +
+                                                              round_up64((int64_t)nbc * N * 8, 256));
+  B200OT_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(int), st));
+  int rc = softmin_pack_impl(y, hy_a, hy_b, hy_s, center, M, 3, 2, eps, cols, st, nullptr);
+  if (rc) return rc;
+  if (!sym) {
+    rc = softmin_pack_impl(x, hx_a, hx_b, hx_s, center, N, 3, 2, eps, rows, st, nullptr);
+    if (rc) return rc;
+  }
+  const int ntr = (int)ceil_div64(N, PairC::TJ), ntc = (int)ceil_div64(M, PairC::TJ);
+  static_assert(PairC::SMEM_BYTES == SymC::SMEM_BYTES && PairC::NT == SymC::NT, "one launch shape");
+  const auto kern = sym ? softmin_pair_kernel<SymC, true> : softmin_pair_kernel<PairC, false>;
+  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PairC::SMEM_BYTES));
+  const unsigned grid = sym ? (unsigned)(nbr * (nbr + 1) / 2) : (unsigned)(nbr * nbc);
+  kern<<<grid, PairC::NT + 32, PairC::SMEM_BYTES, st>>>(rows, cols, part_a, part_b, N, M, ntr, ntc, nbr, nbc);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  // a point's merged sum must stay within [count 2^-100, 2^100]: the terms flushed below 2^-126 then weigh less
+  // than 2^-26 of it (DESIGN.md §3.1b)
+  rc = finalize_launch<kFinChecked>(part_a, nbc, oa, N, eps, flags, (double)M * 0x1p-100, st);
+  if (rc) return rc;
+  if (!sym) {
+    rc = finalize_launch<kFinChecked>(part_b, nbr, ob, M, eps, flags + 1, (double)N * 0x1p-100, st);
+    if (rc) return rc;
+  }
+  rc = softmin_fwd_gated(x, y, hy_a, hy_b, hy_s, center, N, M, eps, oa, region, flags, st);
+  if (rc || sym) return rc;
+  return softmin_fwd_gated(y, x, hx_a, hx_b, hx_s, center, M, N, eps, ob, region, flags + 1, st);
 }
 
 }  // namespace b200ot
@@ -202,7 +359,8 @@ B200OT_API int64_t b200ot_softmin_scratch_bytes(int64_t N, int64_t M, int32_t D)
   const int64_t cols = b200ot_packed_cols_floats(M, D, 1) * 4;
   // forward partials are (m, s) pairs; the backward pass keeps D+1 sums per (split, row)
   const int64_t part = (int64_t)pl.n_split * N * 4 * (D + 1 > 2 ? D + 1 : 2);
-  const int64_t simt = round_up64(cols, 256) + round_up64(part, 256);
+  int64_t simt = round_up64(cols, 256) + round_up64(part, 256);
+  if (N == M && pair_shape(N, M, D, 2)) simt = std::max(simt, sym_bytes(N));  // x may be y: the symmetric kernel
   if (!tc_any_routed(D, N, M)) return simt;
   const int64_t tc = tc_scratch_bytes(N, M, D);
   return simt > tc ? simt : tc;
@@ -277,10 +435,9 @@ B200OT_API int b200ot_softmin_finalize(const float* part, int32_t n_part, const 
   if (!part || n_part <= 0 || N <= 0 || (!out && !lse2_out) || !(eps > 0.f)) return B200OT_EINVAL;
   if (((uintptr_t)part) & 7) return B200OT_EALIGN;
   const int threads = 256;
-  softmin_finalize_kernel<<<(unsigned)ceil_div64(N, threads), threads, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const float2*>(part), n_part, out_old, alpha_old, beta, out, lse2_out, N, -eps * kLn2);
-  B200OT_CUDA_TRY(cudaGetLastError());
-  return B200OT_OK;
+  return finalize_launch<kFinPlain>(reinterpret_cast<const float2*>(part), n_part,
+                                    SoftminOut{out_old, alpha_old, beta, out, lse2_out}, N, eps, nullptr, 0.0,
+                                    (cudaStream_t)stream);
 }
 
 B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h_a, const float* h_b,
@@ -295,16 +452,53 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
   if (tc)
     return tc_softmin_fwd(x, y, h_a, h_b, h_scale_b, center, out_old, alpha_old, beta, out, lse2_out, N, M, D, p, eps,
                           scratch, stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  const SoftminOut o{out_old, alpha_old, beta, out, lse2_out};
+  if (x == y && N == M && pair_on() && pair_shape(N, M, D, p)) {
+    // one exponential per unordered pair; refused when an output overlaps an input the recomputation would read
+    const void* ins[] = {x, h_a, h_b, center, out_old};
+    const int64_t lens[] = {N * D, N, N, D, N};
+    if (!out_aliases(o, N, ins, lens, 5) && !overlaps(out, N, lse2_out, N))
+      return pair_fwd(true, x, x, h_a, h_b, h_scale_b, h_a, h_b, h_scale_b, center, N, N, eps, o, o, scratch, st);
+  }
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) +
                                          round_up64(b200ot_packed_cols_floats(M, D, 1) * 4, 256));
-  cudaStream_t st = (cudaStream_t)stream;
   int rc = softmin_pack_impl(y, h_a, h_b, h_scale_b, center, M, D, p, eps, cols, st, nullptr);
   if (rc) return rc;
   rc = softmin_partial_impl(x, center, cols, part, pl, N, D, p, eps, st);
   if (rc) return rc;
   return b200ot_softmin_finalize(part, pl.n_split, out_old, alpha_old, beta, out, lse2_out, N, eps, stream);
+}
+
+B200OT_API int64_t b200ot_softmin_pair_scratch_bytes(int64_t N, int64_t M, int32_t D) {
+  if (N <= 0 || M <= 0 || !pair_shape(N, M, D, 2)) return 0;
+  return pair_bytes(N, M);
+}
+
+B200OT_API int b200ot_softmin_fwd_pair(const float* x, const float* y, const float* hy_a, const float* hy_b,
+                                       float hy_scale_b, const float* out_a_old, float alpha_a_old, float beta_a,
+                                       float* out_a, float* lse2_a, const float* hx_a, const float* hx_b,
+                                       float hx_scale_b, const float* out_b_old, float alpha_b_old, float beta_b,
+                                       float* out_b, float* lse2_b, const float* center, int64_t N, int64_t M,
+                                       int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                       void* stream) {
+  if (!x || !y || !hy_a || !hx_a || !scratch || N <= 0 || M <= 0 || !valid_p(p) || !(eps > 0.f) ||
+      (!out_a && !lse2_a) || (!out_b && !lse2_b) || !pair_shape(N, M, D, p))
+    return B200OT_EINVAL;
+  const SoftminOut oa{out_a_old, alpha_a_old, beta_a, out_a, lse2_a};
+  const SoftminOut ob{out_b_old, alpha_b_old, beta_b, out_b, lse2_b};
+  // the recomputation of a softmin reads every input after the finalize wrote the outputs: no output may overlap one
+  const void* ins[] = {x, y, hy_a, hy_b, hx_a, hx_b, center, out_a_old, out_b_old};
+  const int64_t lens[] = {N * D, M * D, M, M, N, N, D, N, M};
+  if (out_aliases(oa, N, ins, lens, 9) || out_aliases(ob, M, ins, lens, 9) || overlaps(out_a, N, lse2_a, N) ||
+      overlaps(out_b, M, lse2_b, M) || overlaps(out_a, N, out_b, M) || overlaps(out_a, N, lse2_b, M) ||
+      overlaps(lse2_a, N, out_b, M) || overlaps(lse2_a, N, lse2_b, M))
+    return B200OT_EINVAL;
+  if (const int rc = scratch_check(scratch, scratch_bytes, pair_bytes(N, M))) return rc;
+  return pair_fwd(false, x, y, hy_a, hy_b, hy_scale_b, hx_a, hx_b, hx_scale_b, center, N, M, eps, oa, ob, scratch,
+                  (cudaStream_t)stream);
 }
 
 }  // extern "C"

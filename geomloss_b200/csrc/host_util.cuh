@@ -38,7 +38,8 @@ inline float softmin_coord_scale(int p, float eps) {
 
 // Shared between translation units (defined in b200ot_softmin.cu).
 int softmin_pack_impl(const float* y, const float* h_a, const float* h_b, float h_scale_b, const float* center,
-                      int64_t M, int D, int p, float eps, float* cols_out, cudaStream_t st, const int* src);
+                      int64_t M, int D, int p, float eps, float* cols_out, cudaStream_t st, const int* src,
+                      const int* gate = nullptr);
 
 // ---- the tensor-core (wgmma) path, b200ot_tc.cu ----
 // The kernels serve any 1 <= D <= 64 (coordinates are zero-padded to a multiple of 16); above B200OT_MAX_D they are the

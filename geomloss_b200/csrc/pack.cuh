@@ -15,12 +15,15 @@ namespace b200ot {
 // Gather mode (src != null; ranges mode of the reductions): slot j holds column src[j] of the inputs, or a
 // neutral padding column when src[j] < 0 — this is how clusters / batch elements are aligned to chunk
 // boundaries without touching the caller's arrays.
+// gate != null: the pack returns at once unless *gate is set (the recomputation of a paired softmin, softmin_pair.cuh).
 // -------------------------------------------------------------------------------------------------
 static __global__ void pack_cols_kernel(const float* __restrict__ y, const float* __restrict__ h_a,
                                         const float* __restrict__ h_b, float h_scale_b, float h_scale,
                                         const float* __restrict__ w, const float* __restrict__ center, float scale,
                                         int direct, int D, int nf2, int64_t M, int64_t Mpad,
-                                        float* __restrict__ out, const int* __restrict__ src = nullptr) {
+                                        float* __restrict__ out, const int* __restrict__ src = nullptr,
+                                        const int* __restrict__ gate = nullptr) {
+  if (gate != nullptr && *gate == 0) return;
   const int64_t slot = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (slot >= Mpad) return;
   float* pk = out + (slot >> 1) * (int64_t)(nf2 * 2) + (slot & 1);

@@ -123,12 +123,18 @@ __device__ __forceinline__ void load_packet(const float4* __restrict__ tp, int p
 // RANGES = false: dense grid (row tiles x column splits).  RANGES = true: segments + pieces (b200ot.h, "ranges mode");
 // a separate instantiation so that the dense kernel — the headline path — carries none of its registers
 // (measured: 65 vs 72 registers, 245.2 vs 248.2 ms at N = M = 1e6 when the two shared one body).
-template <class C, bool RANGES>
+// GATED: the kernel returns at once unless *gate is set — the recomputation of a paired softmin whose sums left the
+// plan-scale range (softmin_pair.cuh), always enqueued.  The gate is the last parameter, so the other instantiations
+// keep their code.
+template <class C, bool RANGES, bool GATED = false>
 __global__ void __launch_bounds__(C::NT + 32, C::MINB)
     softmin_partial_kernel(const float* __restrict__ x, const float* __restrict__ center, float scale,
                            float clampq, const float* __restrict__ cols, float2* __restrict__ part, int64_t N,
                            int ntiles, int tiles_per_split, int last_pairs, const int4* __restrict__ seg,
-                           const int2* __restrict__ pieces) {
+                           const int2* __restrict__ pieces, const int* __restrict__ gate) {
+  if constexpr (GATED) {
+    if (*gate == 0) return;
+  }
   constexpr int D = C::D, R = C::R, NT = C::NT, NF2 = C::NF2, CH = C::CH, STAGES = C::STAGES;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   float* tiles = reinterpret_cast<float*>(smem_raw);

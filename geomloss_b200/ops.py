@@ -315,6 +315,104 @@ def softmin_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, ou
     return _softmin(_SOFTMIN, eps, x, y, h_a, h_b, h_scale_b, p, center, out_old, alpha_old, beta, out, want_lse2)
 
 
+# Two softmins of one Jacobi iteration that mirror each other (A's rows are B's columns and A's columns B's rows, same
+# eps, p and center) share their exponentials: b200ot_softmin_fwd_pair.  B200OT_PAIR=0, read on every call, runs every
+# call on its own (the library's symmetric xx / yy kernel follows the same switch).
+def _same(s, t):
+    """The same tensor data: one object, or views such as two ``.detach()`` of one cloud."""
+    if s is None or t is None:
+        return s is t
+    return s is t or (s.data_ptr() == t.data_ptr() and s.shape == t.shape and s.stride() == t.stride()
+                      and s.dtype == t.dtype and s.device == t.device)
+
+
+def _mirrors(a, b):
+    """Whether the ``softmin_raw`` calls ``a``, ``b`` (each ``(args, kwargs)``) can run as one paired launch group."""
+    (ea, xa, ya, *_), ka = a
+    (eb, xb, yb, *_), kb = b
+    if _same(xa, ya) or not _same(xa, yb) or not _same(ya, xb) or float(ea) != float(eb):
+        return False
+    if ka.get("p", 2) != 2 or kb.get("p", 2) != 2 or not _same(ka.get("center"), kb.get("center")):
+        return False
+    if xa.dim() != 2 or xa.shape[-1] != 3 or ya.dim() != 2 or ya.shape[-1] != 3:
+        return False
+    # the recomputation of a softmin whose sums leave the paired range reads every input after the outputs are written
+    ins = [t for args, kw in (a, b) for t in (*args[1:], kw.get("out_old"), kw.get("center")) if torch.is_tensor(t)]
+    outs = [o for o in (ka.get("out"), kb.get("out")) if o is not None]
+    shared = lambda s, t: s.untyped_storage().data_ptr() == t.untyped_storage().data_ptr()  # noqa: E731
+    return not any(shared(o, t) for o in outs for t in ins) and not (len(outs) == 2 and shared(*outs))
+
+
+def pair_plan(calls):
+    """The launch groups of ``softmin_raw_many(calls)``: ``(i, j)`` for two calls that run paired, ``(k,)`` for one
+    that runs alone, in the order of the first call of each group."""
+    plan, used = [], set()
+    for i in range(len(calls)):
+        if i in used:
+            continue
+        j = next((j for j in range(i + 1, len(calls)) if j not in used and _mirrors(calls[i], calls[j])), None)
+        if j is None:
+            plan.append((i,))
+        else:
+            plan.append((i, j))
+            used.add(j)
+    return plan
+
+
+def _softmin_pair(a, b):
+    """``softmin_raw(*a)`` and ``softmin_raw(*b)`` from one pass over the pairs (``_mirrors(a, b)`` holds), or None
+    when the library does not pair this shape."""
+    (eps, x, y, h_a, *ha_more), ka = a
+    (_, _, _, g_a, *hb_more), kb = b
+    h_b, h_scale_b = (ha_more + [None, 0.0])[:2]
+    g_b, g_scale_b = (hb_more + [None, 0.0])[:2]
+    p, center = ka.get("p", 2), ka.get("center")
+    (_, N, M, D), sizes, (x, y, h_a, h_b, g_a, g_b, out_a_old, out_a, out_b_old, out_b, center) = _inputs(
+        _SOFTMIN, p, x, y, ((h_a, "h_a"), (h_b, "h_b")), ((g_a, "h_a"), (g_b, "h_b"), (ka.get("out_old"), "out_old"),
+                                                          (ka.get("out"), "out")),
+        (kb.get("out_old"), "out_old"), (kb.get("out"), "out"), (center, "center"))
+    if (out_b_old is not None and out_b_old.numel() != M) or (out_b is not None and out_b.numel() != M):
+        raise ValueError(f"out_old / out of the columns' softmin must have {M} entries")
+    dev = x.device
+    nbytes = _query(dev, "b200ot_softmin_pair_scratch_bytes", N, M, D)
+    if nbytes == 0:
+        return None
+    for o, given in ((out_a, ka.get("out")), (out_b, kb.get("out"))):
+        if given is not None and (o is not given or given.device != dev):
+            raise ValueError(f"out must be contiguous and on {dev}, got strides {given.stride()} on {given.device}")
+    with nvtx_range("b200ot.softmin_pair N={} M={} D={} eps={:.3g}", N, M, D, float(eps)):
+        out_a = torch.empty(N, dtype=torch.float32, device=dev) if out_a is None else out_a
+        out_b = torch.empty(M, dtype=torch.float32, device=dev) if out_b is None else out_b
+        lse2_a = torch.empty(N, dtype=torch.float32, device=dev) if ka.get("want_lse2") else None
+        lse2_b = torch.empty(M, dtype=torch.float32, device=dev) if kb.get("want_lse2") else None
+        scratch = _scratch(nbytes, dev, "softmin_pair")
+        # two packs, the paired pass, two checked finalizes, and the gated pack, partial and finalize of each softmin
+        _call(dev, "b200ot_softmin_fwd_pair", x, y, h_a, h_b, float(h_scale_b), out_a_old, float(ka.get("alpha_old", 0.0)),
+              float(ka.get("beta", 1.0)), out_a, lse2_a, g_a, g_b, float(g_scale_b), out_b_old,
+              float(kb.get("alpha_old", 0.0)), float(kb.get("beta", 1.0)), out_b, lse2_b, center, N, M, D, int(p),
+              float(eps), scratch, scratch.numel(), launches=11)
+    return (out_a, lse2_a), (out_b, lse2_b)
+
+
+def softmin_raw_many(calls):
+    """``[softmin_raw(*args, **kw) for args, kw in calls]``, the mirrored calls of ``pair_plan(calls)`` paired."""
+    res = [None] * len(calls)
+    paired = _os.environ.get("B200OT_PAIR", "1") != "0"
+    for group in (pair_plan(calls) if paired else [(k,) for k in range(len(calls))]):
+        both = _softmin_pair(calls[group[0]], calls[group[1]]) if len(group) == 2 else None
+        if both is not None:
+            res[group[0]], res[group[1]] = both
+        else:
+            for k in group:
+                args, kw = calls[k]
+                res[k] = softmin_raw(*args, **kw)
+    return res
+
+
+# what sinkhorn.softmin_many looks up on the operator it is handed: the library's softmin_raw, not a stand-in for it
+softmin_raw.softmin_raw_many = softmin_raw_many
+
+
 def softmin_grad_rows(eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, *, p=2, center=None):
     """grad_x of <grad_out, softmin(eps, (x, y), h)> with y, h constant (b200ot_softmin_bwd_x)."""
     return _softmin_grad_rows(_SOFTMIN, eps, x, y, h_a, h_b, h_scale_b, lse2, grad_out, p, center)

@@ -61,9 +61,11 @@ def scaling_parameters(x, y, p, blur, reach, diameter, scaling):
 
 def softmin_many(sm, calls):
     """Run the independent softmins ``calls = [(args, kwargs), ...]`` of one Jacobi iteration through ``sm``; an engine
-    that can overlap their collectives (distributed.ColumnShardedEngine.softmin_raw_many) gets them all at once."""
+    that can overlap their collectives (distributed.ColumnShardedEngine.softmin_raw_many) gets them all at once, and
+    ``ops.softmin_raw`` runs mirrored calls (the xy and yx updates) as one paired launch group (ops.softmin_raw_many).
+    An operator that offers neither (an injected or recording one) gets the calls one by one."""
     owner = getattr(sm, "__self__", None)
-    many = getattr(owner, "softmin_raw_many", None) if owner is not None else None
+    many = getattr(sm if owner is None else owner, "softmin_raw_many", None)
     if many is not None:
         return many(calls)
     return [sm(*args, **kw) for args, kw in calls]

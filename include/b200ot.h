@@ -26,6 +26,8 @@
  *   B200OT_TC_MIN_D      "d" or "softmin_fwd,softmin_bwd,conv_fwd,conv_bwd": smallest D <= B200OT_MAX_D an operator
  *                        hands to the tensor-core kernels (default "7,9,5,9": forward softmin from 7, gaussian from 5)
  *   B200OT_TC_MIN_PAIRS  smallest N*M for that hand-over (default 8e8)
+ *   B200OT_PAIR          "0": b200ot_softmin_fwd never takes the symmetric kernel (see b200ot_softmin_fwd_pair)
+ *   B200OT_PAIR_TILES    test hook: at least this many 1024-point tiles per block of the paired kernels
  */
 #ifndef B200OT_H_
 #define B200OT_H_
@@ -94,6 +96,25 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
                        const float* center, const float* out_old, float alpha_old, float beta, float* out,
                        float* lse2_out, int64_t N, int64_t M, int32_t D, int32_t p, float eps, void* scratch,
                        int64_t scratch_bytes, void* stream);
+
+/* Two softmins of one Jacobi Sinkhorn iteration from one pass over the pairs: A (rows x, columns y, column potential
+ * hy_a + hy_scale_b * hy_b; out_a, lse2_a: N) and B (rows y, columns x, column potential hx_a + hx_scale_b * hx_b;
+ * out_b, lse2_b: M), each with the epilogue of b200ot_softmin_fwd.  One exponential 2^T_ij, T_ij = log2e (hx_i + hy_j -
+ * C_ij / eps), feeds row sum i of A and column sum j of B.  A softmin whose merged sums leave the range in which that
+ * is exact (a point's sum outside [count 2^-100, 2^100]: zero-weight points, potentials that move by tens of nats
+ * in one step) is recomputed on the path of b200ot_softmin_fwd, bit for bit, with no host synchronisation.
+ * D = 3, p = 2, and a shape b200ot_softmin_pair_scratch_bytes accepts; no output may overlap an input or another
+ * output (EINVAL).  b200ot_softmin_fwd takes the symmetric variant of this kernel by itself when x == y and N == M
+ * (each unordered pair evaluated once), unless $B200OT_PAIR=0.  Deterministic: no atomics on the sums.
+ * scratch: >= b200ot_softmin_pair_scratch_bytes(N, M, D), which is 0 for a shape the paired kernel does not serve. */
+B200OT_API int64_t b200ot_softmin_pair_scratch_bytes(int64_t N, int64_t M, int32_t D);
+B200OT_API int b200ot_softmin_fwd_pair(const float* x, const float* y, const float* hy_a, const float* hy_b,
+                                       float hy_scale_b, const float* out_a_old, float alpha_a_old, float beta_a,
+                                       float* out_a, float* lse2_a, const float* hx_a, const float* hx_b,
+                                       float hx_scale_b, const float* out_b_old, float alpha_b_old, float beta_b,
+                                       float* out_b, float* lse2_b, const float* center, int64_t N, int64_t M,
+                                       int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
+                                       void* stream);
 
 /* Gradient of the softmin w.r.t. the row cloud (the only gradient the reference's autograd
  * contract carries: columns and h are detached, sinkhorn_samples.py:179-185, sinkhorn_divergence.py:616-623):

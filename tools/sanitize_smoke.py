@@ -31,7 +31,7 @@ def check(name, got, ref, tol=2e-5):
     assert err < tol, name
 
 
-which = set(sys.argv[1:]) or {"softmin", "ranges", "conv", "tc", "batched", "l1", "wide", "blocks", "grid", "loss",
+which = set(sys.argv[1:]) or {"softmin", "pair", "ranges", "conv", "tc", "batched", "l1", "wide", "blocks", "grid", "loss",
                               "small", "apply", "apply_wide", "dense"}
 if "ring" in which:
     # the dense kernels with MANY tiles per CTA (B200OT_FORCE_SPLITS=1 in the environment): every stage of the TMA ring
@@ -74,6 +74,21 @@ if "softmin" in which:
         check("softmin_" + tag, out, ref_softmin(0.05, x, y, h, p))
         (gx,) = torch.autograd.grad(out.sum(), xg)
         assert torch.isfinite(gx).all()
+if "pair" in which:
+    # the paired kernels (softmin_pair.cuh): the xy / yx pair and the symmetric xx softmin, many blocks, ragged sizes
+    import os
+
+    os.environ["B200OT_PAIR_TILES"] = "1"
+    x, y = torch.rand(5000, 3, generator=g), torch.rand(6100, 3, generator=g)
+    hx, hy = torch.randn(5000, generator=g) * 0.1, torch.randn(6100, generator=g) * 0.1
+    xd, yd, hxd, hyd = x.to(DEV), y.to(DEV), hx.to(DEV), hy.to(DEV)
+    c = ops.default_center(xd, yd)
+    (fa, _), (fb, _) = ops.softmin_raw_many([((0.05, xd, yd, hyd), dict(p=2, center=c)),
+                                             ((0.05, yd, xd, hxd), dict(p=2, center=c))])
+    check("pair_xy", fa, ref_softmin(0.05, x, y, hy, 2))
+    check("pair_yx", fb, ref_softmin(0.05, y, x, hx, 2))
+    check("pair_xx", ops.softmin_raw(0.05, xd, xd, hxd, p=2, center=c)[0], ref_softmin(0.05, x, x, hx, 2))
+    del os.environ["B200OT_PAIR_TILES"]
 if "ranges" in which:
     for variant, n, m in ((ranges.SMALL, 900, 700), (ranges.BIG, 2500, 3000)):
         R = 5
