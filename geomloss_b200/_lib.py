@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("B200OT_LIB") or os.path.join(_PKG, "libb200ot.so")
 _lib = None
 
 _P = c_void_p  # device pointers and streams travel as void*
+_I32P, _F32P = ctypes.POINTER(c_int32), ctypes.POINTER(c_float)  # small host arrays (per-axis grid geometry)
 
 
 class B200OTError(RuntimeError):
@@ -127,6 +128,10 @@ _SIGNATURES = {
     "b200ot_kernel_mmd_bwd_small": (c_int32, [_P] * 7 + [c_int64, c_int64, c_int64, c_int32, c_int32, c_float, _P]),
     "b200ot_softmin_grid": (c_int32, [_P, _P, c_float, _P, c_float, c_float, _P, c_int64, c_int32, c_int32, c_int32,
                                       c_float, _P]),
+    "b200ot_softmin_grid_axes": (c_int32, [_P, _P, c_float, _P, c_float, c_float, _P, c_int64, c_int32, _I32P, _F32P,
+                                           _I32P, c_float, _P]),
+    "b200ot_grid_plan_apply": (c_int32, [_P, _P, c_float, _P, _P, _P, c_int64, c_int32, c_int32, _I32P, _F32P, _I32P,
+                                         c_float, _P]),
     "b200ot_ubench": (c_int32, [c_int32, c_int32, c_int32, _P, ctypes.POINTER(c_int32), _P]),
 }
 

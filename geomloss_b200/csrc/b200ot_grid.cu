@@ -15,6 +15,9 @@
 // and written back with the access pattern of the load, so passes run in place.
 // Work per pass: N^(dim+1) pairs -> SFU-bound like the point-cloud softmin (256^3: 4.3e9 pairs, ~1 ms);
 // HBM traffic 2 x 4 N^dim bytes per pass.
+// b200ot_softmin_grid_axes runs the same pass on grids with their own side, pitch and periodic flag per axis (the
+// PERIODIC instantiations), and b200ot_grid_plan_apply applies the plan of that softmin to K value channels
+// (grid_apply_kernel below): the operators of ot.solve_grid.
 #include <math.h>
 
 #include "b200ot.h"
@@ -39,7 +42,16 @@ struct GridPassArgs {
   int64_t outer, inner;
 };
 
-template <int P, int TW>
+// Offset n between two indices of an axis of side N: |n|, or the shorter way round min(|n|, N - |n|) on a periodic
+// axis.  Exact in fp32 for N <= 1024.
+template <bool PERIODIC>
+__device__ __forceinline__ float grid_offset(float n, float Nf) {
+  if (!PERIODIC) return n;
+  const float a = fabsf(n);
+  return fminf(a, Nf - a);
+}
+
+template <int P, int TW, bool PERIODIC>
 __global__ void __launch_bounds__(kGridWarps * 32) grid_pass_kernel(GridPassArgs A) {
   constexpr int kGridTW = TW, kGridRS = TW + 1, NSUB = 32 / TW;
   extern __shared__ float smem_f[];
@@ -117,7 +129,8 @@ __global__ void __launch_bounds__(kGridWarps * 32) grid_pass_kernel(GridPassArgs
       float2 W[14];
 #pragma unroll
       for (int k = -6; k <= 7; ++k) {
-        const float2 n = fadd2(base, make_float2((float)k, (float)(k - 1)));
+        float2 n = fadd2(base, make_float2((float)k, (float)(k - 1)));
+        if constexpr (PERIODIC) n = make_float2(grid_offset<true>(n.x, (float)N), grid_offset<true>(n.y, (float)N));
         if (P == 2) {
           W[k + 6] = fmul2(fmul2(n, n), dup2(kq));
         } else {
@@ -140,7 +153,7 @@ __global__ void __launch_bounds__(kGridWarps * 32) grid_pass_kernel(GridPassArgs
           float cm = -INFINITY;
 #pragma unroll
           for (int c = 0; c < 8; ++c) {
-            const float n = (float)(ib + r - j0 - c);
+            const float n = grid_offset<PERIODIC>((float)(ib + r - j0 - c), (float)N);
             const float av = (c & 1) ? a2[c >> 1].y : a2[c >> 1].x;
             t[c] = av + kq * ((P == 2) ? n * n : fabsf(n));
             cm = fmaxf(cm, t[c]);
@@ -189,6 +202,198 @@ __global__ void __launch_bounds__(kGridWarps * 32) grid_pass_kernel(GridPassArgs
   }
 }
 
+// ---- the plan applied to K value channels ------------------------------------------------------------------------
+// Each pixel carries a state (l, s_1..s_K): weight 2^l and weighted mean s.  A pass along one axis maps it to
+//     l'_i = log2 sum_j 2^(l_j - c(i, j)),      s'_i = sum_j 2^(l_j - c(i, j)) s_j / 2^(l'_i),
+// c the log2-domain cost of that axis.  The Gaussian kernel factorises over the axes, so after one pass per axis l is
+// the log2-sum of the full grid softmin and s the full conditional mean sum_j w_ij V_j / sum_j w_ij; every
+// intermediate s is a convex combination of V, bounded by max |V| whatever the signs.  A slab of up to kGridApplyKS
+// channels per launch: the pair's one MUFU.EX2 feeds the denominator and one FMA per channel; all of them share the
+// lazy max and its 2^64 rebase of grid_pass_kernel.  Inputs (l and the slab's channels of all TW lines) are staged in
+// shared memory; outputs are stored straight from registers, which keeps the tile at (1 + K) N (TW + 1) floats and
+// lets the pass run in place (the CTA has read all of its lines before any store).
+constexpr int kGridApplyKS = 4;
+
+struct GridApplyArgs {
+  const float* h_a;  // first pass: l = log2(e) (h_a + h_scale_b h_b); later passes read `ell` in place
+  const float* h_b;  // nullable
+  const float* v;    // first pass: channel k of the slab at v[k * vstride + pixel]; later passes read `s` in place
+  float* ell;
+  float* s;
+  float h_scale_b, xscale;
+  int N, nk, first;
+  int64_t outer, inner, vstride;
+};
+
+template <int TW, bool PERIODIC>
+__global__ void __launch_bounds__(kGridWarps * 32) grid_apply_kernel(GridApplyArgs A) {
+  constexpr int RS = TW + 1, NSUB = 32 / TW, KS = kGridApplyKS;
+  extern __shared__ float smem_f[];
+  const int N = A.N, nk = A.nk;
+  float* tile = smem_f;          // [N][RS] log2 weights
+  float* vtile = smem_f + N * RS;  // [nk][N][RS] means
+  const int lane = (threadIdx.x & 31) % TW, warp = (threadIdx.x >> 5) * NSUB + (threadIdx.x & 31) / TW;
+  const bool last_axis = (A.inner == 1);
+  int64_t o, w0;
+  int nw;
+  if (last_axis) {
+    o = (int64_t)blockIdx.x * TW;
+    w0 = 0;
+    nw = (int)min((int64_t)TW, A.outer - o);
+  } else {
+    const int64_t tiles_in = (A.inner + TW - 1) / TW;
+    o = blockIdx.x / tiles_in;
+    w0 = (blockIdx.x % tiles_in) * TW;
+    nw = (int)min((int64_t)TW, A.inner - w0);
+  }
+  auto index = [&](int j, int w) -> int64_t {
+    return last_axis ? ((o + w) * N + j) : ((o * N + j) * A.inner + w0 + w);
+  };
+
+  for (int idx = threadIdx.x; idx < N * TW; idx += blockDim.x) {
+    const int j = last_axis ? idx % N : idx / TW, w = last_axis ? idx / N : idx % TW;
+    float l = -INFINITY;
+    if (w < nw) {
+      const int64_t gi = index(j, w);
+      if (A.first) {
+        l = A.h_a[gi];
+        if (A.h_b) l = fmaf(A.h_scale_b, A.h_b[gi], l);
+        l *= kLog2e;
+      } else {
+        l = A.ell[gi];
+      }
+    }
+    tile[j * RS + w] = l;
+    const float* src = A.first ? A.v : A.s;
+    for (int k = 0; k < nk; ++k) vtile[(k * N + j) * RS + w] = (w < nw) ? src[k * A.vstride + index(j, w)] : 0.f;
+  }
+  __syncthreads();
+
+  const float kq = -A.xscale * A.xscale, Nf = (float)N;
+  const int per_warp = (N + kGridWarps * NSUB - 1) / (kGridWarps * NSUB);
+  const int i_end = min(N, (warp + 1) * per_warp);
+  int kk[KS];  // channel tile read for slab slot k (the last live one for the dead slots: their sums are discarded)
+#pragma unroll
+  for (int k = 0; k < KS; ++k) kk[k] = min(k, nk - 1) * N * RS;
+  for (int ib = warp * per_warp; ib < i_end; ib += kGridR) {
+    float m[kGridR], den[kGridR], num[kGridR][KS];
+#pragma unroll
+    for (int r = 0; r < kGridR; ++r) {
+      m[r] = (ib + r < N) ? fmaxf(tile[(ib + r) * RS + lane], kNegBig) : kNegBig;  // the j = i term, as above
+      den[r] = 0.f;
+#pragma unroll
+      for (int k = 0; k < KS; ++k) num[r][k] = 0.f;
+    }
+    for (int j0 = 0; j0 < N; j0 += 8) {
+      float a[8], v[8][KS];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const bool in = (j0 + c < N);
+        a[c] = in ? tile[(j0 + c) * RS + lane] : -INFINITY;
+#pragma unroll
+        for (int k = 0; k < KS; ++k) v[c][k] = in ? vtile[kk[k] + (j0 + c) * RS + lane] : 0.f;
+      }
+      float W[15];  // -c(i, j) for the offsets n = (ib - j0) + t, t = r - c in [-7, 7]
+#pragma unroll
+      for (int t = -7; t <= 7; ++t) {
+        const float n = grid_offset<PERIODIC>((float)(ib - j0 + t), Nf);
+        W[t + 7] = (n * n) * kq;
+      }
+#pragma unroll
+      for (int r = 0; r < kGridR; ++r) {
+        float e[8], cs = 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          e[c] = ex2_approx((a[c] + W[r - c + 7]) - m[r]);
+          cs += e[c];
+        }
+        if (!(cs <= 1.8446744e19f)) {
+          // outdated max: rebase the denominator and the numerators on this chunk's max and redo it
+          float cm = -INFINITY;
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            e[c] = a[c] + W[r - c + 7];
+            cm = fmaxf(cm, e[c]);
+          }
+          cs = 0.f;
+          if (cm > kNegBig) {
+            const float sc = ex2_approx(m[r] - cm);
+            den[r] *= sc;
+#pragma unroll
+            for (int k = 0; k < KS; ++k) num[r][k] *= sc;
+            m[r] = cm;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+              e[c] = ex2_approx(e[c] - cm);
+              cs += e[c];
+            }
+          } else {
+#pragma unroll
+            for (int c = 0; c < 8; ++c) e[c] = 0.f;  // every input of the chunk is -inf
+          }
+        }
+        den[r] += cs;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+#pragma unroll
+          for (int k = 0; k < KS; ++k) num[r][k] = fmaf(e[c], v[c][k], num[r][k]);
+        }
+      }
+    }
+    if (lane < nw) {
+#pragma unroll
+      for (int r = 0; r < kGridR; ++r) {
+        const int i = ib + r;
+        if (i < i_end) {
+          const int64_t gi = index(i, lane);
+          int ex = 0;
+          const float f = frexpf(den[r], &ex);
+          const bool live = den[r] > 0.f;
+          A.ell[gi] = live ? (m[r] + (float)ex) + log2f(f) : -INFINITY;
+#pragma unroll
+          for (int k = 0; k < KS; ++k)
+            if (k < nk) A.s[k * A.vstride + gi] = live ? num[r][k] / den[r] : 0.f;
+        }
+      }
+    }
+  }
+}
+
+// ---- host: per-axis geometry --------------------------------------------------------------------------------------
+// sides[d] in 1..1024, pitch[d] > 0 (finite), periodic[d] (nullable: no periodic axis), d < dim in 1..3; fills the
+// element count of the whole batch.
+static bool grid_geometry_ok(int64_t batch, int32_t dim, const int32_t* sides, const float* pitch, float eps,
+                             int64_t* total) {
+  if (batch <= 0 || dim < 1 || dim > 3 || !sides || !pitch || !(eps > 0.f) || !(eps < INFINITY)) return false;
+  *total = batch;
+  for (int d = 0; d < dim; ++d) {
+    if (sides[d] < 1 || sides[d] > 1024 || !(pitch[d] > 0.f) || !(pitch[d] < INFINITY)) return false;
+    *total *= sides[d];
+  }
+  return true;
+}
+
+static bool overlaps(const void* p, int64_t p_bytes, const void* q, int64_t q_bytes) {
+  if (!p || !q) return false;
+  const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
+  return a < b + (uintptr_t)q_bytes && b < a + (uintptr_t)p_bytes;
+}
+
+// The view [outer][N_axis][inner] of a (batch, sides...) tensor and the CTA count of a pass over it with TW lines.
+struct GridPass {
+  int32_t N;
+  int64_t outer, inner, blocks;
+};
+static GridPass grid_pass_shape(int64_t total, int32_t dim, const int32_t* sides, int axis, int tw) {
+  GridPass g;
+  g.N = sides[axis];
+  g.inner = 1;
+  for (int d = axis + 1; d < dim; ++d) g.inner *= sides[d];
+  g.outer = total / ((int64_t)g.N * g.inner);
+  g.blocks = (g.inner == 1) ? ceil_div64(g.outer, tw) : g.outer * ceil_div64(g.inner, tw);
+  return g;
+}
+
 }  // namespace b200ot
 
 using namespace b200ot;
@@ -209,8 +414,8 @@ B200OT_API int b200ot_softmin_grid(const float* h_a, const float* h_b, float h_s
   const float xscale = (p == 2 ? sqrtf(kLog2e / (2.0f * eps)) : kLog2e / eps) / (float)N;
   const int tw = ((size_t)2 * N * (kGridTW + 1) * sizeof(float) <= 227 * 1024) ? kGridTW : 16;
   const size_t smem = (size_t)2 * N * (tw + 1) * sizeof(float);
-  auto kern = (tw == kGridTW) ? ((p == 2) ? grid_pass_kernel<2, kGridTW> : grid_pass_kernel<1, kGridTW>)
-                              : ((p == 2) ? grid_pass_kernel<2, 16> : grid_pass_kernel<1, 16>);
+  auto kern = (tw == kGridTW) ? ((p == 2) ? grid_pass_kernel<2, kGridTW, false> : grid_pass_kernel<1, kGridTW, false>)
+                              : ((p == 2) ? grid_pass_kernel<2, 16, false> : grid_pass_kernel<1, 16, false>);
   B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // pass order of the reference: last axis first, then the others (the passes commute mathematically)
   for (int k = 0; k < dim; ++k) {
@@ -236,6 +441,99 @@ B200OT_API int b200ot_softmin_grid(const float* h_a, const float* h_b, float h_s
     const int64_t blocks = (inner == 1) ? ceil_div64(a.outer, tw) : a.outer * ceil_div64(inner, tw);
     kern<<<(unsigned)blocks, kGridWarps * 32, smem, st>>>(a);
     B200OT_CUDA_TRY(cudaGetLastError());
+  }
+  return B200OT_OK;
+}
+
+B200OT_API int b200ot_softmin_grid_axes(const float* h_a, const float* h_b, float h_scale_b, const float* out_old,
+                                        float alpha_old, float beta, float* out, int64_t batch, int32_t dim,
+                                        const int32_t* sides, const float* pitch, const int32_t* periodic, float eps,
+                                        void* stream) {
+  int64_t total = 0;
+  if (!h_a || !out || !grid_geometry_ok(batch, dim, sides, pitch, eps, &total)) return B200OT_EINVAL;
+  const int64_t bytes = total * (int64_t)sizeof(float);
+  if (overlaps(out, bytes, h_a, bytes) || overlaps(out, bytes, h_b, bytes) || overlaps(out, bytes, out_old, bytes))
+    return B200OT_EINVAL;  // passes run in place on `out`
+  cudaStream_t st = (cudaStream_t)stream;
+  const float xs = sqrtf(kLog2e / (2.0f * eps));  // log2-domain exponent - (xs h n)^2 for an offset of n pixels
+  for (int k = 0; k < dim; ++k) {
+    const int axis = dim - 1 - k;  // last axis first, as b200ot_softmin_grid
+    const int N = sides[axis];
+    const int tw = ((size_t)2 * N * (kGridTW + 1) * sizeof(float) <= 227 * 1024) ? kGridTW : 16;
+    const size_t smem = (size_t)2 * N * (tw + 1) * sizeof(float);
+    const bool per = periodic && periodic[axis];
+    auto kern = (tw == kGridTW) ? (per ? grid_pass_kernel<2, kGridTW, true> : grid_pass_kernel<2, kGridTW, false>)
+                                : (per ? grid_pass_kernel<2, 16, true> : grid_pass_kernel<2, 16, false>);
+    B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const GridPass g = grid_pass_shape(total, dim, sides, axis, tw);
+    GridPassArgs a;
+    a.h_a = h_a;
+    a.h_b = h_b;
+    a.out_old = out_old;
+    a.out = out;
+    a.h_scale_b = h_scale_b;
+    a.in_scale = kLog2e;
+    a.alpha_old = alpha_old;
+    a.beta = beta;
+    a.out_scale = -eps * kLn2;
+    a.xscale = xs * pitch[axis];
+    a.N = N;
+    a.first = (k == 0);
+    a.last = (k == dim - 1);
+    a.outer = g.outer;
+    a.inner = g.inner;
+    kern<<<(unsigned)g.blocks, kGridWarps * 32, smem, st>>>(a);
+    B200OT_CUDA_TRY(cudaGetLastError());
+  }
+  return B200OT_OK;
+}
+
+B200OT_API int b200ot_grid_plan_apply(const float* h_a, const float* h_b, float h_scale_b, const float* v, float* ell,
+                                      float* s, int64_t batch, int32_t K, int32_t dim, const int32_t* sides,
+                                      const float* pitch, const int32_t* periodic, float eps, void* stream) {
+  int64_t total = 0;
+  if (!h_a || !v || !ell || !s || K <= 0 || !grid_geometry_ok(batch, dim, sides, pitch, eps, &total))
+    return B200OT_EINVAL;
+  const int64_t bytes = total * (int64_t)sizeof(float), vbytes = bytes * K;
+  for (const void* in : {(const void*)h_a, (const void*)h_b}) {
+    if (overlaps(ell, bytes, in, bytes) || overlaps(s, vbytes, in, bytes)) return B200OT_EINVAL;
+  }
+  if (overlaps(ell, bytes, v, vbytes) || overlaps(s, vbytes, v, vbytes) || overlaps(ell, bytes, s, vbytes))
+    return B200OT_EINVAL;  // passes run in place on `ell` and `s`
+  cudaStream_t st = (cudaStream_t)stream;
+  const float xs = sqrtf(kLog2e / (2.0f * eps));
+  // one chain of `dim` passes per slab: every chain recomputes the same l from h (bit for bit), so l needs no copy
+  for (int32_t k0 = 0; k0 < K; k0 += kGridApplyKS) {
+    const int nk = min(kGridApplyKS, K - k0);
+    for (int k = 0; k < dim; ++k) {
+      const int axis = dim - 1 - k;
+      const int N = sides[axis];
+      auto bytes_for = [&](int tw) { return (size_t)(1 + nk) * N * (tw + 1) * sizeof(float); };
+      const int tw = bytes_for(32) <= 227 * 1024 ? 32 : bytes_for(16) <= 227 * 1024 ? 16 : 8;
+      const size_t smem = bytes_for(tw);
+      const bool per = periodic && periodic[axis];
+      auto kern = (tw == 32) ? (per ? grid_apply_kernel<32, true> : grid_apply_kernel<32, false>)
+                  : (tw == 16) ? (per ? grid_apply_kernel<16, true> : grid_apply_kernel<16, false>)
+                               : (per ? grid_apply_kernel<8, true> : grid_apply_kernel<8, false>);
+      B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      const GridPass g = grid_pass_shape(total, dim, sides, axis, tw);
+      GridApplyArgs a;
+      a.h_a = h_a;
+      a.h_b = h_b;
+      a.v = v + k0 * total;
+      a.ell = ell;
+      a.s = s + k0 * total;
+      a.h_scale_b = h_scale_b;
+      a.xscale = xs * pitch[axis];
+      a.N = N;
+      a.nk = nk;
+      a.first = (k == 0);
+      a.outer = g.outer;
+      a.inner = g.inner;
+      a.vstride = total;
+      kern<<<(unsigned)g.blocks, kGridWarps * 32, smem, st>>>(a);
+      B200OT_CUDA_TRY(cudaGetLastError());
+    }
   }
   return B200OT_OK;
 }

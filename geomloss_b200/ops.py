@@ -751,6 +751,63 @@ def dense_softmin_rows_grad(eps, C, log_w, pot, lse2, go):
     return grad_C
 
 
+# ------------------------------------------------------------------------------------------------
+# regular grids with their own side, pitch and periodicity per axis (b200ot_softmin_grid_axes, b200ot_grid_plan_apply,
+# csrc/b200ot_grid.cu): one launch per axis, one chain of them per slab of GRID_APPLY_SLAB value channels
+# ------------------------------------------------------------------------------------------------
+GRID_MAX_SIDE = 1024
+GRID_APPLY_SLAB = 4  # kGridApplyKS: value channels per launch of b200ot_grid_plan_apply
+
+
+def _grid_geometry(shape, pitch, periodic):
+    """(batch, dim, sides, pitch, periodic) of a (B, *grid) tensor as the host arrays of the grid entries."""
+    dim = len(shape) - 1
+    if not 1 <= dim <= 3 or len(pitch) != dim or len(periodic) != dim:
+        raise ValueError(f"expected a (B, N1[, N2[, N3]]) grid with one pitch and one periodic flag per axis; got "
+                         f"{tuple(shape)}, pitch {tuple(pitch)}, periodic {tuple(periodic)}")
+    if any(not 1 <= n <= GRID_MAX_SIDE for n in shape[1:]):
+        raise ValueError(f"grid sides must be in 1..{GRID_MAX_SIDE}, got {tuple(shape[1:])}")
+    return (shape[0], dim, (ctypes.c_int32 * dim)(*shape[1:]), (ctypes.c_float * dim)(*map(float, pitch)),
+            (ctypes.c_int32 * dim)(*(int(bool(p)) for p in periodic)))
+
+
+def softmin_grid_axes_raw(eps, h_a, h_b=None, h_scale_b=0.0, *, pitch, periodic, out_old=None, alpha_old=0.0,
+                          beta=1.0):
+    """``alpha_old out_old + beta (-eps log sum_j exp(h_j - |x_i - x_j|^2 / (2 eps)))`` over a (B, *grid) grid with
+    pixel pitch ``pitch[d]`` and wrap-around on the axes where ``periodic[d]``; h = h_a + h_scale_b h_b.
+    No autograd."""
+    h_a, h_b, out_old = _f32c(h_a, "h_a"), _f32c(h_b, "h_b"), _f32c(out_old, "out_old")
+    for t, name in ((h_b, "h_b"), (out_old, "out_old")):
+        if t is not None and (t.shape != h_a.shape or t.device != h_a.device):
+            raise ValueError(f"{name} must match h_a ({tuple(h_a.shape)} on {h_a.device}), got {tuple(t.shape)}")
+    B, dim, sides, pitch_c, periodic_c = _grid_geometry(h_a.shape, pitch, periodic)
+    dev = h_a.device
+    with nvtx_range("b200ot.softmin_grid_axes shape={} eps={:.3g}", tuple(h_a.shape), float(eps)):
+        out = torch.empty_like(h_a)
+        _call(dev, "b200ot_softmin_grid_axes", h_a, h_b, float(h_scale_b), out_old, float(alpha_old), float(beta), out,
+              B, dim, sides, pitch_c, periodic_c, float(eps), launches=dim)
+    return out
+
+
+def grid_plan_apply_raw(eps, h_a, h_b, h_scale_b, v, *, pitch, periodic):
+    """The weights ``w_ij = exp(h_j - |x_i - x_j|^2 / (2 eps))`` of that softmin applied to K channels, v (K, B, *grid)
+    channel-major: returns ``(ell, s)`` with ``ell = log2 sum_j w_ij`` (B, *grid) and ``s = sum_j w_ij v_j / sum_j
+    w_ij`` (K, B, *grid), s = 0 where every weight is 0.  No autograd."""
+    h_a, h_b, v = _f32c(h_a, "h_a"), _f32c(h_b, "h_b"), _f32c(v, "v")
+    if h_b is not None and (h_b.shape != h_a.shape or h_b.device != h_a.device):
+        raise ValueError(f"h_b must match h_a ({tuple(h_a.shape)} on {h_a.device}), got {tuple(h_b.shape)}")
+    if v.dim() != h_a.dim() + 1 or v.shape[1:] != h_a.shape or v.shape[0] == 0 or v.device != h_a.device:
+        raise ValueError(f"v must be (K, *h_a.shape) = (K, {', '.join(map(str, h_a.shape))}) with K >= 1 on "
+                         f"{h_a.device}, got {tuple(v.shape)}")
+    B, dim, sides, pitch_c, periodic_c = _grid_geometry(h_a.shape, pitch, periodic)
+    K, dev = v.shape[0], h_a.device
+    with nvtx_range("b200ot.grid_plan_apply shape={} K={} eps={:.3g}", tuple(h_a.shape), K, float(eps)):
+        ell, s = torch.empty_like(h_a), torch.empty_like(v)
+        _call(dev, "b200ot_grid_plan_apply", h_a, h_b, float(h_scale_b), v, ell, s, B, K, dim, sides, pitch_c,
+              periodic_c, float(eps), launches=dim * -(-K // GRID_APPLY_SLAB))
+    return ell, s
+
+
 # which operators serve which clouds: the one place that compares D with MAX_D / MAX_D_TC.  The operators are module
 # globals read at every call, so a replaced operator is the one returned.
 def softmin_operators(D, p=2, batched=False):

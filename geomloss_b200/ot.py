@@ -1,4 +1,5 @@
-"""``geomloss.ot.solve_sample``, ``solve`` and ``solve_batch`` over the CUDA kernels (SURVEY.md section 8, row f-3).
+"""``geomloss.ot.solve_sample``, ``solve``, ``solve_batch`` and ``solve_grid`` over the CUDA kernels (SURVEY.md
+section 8, row f-3; ``solve_grid`` and its result object are at the end of this file).
 
 The reference's "new API" for point clouds (src/geomloss/ot/_implementations/sample.py:190-395) builds dense (N, M)
 cost matrices and runs ``sinkhorn_loop`` (ot/_abstract_solvers/sinkhorn_ot.py:240-447) on them.  Here the same
@@ -37,8 +38,8 @@ import torch
 from . import ops
 from .sinkhorn import log_weights, max_diameter
 
-__all__ = ["solve", "solve_batch", "solve_sample", "solve_sample_batch", "OTResultMatrix", "OTResultSample",
-           "LinearOperator"]
+__all__ = ["solve", "solve_batch", "solve_grid", "solve_sample", "solve_sample_batch", "OTResultGrid",
+           "OTResultMatrix", "OTResultSample", "LinearOperator"]
 
 _DENSE_LIMIT = 1 << 27  # entries of a dense (N, M) plan we are willing to materialise on request
 
@@ -722,3 +723,281 @@ class OTResultMatrix:
         for k in ("value", "_marginals", "marginal_a", "marginal_b", "density", "plan", "density_operator",
                   "plan_operator"):
             self.__dict__.pop(k, None)
+
+
+# ----------------------------------------------------------------------------------------------------
+# regular grids (images, volumes)                       ot/_implementations/grid.py:215-242 (a stub there)
+# ----------------------------------------------------------------------------------------------------
+class _Grid:
+    """The pixel grid shared by ``a`` and ``b``: side N_d, extent [lo_d, hi_d), pitch h_d = (hi_d - lo_d) / N_d and
+    pixel centres lo_d + (k + 1/2) h_d on every axis d; offsets on a periodic axis go the shorter way round."""
+
+    def __init__(self, sides, axes, periodic):
+        self.sides, self.D = tuple(int(n) for n in sides), len(sides)
+        D = self.D
+        if axes is None:
+            pairs = [(0.0, 1.0)] * D
+        elif torch.is_tensor(axes) or isinstance(axes, np.ndarray) or (
+                isinstance(axes, (tuple, list)) and any(torch.is_tensor(t) or isinstance(t, np.ndarray) for t in axes)):
+            raise NotImplementedError("solve_grid serves uniform grids given by (lo, hi) extents; explicit pixel "
+                                      "coordinates (non-uniform spacing) are not supported.")
+        elif isinstance(axes, (tuple, list)) and len(axes) == 2 and all(_is_real(t) for t in axes):
+            pairs = [tuple(axes)] * D
+        elif (isinstance(axes, (tuple, list)) and len(axes) == D
+              and all(isinstance(t, (tuple, list)) and len(t) == 2 and all(_is_real(u) for u in t) for t in axes)):
+            pairs = [tuple(t) for t in axes]
+        else:
+            raise ValueError(f"'axes' should be None, one (lo, hi) pair for every axis or a tuple of {D} (lo, hi) "
+                             f"pairs, one per axis. Received {axes!r}.")
+        for lo, hi in pairs:
+            if not (math.isfinite(lo) and math.isfinite(hi) and hi > lo):
+                raise ValueError(f"Every axis extent (lo, hi) should satisfy lo < hi. Received {(lo, hi)}.")
+        if isinstance(periodic, (bool, np.bool_)):
+            periodic = (bool(periodic),) * D
+        elif not (isinstance(periodic, (tuple, list)) and len(periodic) == D
+                  and all(isinstance(t, (bool, np.bool_)) for t in periodic)):
+            raise ValueError(f"'periodic' should be a bool or a tuple of {D} bools, one per axis. Received "
+                             f"{periodic!r}.")
+        self.lo = tuple(float(lo) for lo, _ in pairs)
+        self.pitch = tuple((float(hi) - float(lo)) / n for (lo, hi), n in zip(pairs, self.sides))
+        self.periodic = tuple(bool(t) for t in periodic)
+
+    @property
+    def diameter(self):
+        """Diagonal of the box of pixel centres; half the side on a periodic axis, its largest offset."""
+        ext = [(n // 2 if per else n - 1) * h for n, h, per in zip(self.sides, self.pitch, self.periodic)]
+        return math.sqrt(sum(e * e for e in ext))
+
+    def center(self, d):
+        return self.lo[d] + 0.5 * self.sides[d] * self.pitch[d]
+
+    def coords(self, d, device):
+        """(N_d,) fp64 pixel centres of axis d, relative to the middle of the axis."""
+        k = torch.arange(self.sides[d], dtype=torch.float64, device=device)
+        return (k + 0.5 - 0.5 * self.sides[d]) * self.pitch[d]
+
+    def axis_cost(self, d, device):
+        """(N_d, N_d) fp64 squared distances along axis d."""
+        k = torch.arange(self.sides[d], dtype=torch.float64, device=device)
+        n = (k[:, None] - k[None, :]).abs()
+        if self.periodic[d]:
+            n = torch.minimum(n, self.sides[d] - n)
+        return (n * self.pitch[d]) ** 2
+
+    def _along(self, t, d):
+        """(B, N_d) -> (B, 1, .., N_d, .., 1), broadcastable over the grid."""
+        shape = [t.shape[0]] + [1] * self.D
+        shape[1 + d] = self.sides[d]
+        return t.reshape(shape)
+
+    def points(self, device):
+        """(P, D) fp32 pixel centres in the order of a flattened grid."""
+        cs = torch.meshgrid(*[self.coords(d, device) + self.center(d) for d in range(self.D)], indexing="ij")
+        return torch.stack([c.reshape(-1) for c in cs], 1).float()
+
+    def cost(self, device):
+        """(P, P) fp64 cost matrix sum_d dist_d^2 between pixels (small grids only)."""
+        idx = torch.meshgrid(*[torch.arange(n, device=device) for n in self.sides], indexing="ij")
+        return sum(self.axis_cost(d, device)[k.reshape(-1)][:, k.reshape(-1)] for d, k in enumerate(idx))
+
+    def at_infinity(self, w_rows, w_cols, damp):
+        """eps = +inf: f_i = sum_j w_j C_ij / sum_j w_j, separably in fp64 (sum_d of the axis cost applied to the axis
+        marginal of w), then the per-point offset and dampening of ``_Softmin.at_infinity``."""
+        w = w_cols.double()
+        dims = tuple(range(1, self.D + 1))
+        W = w.sum(dims)
+        f = torch.zeros_like(w)
+        for d in range(self.D):
+            other = tuple(e for e in dims if e != 1 + d)
+            m = w.sum(other) if other else w  # (B, N_d) marginal along axis d
+            fd = (m[:, None, :] * self.axis_cost(d, w.device)[None]).sum(-1)  # one row reduction per output
+            f = f + self._along(fd / W[:, None], d)
+        return (damp * (f - 0.5 * w_rows.double() * f)).float()
+
+    def softmin(self, eps, log_w, pot, *, damp=1.0, old=None):
+        """damp * softmin(eps, log_w, C, pot) of the new API on the grid, or its average with ``old``; with e = eps / 2
+        the kernel's -e log sum exp(h - |x-y|^2 / (2e)) is half of it, as in ``_Softmin``."""
+        kw = dict(pitch=self.pitch, periodic=self.periodic)
+        if old is None:
+            return ops.softmin_grid_axes_raw(0.5 * eps, log_w, pot, 1.0 / eps, beta=2.0 * damp, **kw)
+        return ops.softmin_grid_axes_raw(0.5 * eps, log_w, pot, 1.0 / eps, out_old=old, alpha_old=0.5, beta=damp, **kw)
+
+
+def _is_real(t):
+    return isinstance(t, (int, float, np.integer, np.floating)) and not isinstance(t, bool)
+
+
+def solve_grid(a, b, cost="sqeuclidean", axes=None, periodic=False, debias=False, reg=None, unbalanced=None,
+               unbalanced_type="KL", method="auto", max_iter=None, tol=None, p=None, blur=None, reach=None):
+    """Entropic (un)balanced OT between B pairs of images or volumes on one regular grid (the new API's
+    ``solve_grid``, a stub in the reference: ot/_implementations/grid.py:215-242).
+
+    a, b: (B, N1[, N2[, N3]]) non-negative float32 CUDA tensors, axis 0 the batch, sides up to 1024.  ``axes``: None
+    ([0, 1) on every axis), one (lo, hi) pair for every axis, or one pair per axis; pixel centres lo + (k + 1/2) h_d
+    with h_d = (hi - lo) / N_d.  ``periodic``: a bool or one per axis.  Conventions of :func:`solve_sample`: cost
+    ``|x - y|^2`` (no 1/2; wrapped around on periodic axes), ``reg`` the temperature, ``unbalanced`` the KL penalty,
+    ``blur`` / ``reach`` shortcuts for ``2 blur^2`` / ``2 reach^2``, the same eps ladder, start and updates.  Element k
+    of the result is ``solve_sample(X, X, a[k].flatten(), b[k].flatten(), ...)`` with X the pixel centres; the softmins
+    run on the separable grid kernel (one launch per axis) and never form a (P, P) matrix.  Returns an
+    :class:`OTResultGrid`; ``value`` is differentiable w.r.t. a and b."""
+    if p is not None and p != 2:
+        raise NotImplementedError(f"solve_grid serves the squared Euclidean cost (p = 2) only. Received p={p}.")
+    if cost != "sqeuclidean":
+        raise NotImplementedError(f"solve_grid serves cost='sqeuclidean' only. Received cost={cost!r}.")
+    if blur is not None:
+        if reg is not None:
+            raise ValueError("Parameters 'reg' and 'blur' are redundant. Please specify only one of them.")
+        reg = 2 * blur**2
+    if reach is not None:
+        if unbalanced is not None:
+            raise ValueError("Parameters 'unbalanced' and 'reach' are redundant. Please specify only one of them.")
+        unbalanced = 2 * reach**2
+    _check_regularization(reg, unbalanced, unbalanced_type, method, tol, max_iter)
+    if not (torch.is_tensor(a) and torch.is_tensor(b)):
+        raise TypeError("a and b must be torch CUDA tensors (this engine has no NumPy / CPU path)")
+    if not 2 <= a.dim() <= 4:
+        raise ValueError(f"Expected a to be a (B, N1[, N2[, N3]]) batch of 1-, 2- or 3-D grids. Received "
+                         f"{tuple(a.shape)}.")
+    if any(n > ops.GRID_MAX_SIDE for n in a.shape[1:]) or a.numel() == 0:
+        raise ValueError(f"solve_grid serves non-empty grids with sides up to {ops.GRID_MAX_SIDE}. Received "
+                         f"{tuple(a.shape)}.")
+    a = _check_marginal(a, a, None, "a")
+    b = _check_marginal(b, a, None, "b")
+    geo = _Grid(a.shape[1:], axes, periodic)
+    dims = tuple(range(1, a.dim()))
+    if unbalanced is None:
+        _check_masses(a.detach().sum(dims), b.detach().sum(dims))
+    for t, name in ((a, "a"), (b, "b")):
+        if not (t.is_cuda and t.dtype == torch.float32):
+            raise TypeError(f"{name} must be a float32 CUDA tensor (this engine computes in fp32 on the GPU), got "
+                            f"{t.dtype} on {t.device}")
+    reg = float(reg)
+    rho = None if unbalanced is None else float(unbalanced)
+
+    def damp(eps):
+        return 1.0 if rho is None else 1.0 / (1.0 + eps / rho)
+
+    with torch.no_grad():
+        a_d, b_d = a.detach().contiguous(), b.detach().contiguous()
+        eps_list = annealing_eps(geo.diameter ** 2, reg, int(max_iter))
+        log_a, log_b = log_weights(a_d), log_weights(b_d)
+        sm = geo.softmin
+        lam = damp(eps_list[0])
+        f_ba, g_ab = geo.at_infinity(a_d, b_d, lam), geo.at_infinity(b_d, a_d, lam)
+        if debias:
+            f_aa, g_bb = geo.at_infinity(a_d, a_d, lam), geo.at_infinity(b_d, b_d, lam)
+        for eps in eps_list:
+            lam = damp(eps)
+            ft_ba = sm(eps, log_b, g_ab, damp=lam, old=f_ba)
+            gt_ab = sm(eps, log_a, f_ba, damp=lam, old=g_ab)
+            if debias:
+                f_aa = sm(eps, log_a, f_aa, damp=lam, old=f_aa)
+                g_bb = sm(eps, log_b, g_bb, damp=lam, old=g_bb)
+            f_ba, g_ab = ft_ba, gt_ab
+        # last, non-averaged update (last_extrapolation=True, sinkhorn_ot.py:419-436)
+        f_ba, g_ab = sm(eps, log_b, g_ab, damp=lam), sm(eps, log_a, f_ba, damp=lam)
+        if debias:
+            f_aa, g_bb = sm(eps, log_a, f_aa, damp=lam), sm(eps, log_b, g_bb, damp=lam)
+    if not debias:
+        f_aa = g_bb = None
+    return OTResultGrid(a=a, b=b, grid=geo, reg=reg, unbalanced=rho, potentials=(f_aa, g_bb, g_ab, f_ba))
+
+
+class OTResultGrid(OTResultSample):
+    """Result of :func:`solve_grid`, with the attributes of :class:`OTResultSample` shaped like the grids:
+    ``potential_a/b/aa/bb`` and ``marginal_a/b`` (B, *grid), ``value`` (B,), ``a_to_b`` / ``b_to_a`` (B, *grid, D)
+    displacement fields, ``plan_operator`` / ``density_operator`` from ``b.shape`` to ``a.shape`` with trailing channels
+    (and ``.T``), dense ``plan`` / ``density`` (B, P, P) for small grids only.
+
+    Every operator application is ONE ``b200ot_grid_plan_apply`` call (``ops.grid_plan_apply_raw``: the normalised
+    weights of each row applied to all the channels), then the row factor ``w_i exp((f_i - sm_i) / reg)``, whose
+    softmin sm comes from the same call; it is differentiable w.r.t. its input through the transposed operator."""
+
+    def __init__(self, *, a, b, grid, reg, unbalanced, potentials):
+        super().__init__(X_a=None, X_b=None, a=a, b=b, reg=reg, unbalanced=unbalanced, debias=potentials[0] is not None,
+                         potentials=potentials, softmin=None)
+        self._grid = grid
+
+    @cached_property
+    def value(self):
+        B = self._a.shape[0]
+        a, b, f_aa, g_bb, g_ab, f_ba = (None if t is None else t.reshape(B, -1) for t in self._live)
+        return _ot_value(a, b, f_ba, g_ab, self._reg, self._unbalanced, f_aa, g_bb)
+
+    def _weights(self, transpose):
+        """(f, g, w_rows, w_cols) of the operator's direction."""
+        if transpose:
+            return self._g_ab, self._f_ba, self._b, self._a
+        return self._f_ba, self._g_ab, self._a, self._b
+
+    def _apply_state(self, transpose, weighted):
+        """(None, None, row factor): w_rows exp((f - sm) / reg), sm the softmin of log w_cols + g / reg (the marginal
+        when ``weighted``), cached until ``cache_clear``."""
+        cache = self.__dict__.setdefault("_apply_cache", {})
+        key = (bool(transpose), bool(weighted))
+        if key not in cache:
+            f, g, w_rows, w_cols = self._weights(transpose)
+            with torch.no_grad():
+                log_w = log_weights(w_cols) if weighted else torch.zeros_like(w_cols)
+                factor = torch.exp((f - self._grid.softmin(self._reg, log_w, g)) / self._reg)
+                cache[key] = (None, None, (w_rows * factor if weighted else factor).contiguous())
+        return cache[key]
+
+    def _apply(self, s, transpose, weighted, *, normalized=False):
+        """plan @ s (weighted) or density @ s for s of shape (B, *grid, K) [``.T @ s`` with ``transpose``];
+        ``normalized``: rows of weights summing to one (no row factor).  Detached."""
+        f, g, w_rows, w_cols = self._weights(transpose)
+        eps, geo = self._reg, self._grid
+        with torch.no_grad():
+            log_w = log_weights(w_cols) if weighted else torch.zeros_like(w_cols)
+            v = s.detach().float().movedim(-1, 0).contiguous()
+            ell, out = ops.grid_plan_apply_raw(0.5 * eps, log_w, g, 1.0 / eps, v, pitch=geo.pitch,
+                                               periodic=geo.periodic)
+            out = out.movedim(0, -1)
+            if normalized:
+                return out
+            factor = torch.exp((f - (-eps * math.log(2.0)) * ell) / eps)  # sm = -eps ln2 ell, new-API scale
+            return ((w_rows * factor) if weighted else factor)[..., None] * out
+
+    def _density_matmat(self, s, transpose, weighted=False):
+        if torch.is_grad_enabled() and s.requires_grad:
+            return _PlanApply.apply(self, s, transpose, weighted)
+        return self._apply(s, transpose, weighted)
+
+    def _operator(self, weighted):
+        shape = tuple(self._a.shape)
+        return LinearOperator(matmat=lambda s: self._density_matmat(s, False, weighted),
+                              rmatmat=lambda s: self._density_matmat(s, True, weighted), input_shape=shape,
+                              output_shape=shape)
+
+    def _barycentric(self, transpose):
+        geo, dev = self._grid, self._a.device
+        B = self._a.shape[0]
+        cs = torch.meshgrid(*[geo.coords(d, dev) for d in range(geo.D)], indexing="ij")
+        x = torch.stack(cs, -1).float().expand((B,) + geo.sides + (geo.D,))  # centred pixel coordinates
+        return self._apply(x, transpose, True, normalized=True) - x
+
+    @cached_property
+    def a_to_b(self):
+        """(B, *grid, D): sum_j P_ij y_j / sum_j P_ij - x_i (also defined for unbalanced problems); detached."""
+        return self._barycentric(False)
+
+    @cached_property
+    def b_to_a(self):
+        """(B, *grid, D): the same on the transposed plan; detached."""
+        return self._barycentric(True)
+
+    @cached_property
+    def density(self):
+        B, P = self._a.shape[0], self._a[0].numel()
+        if B * P * P > _DENSE_LIMIT:
+            raise MemoryError(f"a dense ({B}, {P}, {P}) density does not fit the budget of this accessor; use "
+                              "density_operator / plan_operator, which never build the matrix")
+        C = self._grid.cost(self._a.device).float()
+        f, g = self._f_ba.reshape(B, P), self._g_ab.reshape(B, P)
+        return torch.exp((f[:, :, None] + g[:, None, :] - C) / self._reg)
+
+    @cached_property
+    def plan(self):
+        B = self._a.shape[0]
+        return self.density * self._a.reshape(B, -1, 1) * self._b.reshape(B, 1, -1)

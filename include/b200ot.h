@@ -564,6 +564,26 @@ B200OT_API int b200ot_softmin_grid(const float* h_a, const float* h_b, float h_s
                                    float alpha_old, float beta, float* out, int64_t batch, int32_t N, int32_t dim,
                                    int32_t p, float eps, void* stream);
 
+/* The same softmin (p = 2 only) on a (batch, sides[0][, sides[1][, sides[2]]]) grid with its own geometry per axis:
+ * side sides[d] in 1..1024, pixel pitch pitch[d] > 0, and periodic[d] != 0 for an axis that wraps around (offsets n
+ * become min(|n|, N_d - |n|)); `periodic` may be NULL (no periodic axis).  The three arrays are host memory, dim long.
+ *   out <- alpha_old * out_old + beta * ( -eps * LSE_j ( h_j - |x_i - y_j|^2 / (2 eps) ) ),  x = (k + 1/2) pitch.
+ * `out` must not overlap an input.  One launch per axis. */
+B200OT_API int b200ot_softmin_grid_axes(const float* h_a, const float* h_b, float h_scale_b, const float* out_old,
+                                        float alpha_old, float beta, float* out, int64_t batch, int32_t dim,
+                                        const int32_t* sides, const float* pitch, const int32_t* periodic, float eps,
+                                        void* stream);
+
+/* The plan of that softmin applied to K value channels, w_ij = exp(h_j - |x_i - y_j|^2 / (2 eps)) on the same geometry:
+ *   ell_i = log2 sum_j w_ij           (so -eps ln2 ell is b200ot_softmin_grid_axes of h with beta = 1),
+ *   s_ki  = sum_j w_ij v_kj / sum_j w_ij,      0 where every w_ij is 0 (ell = -inf).
+ * h = h_a + h_scale_b h_b (h_b nullable), (batch, *grid); v and s are channel-major, (K, batch, *grid).  Outputs must
+ * not overlap an input or each other (the passes run in place on them).  One launch per axis and per slab of 4
+ * channels; no scratch. */
+B200OT_API int b200ot_grid_plan_apply(const float* h_a, const float* h_b, float h_scale_b, const float* v, float* ell,
+                                      float* s, int64_t batch, int32_t K, int32_t dim, const int32_t* sides,
+                                      const float* pitch, const int32_t* periodic, float eps, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Pipe-ceiling micro-benchmarks (used by bench.py to measure the MUFU / FP32 roofline of the
  * device it runs on; each launches one kernel doing `iters` dependent steps per thread and

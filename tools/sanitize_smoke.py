@@ -244,6 +244,15 @@ if "grid" in which:
         out = softmin_grid(0.01, 2, h.to(DEV))
         assert torch.isfinite(out).all()
         print("grid", shape, "ok")
+    # per-axis geometry and the plan applied to K channels: unequal sides, a periodic axis, the 32-, 16- and 8-line
+    # tiles of the apply kernel and a partial second slab of channels
+    for shape, K in (((2, 33, 7), 5), ((1, 1024), 1), ((1, 1024), 4), ((1, 9, 16, 5), 2)):
+        h = torch.randn(*shape, generator=g).to(DEV)
+        geo = dict(pitch=[1.0 / n for n in shape[1:]], periodic=[d == 0 for d in range(len(shape) - 1)])
+        out = ops.softmin_grid_axes_raw(0.01, h, **geo)
+        ell, s = ops.grid_plan_apply_raw(0.01, h, None, 0.0, torch.randn((K,) + shape, generator=g).to(DEV), **geo)
+        assert torch.isfinite(out).all() and torch.isfinite(ell).all() and torch.isfinite(s).all()
+        print("grid axes / plan apply", shape, K, "ok")
 if "loss" in which:
     x, y = torch.rand(3, 300, 3, generator=g).to(DEV), torch.rand(3, 200, 3, generator=g).to(DEV)
     v = SamplesLoss("sinkhorn", blur=0.1)(x.requires_grad_(True), y)
