@@ -33,6 +33,9 @@ _SIGNATURES = {
     "b200ot_softmin_fwd_pair": (c_int32, [_P, _P, _P, _P, c_float, _P, c_float, c_float, _P, _P, _P, _P, c_float, _P,
                                           c_float, c_float, _P, _P, _P, c_int64, c_int64, c_int32, c_int32, c_float,
                                           _P, c_int64, _P]),
+    "b200ot_softmin_step_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32]),
+    "b200ot_softmin_fwd_step": (c_int32, [_P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32, c_float, _P, c_int64,
+                                          _P]),
     "b200ot_softmin_bwd_x": (c_int32, [_P, _P, _P, _P, c_float, _P, _P, _P, _P, c_int64, c_int64, c_int32, c_int32,
                                        c_float, _P, c_int64, _P]),
     "b200ot_plan_apply_scratch_bytes": (c_int64, [c_int64, c_int64, c_int32, c_int64]),
@@ -134,6 +137,12 @@ _SIGNATURES = {
                                          c_float, _P]),
     "b200ot_ubench": (c_int32, [c_int32, c_int32, c_int32, _P, ctypes.POINTER(c_int32), _P]),
 }
+
+
+class SoftminSlot(ctypes.Structure):
+    """``b200ot_softmin_slot`` of include/b200ot.h: one softmin of a b200ot_softmin_fwd_step group."""
+    _fields_ = [("h_a", _P), ("h_b", _P), ("h_scale_b", c_float), ("out_old", _P), ("alpha_old", c_float),
+                ("beta", c_float), ("out", _P), ("lse2", _P)]
 
 
 class DenseRows(ctypes.Structure):

@@ -217,10 +217,8 @@ static int finalize_launch(const float2* part, int n_part, const SoftminOut& o, 
   return B200OT_OK;
 }
 
-// 8 rows per thread; the paired kernel fits 4 CTAs/SM in 96 registers, the symmetric one (its column and row-only
-// blocks in one body) needs 3 to stay free of spills
+// 8 rows per thread, 4 CTAs/SM in 96 registers
 using PairC = PairCfg<8, 128, 4>;
-using SymC = PairCfg<8, 128, 3>;
 
 // $B200OT_PAIR=0 (read on every call): every softmin takes the unpaired path, for A/B runs and tests
 static bool pair_on() {
@@ -251,16 +249,38 @@ static int64_t unpaired_bytes(int64_t N, int64_t M) {
          round_up64((int64_t)make_plan(N, M, 3).n_split * N * 16, 256);
 }
 static int64_t packed_bytes(int64_t n) { return round_up64(b200ot_packed_cols_floats(n, 3, 1) * 4, 256); }
-// Scratch: the two range flags, then the region the paired pass uses and the recomputation reuses
+// One softmin of a paired launch group: rows (nr points) against columns (nc points, column potential
+// h_a + h_s * h_b), with its epilogue
+struct PairedSoftmin {
+  const float* rows;
+  const float* cols;
+  int64_t nr, nc;
+  const float *h_a, *h_b;
+  float h_s;
+  SoftminOut o;
+};
+// Scratch: the range flags (one per softmin), then the region the paired pass uses and the recomputation reuses: each
+// softmin's packed columns, then each softmin's partials
 constexpr int64_t kPairFlagBytes = 256;
-static int64_t pair_bytes(int64_t N, int64_t M) {
-  const int64_t paired = packed_bytes(M) + packed_bytes(N) + round_up64((int64_t)pair_blocks(M) * N * 8, 256) +
-                         round_up64((int64_t)pair_blocks(N) * M * 8, 256);
-  return kPairFlagBytes + std::max(paired, std::max(unpaired_bytes(N, M), unpaired_bytes(M, N)));
+static int64_t paired_bytes(const int64_t (*shape)[2], int n) {
+  int64_t paired = 0, unpaired = 0;
+  for (int k = 0; k < n; ++k) {
+    paired += packed_bytes(shape[k][1]) + round_up64((int64_t)pair_blocks(shape[k][1]) * shape[k][0] * 8, 256);
+    unpaired = std::max(unpaired, unpaired_bytes(shape[k][0], shape[k][1]));
+  }
+  return kPairFlagBytes + std::max(paired, unpaired);
 }
 static int64_t sym_bytes(int64_t N) {
-  const int64_t paired = packed_bytes(N) + round_up64((int64_t)pair_blocks(N) * N * 8, 256);
-  return kPairFlagBytes + std::max(paired, unpaired_bytes(N, N));
+  const int64_t shape[1][2] = {{N, N}};
+  return paired_bytes(shape, 1);
+}
+static int64_t pair_bytes(int64_t N, int64_t M) {
+  const int64_t shape[2][2] = {{N, M}, {M, N}};
+  return paired_bytes(shape, 2);
+}
+static int64_t step_bytes(int64_t N, int64_t M) {
+  const int64_t shape[4][2] = {{N, M}, {M, N}, {N, N}, {M, M}};
+  return paired_bytes(shape, 4);
 }
 
 static bool overlaps(const void* a, int64_t na, const void* b, int64_t nb) {
@@ -268,10 +288,22 @@ static bool overlaps(const void* a, int64_t na, const void* b, int64_t nb) {
   const char *pa = (const char*)a, *pb = (const char*)b;
   return pa < pb + nb * 4 && pb < pa + na * 4;
 }
-// an output of a softmin of N rows (columns: M points, column potential h_a, h_b) overlaps one of its inputs
-static bool out_aliases(const SoftminOut& o, int64_t N, const void* const* ins, const int64_t* lens, int nin) {
-  for (int k = 0; k < nin; ++k)
-    if (overlaps(o.out, N, ins[k], lens[k]) || overlaps(o.lse2, N, ins[k], lens[k])) return true;
+// An output of the group s[0..n) overlaps an input of the group or another output: the recomputation of a softmin
+// reads every input after the finalizes wrote the outputs
+static bool paired_aliased(const PairedSoftmin* s, int n, const float* center) {
+  for (int a = 0; a < n; ++a)
+    for (int fa = 0; fa < 2; ++fa) {
+      const float* o = fa ? s[a].o.lse2 : s[a].o.out;
+      if (overlaps(o, s[a].nr, center, 3)) return true;
+      for (int b = 0; b < n; ++b) {
+        const void* ins[] = {s[b].rows, s[b].cols, s[b].h_a, s[b].h_b, s[b].o.out_old};
+        const int64_t lens[] = {s[b].nr * 3, s[b].nc * 3, s[b].nc, s[b].nc, s[b].nr};
+        for (int k = 0; k < 5; ++k)
+          if (overlaps(o, s[a].nr, ins[k], lens[k])) return true;
+        for (int fb = 0; fb < 2; ++fb)
+          if ((a != b || fa != fb) && overlaps(o, s[a].nr, fb ? s[b].o.lse2 : s[b].o.out, s[b].nr)) return true;
+      }
+    }
   return false;
 }
 
@@ -294,45 +326,89 @@ static int softmin_fwd_gated(const float* x, const float* y, const float* h_a, c
   return finalize_launch<kFinGated>(reinterpret_cast<const float2*>(part), pl.n_split, o, N, eps, gate, 0.0, st);
 }
 
-// Softmin A (rows x, columns y, column potential hy) and, unless sym, softmin B (rows y, columns x, column potential
-// hx) from one pass; sym: x is y, hx is hy, one softmin.  Then the range check of every sum, and the gated
-// recomputation of a softmin that failed it.  Arguments validated by the caller; scratch >= pair_bytes / sym_bytes.
-static int pair_fwd(bool sym, const float* x, const float* y, const float* hy_a, const float* hy_b, float hy_s,
-                    const float* hx_a, const float* hx_b, float hx_s, const float* center, int64_t N, int64_t M,
-                    float eps, const SoftminOut& oa, const SoftminOut& ob, void* scratch, cudaStream_t st) {
+// One launch of softmin_pair_kernel over 1 to 3 problems: one CTA per item, the items longest first, so the block
+// scheduler hands out the long ones first and one tail ends the launch
+static int pair_launch(const PairProblem* probs, int nprob, cudaStream_t st) {
+  PairLaunch L{};
+  for (int p = 0; p < nprob; ++p) {
+    const PairProblem& P = probs[p];
+    L.prob[p] = P;
+    const int qr = P.ntr / P.nbr, qc = P.ntc / P.nbc;
+    for (int tr = qr + 1; tr >= qr; --tr)
+      for (int tc = qc + 1; tc >= qc; --tc) {
+        const int nr = pair_blocks_of_size(tr, P.ntr, P.nbr), nc = pair_blocks_of_size(tc, P.ntc, P.nbc);
+        // sym: the unordered pairs within one size class, or of one block of each size (as class (q + 1, q))
+        const int count = !P.sym ? nr * nc : tr == tc ? nr * (nr + 1) / 2 : tr > tc ? nr * nc : 0;
+        if (count > 0) L.cls[L.ncls++] = PairClass{p, tr, tc, count};  // start holds the count until the sort
+      }
+  }
+  // longest first (stable: ties keep problem order)
+  std::stable_sort(L.cls, L.cls + L.ncls, [](const PairClass& a, const PairClass& b) { return a.tr * a.tc > b.tr * b.tc; });
+  for (int c = 0; c < L.ncls; ++c) {
+    const int count = L.cls[c].start;
+    L.cls[c].start = L.items;
+    L.items += count;
+  }
+  const auto kern = softmin_pair_kernel<PairC>;
+  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PairC::SMEM_BYTES));
+  kern<<<L.items, PairC::NT + 32, PairC::SMEM_BYTES, st>>>(L);
+  B200OT_CUDA_TRY(cudaGetLastError());
+  return B200OT_OK;
+}
+
+// The softmins s[0..n) as one launch group: n = 1, one symmetric softmin (rows are columns); n = 2, a mirrored pair
+// (s[1] is s[0] with rows and columns swapped); n = 4, that pair and the symmetric softmins of its rows (s[2]) and of
+// its columns (s[3]).  Zero the flags; pack each softmin's columns with its potential; one paired pass; the range
+// check of every sum; then the gated recomputation of each softmin that failed it, after all the checks since it reuses
+// the region.  Arguments validated by the caller; scratch >= paired_bytes of the shapes.
+static int paired_fwd(const PairedSoftmin* s, int n, const float* center, float eps, void* scratch, cudaStream_t st) {
   int* flags = reinterpret_cast<int*>(scratch);
   char* region = reinterpret_cast<char*>(scratch) + kPairFlagBytes;
-  const int nbr = pair_blocks(N), nbc = pair_blocks(M);
-  float* cols = reinterpret_cast<float*>(region);
-  float* rows = sym ? cols : reinterpret_cast<float*>(region + packed_bytes(M));
-  float2* part_a = reinterpret_cast<float2*>(region + packed_bytes(M) + (sym ? 0 : packed_bytes(N)));
-  float2* part_b = sym ? part_a : reinterpret_cast<float2*>(reinterpret_cast<char*>(part_a) +
-                                                              round_up64((int64_t)nbc * N * 8, 256));
-  B200OT_CUDA_TRY(cudaMemsetAsync(flags, 0, 2 * sizeof(int), st));
-  int rc = softmin_pack_impl(y, hy_a, hy_b, hy_s, center, M, 3, 2, eps, cols, st, nullptr);
-  if (rc) return rc;
-  if (!sym) {
-    rc = softmin_pack_impl(x, hx_a, hx_b, hx_s, center, N, 3, 2, eps, rows, st, nullptr);
-    if (rc) return rc;
+  float* pk[4];
+  float2* part[4];
+  char* at = region;
+  for (int k = 0; k < n; ++k) {
+    pk[k] = reinterpret_cast<float*>(at);
+    at += packed_bytes(s[k].nc);
   }
-  const int ntr = (int)ceil_div64(N, PairC::TJ), ntc = (int)ceil_div64(M, PairC::TJ);
-  static_assert(PairC::SMEM_BYTES == SymC::SMEM_BYTES && PairC::NT == SymC::NT, "one launch shape");
-  const auto kern = sym ? softmin_pair_kernel<SymC, true> : softmin_pair_kernel<PairC, false>;
-  B200OT_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PairC::SMEM_BYTES));
-  const unsigned grid = sym ? (unsigned)(nbr * (nbr + 1) / 2) : (unsigned)(nbr * nbc);
-  kern<<<grid, PairC::NT + 32, PairC::SMEM_BYTES, st>>>(rows, cols, part_a, part_b, N, M, ntr, ntc, nbr, nbc);
-  B200OT_CUDA_TRY(cudaGetLastError());
+  for (int k = 0; k < n; ++k) {
+    part[k] = reinterpret_cast<float2*>(at);
+    at += round_up64((int64_t)pair_blocks(s[k].nc) * s[k].nr * 8, 256);
+  }
+  B200OT_CUDA_TRY(cudaMemsetAsync(flags, 0, n * sizeof(int), st));
+  for (int k = 0; k < n; ++k)
+    if (const int rc = softmin_pack_impl(s[k].cols, s[k].h_a, s[k].h_b, s[k].h_s, center, s[k].nc, 3, 2, eps, pk[k], st,
+                                         nullptr))
+      return rc;
+  // a pair reads its rows from the pack of the mirrored softmin, a symmetric softmin from its own
+  const auto problem = [&](int a, int b) {
+    const int64_t N = s[a].nr, M = s[a].nc;
+    const int ntr = (int)ceil_div64(N, PairC::TJ), ntc = (int)ceil_div64(M, PairC::TJ);
+    return PairProblem{pk[b], pk[a], part[a], part[b], N, M, ntr, ntc, pair_blocks(N), pair_blocks(M), a == b};
+  };
+  PairProblem probs[kPairMaxProblems];
+  int np = 0;
+  if (n == 1) {
+    probs[np++] = problem(0, 0);
+  } else {
+    probs[np++] = problem(0, 1);
+    if (n == 4) {
+      probs[np++] = problem(2, 2);
+      probs[np++] = problem(3, 3);
+    }
+  }
+  if (const int rc = pair_launch(probs, np, st)) return rc;
   // a point's merged sum must stay within [count 2^-100, 2^100]: the terms flushed below 2^-126 then weigh less
   // than 2^-26 of it (DESIGN.md §3.1b)
-  rc = finalize_launch<kFinChecked>(part_a, nbc, oa, N, eps, flags, (double)M * 0x1p-100, st);
-  if (rc) return rc;
-  if (!sym) {
-    rc = finalize_launch<kFinChecked>(part_b, nbr, ob, M, eps, flags + 1, (double)N * 0x1p-100, st);
-    if (rc) return rc;
-  }
-  rc = softmin_fwd_gated(x, y, hy_a, hy_b, hy_s, center, N, M, eps, oa, region, flags, st);
-  if (rc || sym) return rc;
-  return softmin_fwd_gated(y, x, hx_a, hx_b, hx_s, center, M, N, eps, ob, region, flags + 1, st);
+  for (int k = 0; k < n; ++k)
+    if (const int rc = finalize_launch<kFinChecked>(part[k], pair_blocks(s[k].nc), s[k].o, s[k].nr, eps, flags + k,
+                                                    (double)s[k].nc * 0x1p-100, st))
+      return rc;
+  for (int k = 0; k < n; ++k)
+    if (const int rc = softmin_fwd_gated(s[k].rows, s[k].cols, s[k].h_a, s[k].h_b, s[k].h_s, center, s[k].nr, s[k].nc,
+                                         eps, s[k].o, region, flags + k, st))
+      return rc;
+  return B200OT_OK;
 }
 
 }  // namespace b200ot
@@ -456,10 +532,8 @@ B200OT_API int b200ot_softmin_fwd(const float* x, const float* y, const float* h
   const SoftminOut o{out_old, alpha_old, beta, out, lse2_out};
   if (x == y && N == M && pair_on() && pair_shape(N, M, D, p)) {
     // one exponential per unordered pair; refused when an output overlaps an input the recomputation would read
-    const void* ins[] = {x, h_a, h_b, center, out_old};
-    const int64_t lens[] = {N * D, N, N, D, N};
-    if (!out_aliases(o, N, ins, lens, 5) && !overlaps(out, N, lse2_out, N))
-      return pair_fwd(true, x, x, h_a, h_b, h_scale_b, h_a, h_b, h_scale_b, center, N, N, eps, o, o, scratch, st);
+    const PairedSoftmin sym{x, x, N, N, h_a, h_b, h_scale_b, o};
+    if (!paired_aliased(&sym, 1, center)) return paired_fwd(&sym, 1, center, eps, scratch, st);
   }
   const ReducePlan pl = make_plan(N, M, D);
   float* cols = reinterpret_cast<float*>(scratch);
@@ -487,18 +561,38 @@ B200OT_API int b200ot_softmin_fwd_pair(const float* x, const float* y, const flo
   if (!x || !y || !hy_a || !hx_a || !scratch || N <= 0 || M <= 0 || !valid_p(p) || !(eps > 0.f) ||
       (!out_a && !lse2_a) || (!out_b && !lse2_b) || !pair_shape(N, M, D, p))
     return B200OT_EINVAL;
-  const SoftminOut oa{out_a_old, alpha_a_old, beta_a, out_a, lse2_a};
-  const SoftminOut ob{out_b_old, alpha_b_old, beta_b, out_b, lse2_b};
-  // the recomputation of a softmin reads every input after the finalize wrote the outputs: no output may overlap one
-  const void* ins[] = {x, y, hy_a, hy_b, hx_a, hx_b, center, out_a_old, out_b_old};
-  const int64_t lens[] = {N * D, M * D, M, M, N, N, D, N, M};
-  if (out_aliases(oa, N, ins, lens, 9) || out_aliases(ob, M, ins, lens, 9) || overlaps(out_a, N, lse2_a, N) ||
-      overlaps(out_b, M, lse2_b, M) || overlaps(out_a, N, out_b, M) || overlaps(out_a, N, lse2_b, M) ||
-      overlaps(lse2_a, N, out_b, M) || overlaps(lse2_a, N, lse2_b, M))
-    return B200OT_EINVAL;
+  const PairedSoftmin s[2] = {{x, y, N, M, hy_a, hy_b, hy_scale_b, {out_a_old, alpha_a_old, beta_a, out_a, lse2_a}},
+                               {y, x, M, N, hx_a, hx_b, hx_scale_b, {out_b_old, alpha_b_old, beta_b, out_b, lse2_b}}};
+  if (paired_aliased(s, 2, center)) return B200OT_EINVAL;
   if (const int rc = scratch_check(scratch, scratch_bytes, pair_bytes(N, M))) return rc;
-  return pair_fwd(false, x, y, hy_a, hy_b, hy_scale_b, hx_a, hx_b, hx_scale_b, center, N, M, eps, oa, ob, scratch,
-                  (cudaStream_t)stream);
+  return paired_fwd(s, 2, center, eps, scratch, (cudaStream_t)stream);
+}
+
+B200OT_API int64_t b200ot_softmin_step_scratch_bytes(int64_t N, int64_t M, int32_t D) {
+  if (N <= 0 || M <= 0 || !pair_shape(N, M, D, 2) || !pair_shape(N, N, D, 2) || !pair_shape(M, M, D, 2)) return 0;
+  return step_bytes(N, M);
+}
+
+B200OT_API int b200ot_softmin_fwd_step(const float* x, const float* y, const b200ot_softmin_slot* slots,
+                                       const float* center, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
+                                       void* scratch, int64_t scratch_bytes, void* stream) {
+  if (!x || !y || !slots || !scratch || N <= 0 || M <= 0 || !valid_p(p) || !(eps > 0.f) ||
+      b200ot_softmin_step_scratch_bytes(N, M, D) == 0 || !pair_shape(N, M, D, p))
+    return B200OT_EINVAL;
+  // xy, yx, xx, yy
+  const float* rows[4] = {x, y, x, y};
+  const float* cols[4] = {y, x, x, y};
+  const int64_t nrows[4] = {N, M, N, M}, ncols[4] = {M, N, N, M};
+  PairedSoftmin s[4];
+  for (int k = 0; k < 4; ++k) {
+    const b200ot_softmin_slot& q = slots[k];
+    if (!q.h_a || (!q.out && !q.lse2)) return B200OT_EINVAL;
+    s[k] = PairedSoftmin{rows[k], cols[k], nrows[k], ncols[k], q.h_a, q.h_b, q.h_scale_b,
+                         {q.out_old, q.alpha_old, q.beta, q.out, q.lse2}};
+  }
+  if (paired_aliased(s, 4, center)) return B200OT_EINVAL;
+  if (const int rc = scratch_check(scratch, scratch_bytes, step_bytes(N, M))) return rc;
+  return paired_fwd(s, 4, center, eps, scratch, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -316,7 +316,8 @@ def softmin_raw(eps, x, y, h_a, h_b=None, h_scale_b=0.0, *, p=2, center=None, ou
 
 
 # Two softmins of one Jacobi iteration that mirror each other (A's rows are B's columns and A's columns B's rows, same
-# eps, p and center) share their exponentials: b200ot_softmin_fwd_pair.  B200OT_PAIR=0, read on every call, runs every
+# eps, p and center) share their exponentials: b200ot_softmin_fwd_pair, or, with the symmetric softmins of both
+# clouds, b200ot_softmin_fwd_step.  B200OT_PAIR=0, read on every call, runs every
 # call on its own (the library's symmetric xx / yy kernel follows the same switch).
 def _same(s, t):
     """The same tensor data: one object, or views such as two ``.detach()`` of one cloud."""
@@ -336,11 +337,17 @@ def _mirrors(a, b):
         return False
     if xa.dim() != 2 or xa.shape[-1] != 3 or ya.dim() != 2 or ya.shape[-1] != 3:
         return False
-    # the recomputation of a softmin whose sums leave the paired range reads every input after the outputs are written
-    ins = [t for args, kw in (a, b) for t in (*args[1:], kw.get("out_old"), kw.get("center")) if torch.is_tensor(t)]
-    outs = [o for o in (ka.get("out"), kb.get("out")) if o is not None]
+    return _disjoint((a, b))
+
+
+def _disjoint(calls):
+    """No output of ``calls`` shares storage with an input of any of them or with another output: the recomputation
+    of a softmin whose sums leave the paired range reads every input after the outputs are written."""
+    ins = [t for args, kw in calls for t in (*args[1:], kw.get("out_old"), kw.get("center")) if torch.is_tensor(t)]
+    outs = [kw["out"] for _, kw in calls if kw.get("out") is not None]
     shared = lambda s, t: s.untyped_storage().data_ptr() == t.untyped_storage().data_ptr()  # noqa: E731
-    return not any(shared(o, t) for o in outs for t in ins) and not (len(outs) == 2 and shared(*outs))
+    return not any(shared(o, t) for o in outs for t in ins) and not any(
+        shared(o, q) for i, o in enumerate(outs) for q in outs[i + 1:])
 
 
 def pair_plan(calls):
@@ -357,6 +364,34 @@ def pair_plan(calls):
             plan.append((i, j))
             used.add(j)
     return plan
+
+
+def _self_call(c, cloud, eps, kw):
+    """Whether the ``softmin_raw`` call ``c`` is the symmetric softmin of ``cloud`` at ``eps``, p = 2 and the center
+    of ``kw``."""
+    (e, rows, cols, *_), kc = c
+    return (_same(rows, cloud) and _same(cols, cloud) and float(e) == float(eps) and kc.get("p", 2) == 2
+            and _same(kc.get("center"), kw.get("center")))
+
+
+def step_plan(calls):
+    """``pair_plan(calls)`` with each pair ``(i, j)`` that has self calls ``k`` on its rows' cloud and ``l`` on its
+    columns' cloud (same eps, p = 2 and center; no output of the four overlapping an input or another output) merged
+    into one step group ``(i, j, k, l)``: the four softmins of a symmetric Jacobi iteration as one launch group
+    (b200ot_softmin_fwd_step).  Groups in the order of their first call."""
+    plan = pair_plan(calls)
+    free = {g[0] for g in plan if len(g) == 1}
+    steps = {}
+    for g in plan:
+        if len(g) == 2:
+            (eps, x, y, *_), kw = calls[g[0]]
+            kx = next((k for k in sorted(free) if _self_call(calls[k], x, eps, kw)), None)
+            ky = next((k for k in sorted(free - {kx}) if _self_call(calls[k], y, eps, kw)), None)
+            if kx is not None and ky is not None and _disjoint([calls[c] for c in (*g, kx, ky)]):
+                steps[g] = (*g, kx, ky)
+                free -= {kx, ky}
+    taken = {c for st in steps.values() for c in st[2:]}
+    return [steps.get(g, g) for g in plan if len(g) == 2 or g[0] not in taken]
 
 
 def _softmin_pair(a, b):
@@ -394,18 +429,63 @@ def _softmin_pair(a, b):
     return (out_a, lse2_a), (out_b, lse2_b)
 
 
+def _softmin_step(cs):
+    """``softmin_raw(*c)`` for the four calls ``cs`` of a step group (xy, yx, xx, yy; ``step_plan``) from one launch
+    group, or None when the library does not run this shape as one."""
+    (eps, x, y, *_), k0 = cs[0]
+    p, center = k0.get("p", 2), k0.get("center")
+    hs = [(args[3], *(list(args[4:]) + [None, 0.0])[:2]) for args, _ in cs]  # h_a, h_b, h_scale_b of each softmin
+    vecs = lambda k: ((hs[k][0], "h_a"), (hs[k][1], "h_b"), (cs[k][1].get("out_old"), "out_old"),  # noqa: E731
+                      (cs[k][1].get("out"), "out"))
+    # on the columns' cloud (M entries): the potentials of xy and yy, the epilogues of yx and yy; the rest on the rows'
+    on_y = ((hs[0][0], "h_a"), (hs[0][1], "h_b"), *vecs(1)[2:], *vecs(3))
+    on_x = ((hs[1][0], "h_a"), (hs[1][1], "h_b"), *vecs(0)[2:], *vecs(2))
+    (_, N, M, D), sizes, (x, y, *ready) = _inputs(_SOFTMIN, p, x, y, on_y, on_x, (center, "center"))
+    ry, rx, center = ready[:8], ready[8:16], ready[16]
+    dev = x.device
+    nbytes = _query(dev, "b200ot_softmin_step_scratch_bytes", *sizes)
+    if nbytes == 0:
+        return None
+    # per softmin: h_a, h_b, out_old, out as checked, and its row count
+    got = [(ry[0], ry[1], rx[2], rx[3], N), (rx[0], rx[1], ry[2], ry[3], M), (rx[4], rx[5], rx[6], rx[7], N),
+           (ry[4], ry[5], ry[6], ry[7], M)]
+    for (*_, o, _), (_, kw) in zip(got, cs):
+        given = kw.get("out")
+        if given is not None and (o is not given or given.device != dev):
+            raise ValueError(f"out must be contiguous and on {dev}, got strides {given.stride()} on {given.device}")
+    with nvtx_range("b200ot.softmin_step N={} M={} D={} eps={:.3g}", N, M, D, float(eps)):
+        slots, res = (_lib.SoftminSlot * 4)(), []
+        for slot, (h_a, h_b, out_old, out, n), (_, h_scale_b), (_, kw) in zip(slots, got, [h[1:] for h in hs], cs):
+            out = torch.empty(n, dtype=torch.float32, device=dev) if out is None else out
+            lse2 = torch.empty(n, dtype=torch.float32, device=dev) if kw.get("want_lse2") else None
+            slot.h_a, slot.h_b, slot.out_old, slot.out, slot.lse2 = (None if t is None else t.data_ptr()
+                                                                     for t in (h_a, h_b, out_old, out, lse2))
+            slot.h_scale_b, slot.alpha_old, slot.beta = float(h_scale_b), float(kw.get("alpha_old", 0.0)), float(
+                kw.get("beta", 1.0))
+            res.append((out, lse2))
+        scratch = _scratch(nbytes, dev, "softmin_pair")
+        # four packs, the paired pass, four checked finalizes, and the gated pack, partial and finalize of each softmin
+        _call(dev, "b200ot_softmin_fwd_step", x, y, slots, center, *sizes, int(p), float(eps), scratch,
+              scratch.numel(), launches=21)
+    return res
+
+
 def softmin_raw_many(calls):
-    """``[softmin_raw(*args, **kw) for args, kw in calls]``, the mirrored calls of ``pair_plan(calls)`` paired."""
+    """``[softmin_raw(*args, **kw) for args, kw in calls]``, the groups of ``step_plan(calls)`` each from one launch
+    group: a step group through b200ot_softmin_fwd_step, a mirrored pair through b200ot_softmin_fwd_pair (also the
+    pair of a step group whose shape the step entry does not serve, its self calls then on their own)."""
     res = [None] * len(calls)
     paired = _os.environ.get("B200OT_PAIR", "1") != "0"
-    for group in (pair_plan(calls) if paired else [(k,) for k in range(len(calls))]):
-        both = _softmin_pair(calls[group[0]], calls[group[1]]) if len(group) == 2 else None
-        if both is not None:
-            res[group[0]], res[group[1]] = both
-        else:
-            for k in group:
-                args, kw = calls[k]
-                res[k] = softmin_raw(*args, **kw)
+    for group in (step_plan(calls) if paired else [(k,) for k in range(len(calls))]):
+        got = _softmin_step([calls[k] for k in group]) if len(group) == 4 else None
+        if got is None and len(group) >= 2:
+            got = _softmin_pair(calls[group[0]], calls[group[1]])
+        got = list(got or ())
+        for k, r in zip(group, got):
+            res[k] = r
+        for k in group[len(got):]:
+            args, kw = calls[k]
+            res[k] = softmin_raw(*args, **kw)
     return res
 
 

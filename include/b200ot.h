@@ -116,6 +116,29 @@ B200OT_API int b200ot_softmin_fwd_pair(const float* x, const float* y, const flo
                                        int32_t D, int32_t p, float eps, void* scratch, int64_t scratch_bytes,
                                        void* stream);
 
+/* One softmin of b200ot_softmin_fwd_step: column potential h_a + h_scale_b * h_b (h_b nullable) and the epilogue of
+ * b200ot_softmin_fwd (out_old and one of out, lse2 nullable). */
+typedef struct {
+  const float* h_a;
+  const float* h_b;
+  float h_scale_b;
+  const float* out_old;
+  float alpha_old, beta;
+  float* out;
+  float* lse2;
+} b200ot_softmin_slot;
+
+/* The four softmins of one symmetric Jacobi Sinkhorn iteration as one launch group: slots[0] rows x, columns y
+ * (out: N); slots[1] rows y, columns x (M); slots[2] rows x, columns x (N); slots[3] rows y, columns y (M).  The xy / yx
+ * pair of b200ot_softmin_fwd_pair and the symmetric xx and yy softmins of b200ot_softmin_fwd run as one launch of the
+ * paired kernel, with the range check and recomputation of both, and give their results bit for bit.  D = 3, p = 2,
+ * and a shape b200ot_softmin_step_scratch_bytes accepts (0 otherwise); no output may overlap an input or another output
+ * (EINVAL).  scratch: >= b200ot_softmin_step_scratch_bytes(N, M, D), the four range flags first. */
+B200OT_API int64_t b200ot_softmin_step_scratch_bytes(int64_t N, int64_t M, int32_t D);
+B200OT_API int b200ot_softmin_fwd_step(const float* x, const float* y, const b200ot_softmin_slot* slots,
+                                       const float* center, int64_t N, int64_t M, int32_t D, int32_t p, float eps,
+                                       void* scratch, int64_t scratch_bytes, void* stream);
+
 /* Gradient of the softmin w.r.t. the row cloud (the only gradient the reference's autograd
  * contract carries: columns and h are detached, sinkhorn_samples.py:179-185, sinkhorn_divergence.py:616-623):
  *   grad_x[i,:] = grad_out[i] * sum_j softmax_j(h_j - C_ij/eps) * dC(x_i, y_j)/dx_i

@@ -88,6 +88,11 @@ if "pair" in which:
     check("pair_xy", fa, ref_softmin(0.05, x, y, hy, 2))
     check("pair_yx", fb, ref_softmin(0.05, y, x, hx, 2))
     check("pair_xx", ops.softmin_raw(0.05, xd, xd, hxd, p=2, center=c)[0], ref_softmin(0.05, x, x, hx, 2))
+    # the step entry: the pair and both symmetric softmins in one launch
+    got = ops.softmin_raw_many([((0.05, xd, yd, hyd), dict(p=2, center=c)), ((0.05, yd, xd, hxd), dict(p=2, center=c)),
+                                ((0.05, xd, xd, hxd), dict(p=2, center=c)), ((0.05, yd, yd, hyd), dict(p=2, center=c))])
+    for name, (o, _), (r, col, h) in zip(("xy", "yx", "xx", "yy"), got, ((x, y, hy), (y, x, hx), (x, x, hx), (y, y, hy))):
+        check(f"step_{name}", o, ref_softmin(0.05, r, col, h, 2))
     del os.environ["B200OT_PAIR_TILES"]
 if "ranges" in which:
     for variant, n, m in ((ranges.SMALL, 900, 700), (ranges.BIG, 2500, 3000)):
